@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """bench.py -- nucleotides/s through HyenaOperator fwd+bwd at L=1,048,576, d_model=256 (BASELINE.json).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W]            # this repo's sm_100a path
+    python bench.py [--gpus N] [--steps K] [--warmup W]            # this repo's sm_90a path
+    python bench.py ... --dump-outputs DIR                         # also write what the last timed step computed
     python bench.py --impl reference [--steps K] [--warmup W]      # the reference's CPU torch.fft path
 
 A "step" is one forward + backward of the operator over one batch of synthetic single-nucleotide
@@ -13,7 +14,7 @@ One JSON line on stdout (rank 0).  Keys beyond the base contract:
   roofline      HBM roofline of the custom-kernel span (SURVEY.md S8(d): (44+16/B)*D bytes per
                 nucleotide fwd+bwd, in_proj output -> out_proj input), achieved = those bytes / the
                 summed CUDA-event time of this library's kernels inside the timed steps; "kernels"
-                lists each kernel class' share so it can be checked against profiles/*launches*.csv
+                lists each kernel class' share, its algorithmic bytes and achieved GB/s
   cpu_baseline  the oracle (CPU restatement of the reference torch.fft path) timed on the host cores
                 on a bounded sample of the same workload
   e2e           same metric through the public module API with HOST (pinned) buffers: u and dy are
@@ -50,8 +51,8 @@ def parse():
     ap.add_argument("--d-model", type=int, default=D_MODEL)
     ap.add_argument("--batch", type=int, default=1, help="samples per GPU")
     ap.add_argument("--cpu-threads", type=int, default=0,
-                    help="host threads for the CPU arm (0 = min(cores, 16): torch CPU ops were ~40x SLOWER with all "
-                         "128 hardware threads of the B200 host than the survey box was with 8)")
+                    help="host threads for the CPU arm (0 = min(cores, 16): torch CPU ops get much slower, not faster, "
+                         "with a hundred-odd threads on a large shared host)")
     ap.add_argument("--cpu-sample-len", type=int, default=1 << 17,
                     help="sequence length of the bounded CPU sample of the product arm's cpu_baseline leg")
     ap.add_argument("--ref-seconds", type=float, default=200.0,
@@ -62,7 +63,42 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--e2e-chunks", type=int, default=4, help="sequence chunks of the HostStep copy pipeline")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (y, du, every parameter "
+                         "gradient) as DIR/<name>.npy, float32; y and du as a fixed seeded sample of DUMP_SAMPLE "
+                         "elements, at most DUMP_BUDGET bytes in all")
     return ap.parse_args()
+
+
+DUMP_SAMPLE = 1 << 22          # elements of y and du written by --dump-outputs (16 MB each)
+DUMP_BUDGET = 60 << 20         # bytes of all --dump-outputs files together
+
+
+def _sample_index(n, k, seed):
+    """k flat indices into n elements, drawn with a fixed seed (the same in every run), sorted; all n when n <= k."""
+    if n <= k:
+        return torch.arange(n)
+    return torch.randint(n, (k,), generator=torch.Generator().manual_seed(seed)).sort().values
+
+
+def dump_outputs(out_dir, y, du, named_grads):
+    """What a caller of the timed path receives from its last step: y, du = dL/du and the parameter gradients, float32.
+    y and du (B*L*D elements each) are reduced to DUMP_SAMPLE elements at fixed seeded flat indices (_sample_index,
+    seed 0); the parameter gradients are written whole while they fit the rest of DUMP_BUDGET, else each one is reduced
+    the same way (seed 1) to an equal share of it, so that the files never exceed the budget."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    idx = _sample_index(y.numel(), DUMP_SAMPLE, 0).to(y.device)
+    for name, t in (("y", y), ("du", du)):
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.detach().reshape(-1)[idx].float().cpu().numpy())
+    left = (DUMP_BUDGET - 2 * 4 * idx.numel()) // 4
+    whole = sum(g.numel() for _, g in named_grads) <= left
+    share = left // max(len(named_grads), 1)
+    for name, g in named_grads:
+        g = g.detach().float()
+        if not whole:
+            g = g.reshape(-1)[_sample_index(g.numel(), share, 1).to(g.device)]
+        np.save(os.path.join(out_dir, f"grad.{name}.npy"), g.cpu().numpy())
 
 
 # ----------------------------------------------------------------------------------------- clocks
@@ -162,8 +198,8 @@ def build_roofline(prof, steps, B, D, L, ms_step):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak_gbs = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s"
+    peak_gbs = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet 3350 GB/s"
     span_bytes = (44.0 + 16.0 / B) * D * B * L               # SURVEY.md S8(d), per step
     # the projections are this library's kernels too now (csrc/proj_gemm.cuh) but sit OUTSIDE the span of S8(d)
     # (in_proj output -> out_proj input): reported on their own, against the tensor-core roofline
@@ -185,22 +221,17 @@ def build_roofline(prof, steps, B, D, L, ms_step):
         kernels[k] = ent
     dominant = next(iter(kernels), None)
     traffic, traffic_src = None, None
-    try:     # DRAM bytes of the same kernels from the committed ncu capture (same shape only)
-        tj = json.load(open(os.path.join(ROOT, "profiles", "span_traffic.json")))
-        if (L, D, B) == (L_FULL, D_MODEL, 1):
-            traffic, traffic_src = tj["span_dram_bytes_per_step"], tj["source"]
-    except Exception:
-        pass
     projections = None
     if proj:
         pms = sum(v[0] for v in proj.values()) / steps
         flops = 3 * 2.0 * B * L * D * (3 * D + D)            # fwd + input grads + weight grads of in_proj and out_proj
-        tf = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 1590.0)))
+        tf = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 989.0)))
         projections = {"ms_per_step": round(pms, 4), "fp32_equivalent_tflops": round(flops / (pms * 1e-3) / 1e12, 1),
                        "tf32_mma_tflops": round(3 * flops / (pms * 1e-3) / 1e12, 1),
                        "peak_tf32_dense_tflops_derived": round(tf / 2, 1),
                        "frac_of_tf32_peak": round(3 * flops / (pms * 1e-3) / 1e12 / (tf / 2), 4),
-                       "note": "3xTF32: three tf32 MMAs per fp32 product; tf32 peak taken as half the measured bf16 peak",
+                       "note": "3xTF32: three tf32 MMAs per fp32 product; tf32 peak taken as half the bf16 peak "
+                               "(MEASURED_PEAKS.json if present, else the H100 SXM data sheet's dense 989 TFLOP/s)",
                        "kernels": {k: {"ms_per_step": round(v[0] / steps, 4), "launches_per_step": v[1] / steps}
                                    for k, v in proj.items()}}
     return {"bound": "hbm", "kernel": "custom-kernel span (in_proj output -> out_proj input), fwd+bwd, per step",
@@ -257,7 +288,7 @@ def workload_config(L, D, B, world):
     return {"workload": f"large-1m: HyenaOperator fwd+bwd, L={L} d_model={D} order=2 filter_order=64 "
                         f"emb_dim={EMB}, batch {B}/GPU (global {world * B}), fp32, TF32 off",
             "parallelism": f"dp{world} (batch-sharded replicas, grad all-reduce)",
-            "l2": "inputs larger than L2 (u, p, dy are 1-3 GB each; 126 MB L2), no explicit flush"}
+            "l2": "inputs larger than L2 (u, p, dy are 1-3 GB each; 50 MB L2), no explicit flush"}
 
 
 def reference_arm(args):
@@ -285,40 +316,17 @@ def reference_arm(args):
 # ----------------------------------------------------------------------------------------- reference GPU path
 def gpu_reference_run(op, u, dy, steps=3, warmup=1):
     """The reference's own GPU path (plain torch ops: F.linear, F.conv1d, torch.fft -> cuFFT; hyena.py:388-444) on the
-    same device, same weights, same inputs, fp32 with TF32 off: the >=10x denominator of north_star.  Imports the
-    UNMODIFIED reference module when /root/reference exists (build container), else runs the oracle restatement of it
-    on cuda (the GPU box has no /root/reference)."""
+    same device, same weights, same inputs, fp32 with TF32 off: the >=10x denominator of north_star.  Runs the oracle
+    restatement of the reference module (oracle/hyena_oracle.py, pinned to the reference by tests/golden)."""
     import gc
-    dev = u.device
+    from oracle import hyena_oracle as O
     sd = {k: v.detach() for k, v in op.state_dict().items()}
     B, L, D = u.shape
-    which = None
-    ref_dir = "/root/reference"
-    mod = None
-    if os.path.isdir(ref_dir):
-        try:
-            sys.path.insert(0, ref_dir)
-            import standalone_hyenadna as S
-            mod = S.HyenaOperator(D, L, order=2, filter_order=64, emb_dim=EMB, w=W_FREQ, lr_pos_emb=0.0,
-                                  modulate=True, shift=0.0).to(dev)
-            mod.load_state_dict(sd, strict=True)
-            which = "unmodified /root/reference/standalone_hyenadna.HyenaOperator on cuda"
-        except Exception as e:      # pragma: no cover
-            mod, which = None, None
-            sys.stderr.write(f"gpu_reference: reference import failed ({e!r}); using the oracle on cuda\n")
-    if mod is None:
-        from oracle import hyena_oracle as O
-        P = O.canonical(sd)
-        which = "oracle restatement (oracle/hyena_oracle.py) of the reference torch.fft path on cuda (cuFFT)"
+    P = O.canonical(sd)
+    which = "oracle restatement (oracle/hyena_oracle.py) of the reference torch.fft path on cuda (cuFFT)"
 
     def one():
-        if mod is not None:
-            uu = u.detach().clone().requires_grad_(True)
-            for p in mod.parameters():
-                p.grad = None
-            mod(uu).backward(dy)
-        else:
-            O.operator_fwd_bwd(u.detach(), P, dy)
+        O.operator_fwd_bwd(u.detach(), P, dy)
 
     try:
         for _ in range(warmup):
@@ -332,7 +340,6 @@ def gpu_reference_run(op, u, dy, steps=3, warmup=1):
         torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / steps
     finally:
-        mod = None
         gc.collect()
         torch.cuda.empty_cache()
     return {"ms_per_step": round(ms, 3), "value": B * L / (ms * 1e-3), "unit": "nt/s", "steps": steps,
@@ -452,11 +459,15 @@ def main():
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     t_begin = sampler.mark()
     e0.record()
+    y_last = None
     for _ in range(args.steps):
-        step()
+        y_last = step()
     e1.record()
     torch.cuda.synchronize()
     t_end = sampler.mark()
+    if args.dump_outputs and rank == 0 and y_last is not None:
+        dump_outputs(args.dump_outputs, y_last, u.grad, [(n, p.grad) for n, p in op.named_parameters()
+                                                           if p.requires_grad and p.grad is not None])
     barrier()
     ms = e0.elapsed_time(e1)
     prof = H._lib.profile_end()

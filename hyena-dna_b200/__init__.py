@@ -1,4 +1,4 @@
-"""hyena_b200 -- Blackwell-native (sm_100a) Hyena long-convolution operator.
+"""hyena_b200 -- Hopper-native (sm_90a) Hyena long-convolution operator.
 
 Drop-in for the HyenaOperator / HyenaFilter / fftconv surface of HazyResearch/hyena-dna
 (src/models/sequence/hyena.py, src/ops/fftconv.py, csrc/fftconv).  Import as ``hyena_dna_b200``.

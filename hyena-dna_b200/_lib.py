@@ -46,7 +46,6 @@ SIGNATURES = {
     "hyena_b200_fftconv_bwd": (_i, [c_fp] * 7 + [_i, _i, _i, _vp, _sz, _vp]),
     "hyena_b200_gemm_available": (_i, []),
     "hyena_b200_proj_wimg_bytes": (_sz, [_i, _i]),
-    "hyena_b200_proj_debug_buffer": (_i, [_vp]),
     "hyena_b200_proj_wgrad_scratch_bytes": (_sz, [_i, _i]),
     "hyena_b200_proj_wgrad": (_i, [c_fp, c_fp, c_fp, c_fp, _i, _f, _i, _i, _i, _i, _vp, _sz, _vp]),
     "hyena_b200_proj_gemm": (_i, [c_fp, _i, c_fp, _i, _i, c_fp, c_fp, c_fp, _i, _i, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
@@ -66,7 +65,7 @@ class HyenaB200Error(RuntimeError):
 
 
 def build(verbose=False):
-    """Compile csrc/*.cu for sm_100a into libhyena_b200.so (nvcc cross-compiles without a GPU)."""
+    """Compile csrc/*.cu for sm_90a into libhyena_b200.so (nvcc cross-compiles without a GPU)."""
     jobs = str(min(8, os.cpu_count() or 1))
     out = subprocess.run(["make", "-C", CSRC, "-j", jobs], capture_output=True, text=True)
     if verbose or out.returncode != 0:
@@ -91,7 +90,7 @@ def lib():
                 for name, (res, args) in SIGNATURES.items():
                     fn = getattr(L, name)
                     fn.restype, fn.argtypes = res, args
-                if L.hyena_b200_abi_version() != 1:
+                if L.hyena_b200_abi_version() != 2:
                     raise HyenaB200Error("libhyena_b200.so ABI version mismatch")
                 _lib = L
     return _lib

@@ -6,7 +6,7 @@ threads (hidden_states, residual) through the blocks and applies the same dropou
 end): same constructor keywords, attribute names (mixer, norm1, mlp, norm2, dropout1/2) and state_dict keys, so a
 reference checkpoint's ``backbone.layers.N.*`` entries load unchanged.
 
-The dropout -> add -> LayerNorm step runs as ONE sm_100a kernel (csrc/layernorm.cuh) in fp32 -- the residual stream is
+The dropout -> add -> LayerNorm step runs as ONE sm_90a kernel (csrc/layernorm.cuh) in fp32 -- the residual stream is
 kept in fp32 whatever the activation dtype, i.e. residual_in_fp32 semantics.  Dropout / stochastic depth with p > 0,
 post-norm blocks and RMSNorm are outside the hot path and raise; there is no CPU fallback.
 """
@@ -27,7 +27,7 @@ class Block(nn.Module):
                "sequence_parallel": sequence_parallel, "mixer_cls": mixer_cls is None}
         bad = [k for k, v in bad.items() if v]
         if bad:
-            raise HyenaB200Error(f"Block options outside the sm_100a hot path (no fallback): {bad}")
+            raise HyenaB200Error(f"Block options outside the sm_90a hot path (no fallback): {bad}")
         self.prenorm = prenorm
         self.fused_dropout_add_ln = fused_dropout_add_ln      # accepted for config compatibility: the fused kernel always runs
         self.return_residual = return_residual
@@ -49,7 +49,7 @@ class Block(nn.Module):
     @staticmethod
     def _add_norm(hidden_states, residual, norm):
         if not hidden_states.is_cuda:
-            raise HyenaB200Error("Block (hyena_b200) runs on CUDA sm_100a only; there is no CPU fallback")
+            raise HyenaB200Error("Block (hyena_b200) runs on CUDA sm_90a only; there is no CPU fallback")
         x = hidden_states.to(torch.float32).contiguous()
         r = residual.to(torch.float32).contiguous() if residual is not None else None
         return ops.add_layer_norm(x, r, norm.weight.to(torch.float32), norm.bias.to(torch.float32) if norm.bias is not None

@@ -14,7 +14,6 @@
 
 namespace hy {
 
-extern long long* g_proj_dbg;          // k_proj.cu
 static thread_local char g_err[512] = "";
 static std::atomic<unsigned long long> g_launches{0};
 
@@ -104,15 +103,13 @@ static int log_m_for(int L) {         // M = 2^logM >= max(L, 1024)
   while (((size_t)1 << lg) < (size_t)L) ++lg;
   return lg;
 }
-// Row length: 1024 points, one warp per row.  (A 4096-point variant existed in round 1 and lost: 43.85 vs 39.10 ms per
-// step at L = 2^20, profiles/r1_config_sweep.txt; removed.)
+// Row length: 1024 points, one warp per row.
 static int pick_log_m2(int) { return 10; }
 static size_t row_bytes(int L) { return ((size_t)1 << log_m_for(L)) * sizeof(float2); }
 
 static size_t group_budget_bytes() {
-  // scratch rows in flight per launch group.  Measured on B200 (profiles/r1_config_sweep.txt, two sweeps): with
-  // separate kernels per pass the scratch does not survive in L2 anyway, and many waves per launch win, so the
-  // default lets a whole (B=1, D=256, L=2^20) operator go in one launch per pass
+  // scratch rows in flight per launch group: with separate kernels per pass the scratch does not survive in L2 anyway,
+  // and many waves per launch win, so the default lets a whole (B=1, D=256, L=2^20) operator go in one launch per pass
   static size_t v = 0;
   if (!v) {
     const char* e = getenv("HYENA_B200_GROUP_MB");
@@ -159,7 +156,7 @@ static int carve(void* ws, size_t ws_bytes, int B, int D, int L, bool backward, 
 // ---------------------------------------------------------------- pipelined row groups (L2-resident scratch)
 // The three passes of a row group are enqueued back to back on one of S auxiliary streams, group g on stream g % S with
 // scratch slot g % S, G channels per group: the inter-pass scratch of a group (G x B x 8 MB at M = 2^20) is re-read while
-// it is still in the 126 MB L2, a slot is overwritten in place by the next group of its stream (dirty lines never
+// it is still in the 50 MB L2, a slot is overwritten in place by the next group of its stream (dirty lines never
 // have to reach DRAM), and kernels of different groups overlap so that the short launches leave no idle tails.
 // In-stream order carries every dependency (passes of a group, reuse of a slot); the caller's stream forks into the
 // auxiliary streams and joins them again, so to the caller the call is ordered on its own stream as before.
@@ -309,7 +306,7 @@ HY_API size_t hyena_b200_workspace_bytes(int B, int D, int L, int backward) {
 
 // tensor-core filter path: scratch for the tf32 hi/lo weight images (~0.3 MB, grow-only), one per (device, stream): two
 // operators driven from different streams never share it (the prep kernel of one would overwrite the images the other's
-// tcgen05 kernel is still reading)
+// wgmma kernel is still reading)
 static int get_wimg(int D, cudaStream_t stream, float** out) {
   int dev = -1;
   HY_CUDA(cudaGetDevice(&dev));
@@ -589,7 +586,7 @@ HY_API int hyena_b200_core_bwd(const float* dy_pre, const float* p, const float*
   return 0;
 }
 
-/* OUT[pos][n] = sum_k ACT[pos][k] W'[n][k] (+ bias[n]) on tcgen05, fp32 accuracy (3xTF32); see include/hyena_b200.h */
+/* OUT[pos][n] = sum_k ACT[pos][k] W'[n][k] (+ bias[n]) on wgmma, fp32 accuracy (3xTF32); see include/hyena_b200.h */
 HY_API size_t hyena_b200_proj_wimg_bytes(int N, int K) { return (N < 1 || K < 1) ? 0 : proj_wimg_bytes(N, K); }
 
 HY_API int hyena_b200_proj_gemm(const float* act, int act_layout, const float* W, int ldw, int w_transposed,
@@ -608,9 +605,6 @@ HY_API int hyena_b200_proj_gemm(const float* act, int act_layout, const float* W
                            reinterpret_cast<float*>(wimg), (cudaStream_t)stream));
   return 0;
 }
-
-/* debug: device buffer of >= 16 long longs receiving the per-role barrier-wait cycle counters of CTA 0 (NULL: off) */
-HY_API int hyena_b200_proj_debug_buffer(void* buf) { hy::g_proj_dbg = reinterpret_cast<long long*>(buf); return 0; }
 
 HY_API size_t hyena_b200_proj_wgrad_scratch_bytes(int M, int N) { return (M < 1 || N < 1) ? 0 : proj_wgrad_scratch_bytes(M, N); }
 

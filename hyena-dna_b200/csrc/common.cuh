@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a Hyena long-convolution kernels.
+// Shared helpers for the sm_90a Hyena long-convolution kernels.
 //
 // Nothing in this directory includes torch headers: the library is a plain C-ABI
 // shared object (include/hyena_b200.h) and PyTorch only hands it device pointers.
@@ -10,47 +10,23 @@
 namespace hy {
 
 // ---------------------------------------------------------------- complex helpers
-// A complex value is one 64-bit register pair and every helper below is written on the sm_100 packed fp32
-// instructions (add/mul/fma.rn.f32x2 -> SASS FADD2 / FMUL2 / FFMA2): a complex add is ONE instruction and a
-// complex multiply TWO.  Lane swaps and sign flips of an operand ((y, x), (-x, y), ...) are operand modifiers of
-// the packed instructions (.F32x2.LO_HI, .NP), so multiplications by +-i and conjugates stay free.
-// Rounding is identical to the scalar forms fmaf(a.x, b.x, -(a.y * b.y)) etc.
-// HY_SCALAR_COMPLEX (per translation unit) selects the scalar forms instead: measured on B200 (profiles/r2_packed_ab.txt)
-// the packed forms help the column passes (issue-slot bound: loads, stores and integer address math share the port with
-// the butterflies) and hurt the row passes (fp32-pipe bound: FADD2/FFMA2 issue at half rate, same lane throughput, and
-// the register-pair constraints cost MOVs there).
-#ifndef HY_SCALAR_COMPLEX
-__device__ __forceinline__ float2 cadd(float2 a, float2 b) { return __fadd2_rn(a, b); }
-__device__ __forceinline__ float2 csub(float2 a, float2 b) { return __fadd2_rn(a, make_float2(-b.x, -b.y)); }
-__device__ __forceinline__ float2 cmul(float2 a, float2 b) {
-  return __ffma2_rn(make_float2(a.x, a.x), b, __fmul2_rn(make_float2(a.y, a.y), make_float2(-b.y, b.x)));
-}
-// a * conj(b)
-__device__ __forceinline__ float2 cmulc(float2 a, float2 b) {
-  return __ffma2_rn(make_float2(b.x, b.x), a, __fmul2_rn(make_float2(b.y, b.y), make_float2(a.y, -a.x)));
-}
-// a * (c - i s) with compile-time friendly real constants c, s
-__device__ __forceinline__ float2 cmul_cs(float2 a, float c, float s) {
-  return __ffma2_rn(a, make_float2(c, c), __fmul2_rn(make_float2(a.y, a.x), make_float2(s, -s)));
-}
-// elementwise (not complex) product / fma of two sample pairs
-__device__ __forceinline__ float2 pmul(float2 a, float2 b) { return __fmul2_rn(a, b); }
-__device__ __forceinline__ float2 pfma(float2 a, float2 b, float2 c) { return __ffma2_rn(a, b, c); }
-#else
+// A complex value is one float2; a complex multiply is two FMAs and two multiplies.
 __device__ __forceinline__ float2 cadd(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
 __device__ __forceinline__ float2 csub(float2 a, float2 b) { return make_float2(a.x - b.x, a.y - b.y); }
 __device__ __forceinline__ float2 cmul(float2 a, float2 b) {
   return make_float2(fmaf(a.x, b.x, -a.y * b.y), fmaf(a.x, b.y, a.y * b.x));
 }
+// a * conj(b)
 __device__ __forceinline__ float2 cmulc(float2 a, float2 b) {
   return make_float2(fmaf(a.x, b.x, a.y * b.y), fmaf(a.y, b.x, -a.x * b.y));
 }
+// a * (c - i s) with compile-time friendly real constants c, s
 __device__ __forceinline__ float2 cmul_cs(float2 a, float c, float s) {
   return make_float2(fmaf(a.x, c, a.y * s), fmaf(a.y, c, -a.x * s));
 }
+// elementwise (not complex) product / fma of two sample pairs
 __device__ __forceinline__ float2 pmul(float2 a, float2 b) { return make_float2(a.x * b.x, a.y * b.y); }
 __device__ __forceinline__ float2 pfma(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
-#endif
 __device__ __forceinline__ float2 cconj(float2 a) { return make_float2(a.x, -a.y); }
 // -i * a
 __device__ __forceinline__ float2 cmul_negi(float2 a) { return make_float2(a.y, -a.x); }

@@ -899,7 +899,7 @@ __device__ __forceinline__ void row_pass_body(const PassArgs& a, const int bx, c
 // (issued before the forward row FFT / before the first inverse FFT, so the 2 x 64 dependent __ldg's per thread of the
 // two pointwise phases -- `long_scoreboard`, the top stall of the kernel -- become shared-memory reads).  One 8 KB
 // buffer per row, reused for k then g; the partner row's buffer supplies the mirrored bins.  Shared memory per CTA:
-// rows * (EX + 2 * M2) complex = 99 KB for four rows, two CTAs per SM.  Default for batch 1 (2.75 vs 3.51 ms at large-1m, profiles/r2_ab.txt); HYENA_B200_ROW_BWD1_STAGE=0 selects the register-load form.
+// rows * (EX + 2 * M2) complex = 99 KB for four rows, two CTAs per SM.  Default for batch 1; HYENA_B200_ROW_BWD1_STAGE=0 selects the register-load form.
 template <int LOGM2>
 __host__ __device__ constexpr size_t row_bwd1_staged_smem_elems(int rows) {
   return (size_t)rows * (RowGeo<LOGM2>::EX + 2 * RowGeo<LOGM2>::M2);
@@ -981,8 +981,7 @@ __device__ __forceinline__ void row_bwd1_staged_body(const PassArgs& a, const in
 // ------------------------------------------------------------------------------------------------
 // Forward row pass with the filter spectrum row staged by cp.async under the forward row FFT (the register form issues 64
 // __ldg per thread right in front of the pointwise product: long_scoreboard is its top stall).  128-thread CTAs of four
-// rows, shared memory rows * (EX + M2) complex = 66.6 KB: three CTAs per SM.  Default (2.13 -> 1.98 ms at large-1m,
-// profiles/r2_ab.txt run E; a 256-thread staged form with 131 KB per CTA had lost in round 2's first sweep);
+// rows, shared memory rows * (EX + M2) complex = 66.6 KB: three CTAs per SM.  Default;
 // HYENA_B200_ROW_FWD_STAGE=0 selects the register-load form.
 // ------------------------------------------------------------------------------------------------
 template <int LOGM2>

@@ -30,7 +30,7 @@ __device__ __forceinline__ float2 mul_w32(float2 a) {
   else if constexpr (j == 24) return INV ? cmul_negi(a) : cmul_i(a);
   else {
     constexpr float c = cos32(j);
-    constexpr float s = INV ? -sin32(j) : sin32(j);      // multiply by (c - i s): one FMUL2 + one FFMA2
+    constexpr float s = INV ? -sin32(j) : sin32(j);      // multiply by (c - i s)
     return cmul_cs(a, c, s);
   }
 }

@@ -1,9 +1,9 @@
 // Library GEMMs for the in/out projections (the boundary of the custom-kernel span).
 //
-// The projections are plain GEMMs and stay library calls (cuBLASLt).  What this file adds over
-// torch.bmm is the choice of cuBLASLt build: PyTorch 2.11+cu128 bundles cuBLAS 12.8, whose fp32 GEMM
-// on sm_100 is the CUDA-core SGEMM (~55 TFLOP/s measured here).  The CUDA 12.9 toolkit in this image
-// ships cuBLASLt 12.9, which has CUBLAS_COMPUTE_32F_EMULATED_16BFX9: fp32 GEMM emulated on the bf16
+// An alternative to this library's own projection kernels (proj_gemm.cuh): plain library GEMMs (cuBLASLt), selected
+// with HYENA_B200_PROJ=lt or when the user opted into TF32.  What this file adds over torch.bmm is the choice of
+// cuBLASLt build: PyTorch 2.11+cu128 bundles cuBLAS 12.8, whose fp32 GEMM is the CUDA-core SGEMM.  The CUDA 12.9
+// toolkit ships cuBLASLt 12.9, which has CUBLAS_COMPUTE_32F_EMULATED_16BFX9: fp32 GEMM emulated on the bf16
 // tensor cores with nine bf16 products per fp32 product -- fp32-level accuracy (no TF32 rounding), a
 // multiple of the SGEMM rate.  That library is dlopen()ed by absolute path into a private handle
 // (RTLD_LOCAL), so PyTorch's own cuBLAS is untouched.  If it cannot be loaded the entry point reports

@@ -91,7 +91,7 @@ __global__ void time_to_rfft_small_kernel(const float* __restrict__ x, float2* _
   }
 }
 
-static int blocks_for(size_t n) { size_t b = (n + 255) / 256; return (int)(b > 148 * 16 ? 148 * 16 : (b ? b : 1)); }
+static int blocks_for(size_t n) { size_t b = (n + 255) / 256; return (int)(b > 132 * 16 ? 132 * 16 : (b ? b : 1)); }
 
 cudaError_t launch_rfft_to_packed(const float2* X, float2* Z, int H, int logM, int logM1, cudaStream_t s) {
   prof_begin(K_CONVERT, s);

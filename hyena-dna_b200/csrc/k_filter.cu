@@ -36,7 +36,7 @@ cudaError_t launch_filter_bwd(const FilterParams& P, const float* dk, const Filt
   const size_t smem = filter_bwd_smem(P.E);
   cudaError_t e = set_smem(filter_bwd_kernel, smem);
   if (e != cudaSuccess) return e;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int ntiles = (P.L + kBwdTP - 1) / kBwdTP;

@@ -1,6 +1,3 @@
-#include <cstdlib>
-#include <cstring>
-
 #include "launch.h"
 #include "filter_tc.cuh"
 namespace hy {
@@ -14,7 +11,7 @@ cudaError_t launch_filter_bwd_tc(const FilterParams& P, float* wimg, const float
                                  cudaStream_t s) {
   cudaError_t e = set_smem(tc::filter_tc_bwd_kernel, tc::kSmemBytes);
   if (e != cudaSuccess) return e;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   prof_begin(K_FILTER_TC_PREP, s);
@@ -33,7 +30,7 @@ cudaError_t launch_filter_bwd_tc(const FilterParams& P, float* wimg, const float
 cudaError_t launch_filter_fwd_tc(const FilterParams& P, float* wimg, float* kout, cudaStream_t s) {
   cudaError_t e = set_smem(tc::filter_tc_fwd_kernel, tc::kSmemBytes);
   if (e != cudaSuccess) return e;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   prof_begin(K_FILTER_TC_PREP, s);
@@ -42,18 +39,6 @@ cudaError_t launch_filter_fwd_tc(const FilterParams& P, float* wimg, float* kout
   e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   const int ntiles = (P.L + tc::kTileM - 1) / tc::kTileM;
-  static const bool old_form = getenv("HYENA_B200_FILTER_FWD") && !strcmp(getenv("HYENA_B200_FILTER_FWD"), "1");
-  if (P.D <= 256 && !old_form) {                    // TS form: activations in tensor memory, weights resident, two tiles in flight
-    const size_t smem = tc::fwd2_smem_bytes(P.D);
-    e = set_smem(tc::filter_tc_fwd2_kernel, smem);
-    if (e != cudaSuccess) return e;
-    const int pairs = (ntiles + 1) / 2;
-    const int grid2 = pairs < sms ? pairs : sms;
-    prof_begin(K_FILTER_TC_FWD, s);
-    tc::filter_tc_fwd2_kernel<<<grid2, tc::kThreads, smem, s>>>(P, wimg, kout, ntiles);
-    prof_end(K_FILTER_TC_FWD, s);
-    return cudaGetLastError();
-  }
   const int grid = ntiles < sms ? ntiles : sms;
   prof_begin(K_FILTER_TC_FWD, s);
   tc::filter_tc_fwd_kernel<<<grid, tc::kThreads, tc::kSmemBytes, s>>>(P, wimg, kout, ntiles);
@@ -64,7 +49,7 @@ cudaError_t launch_filter_fwd_tc(const FilterParams& P, float* wimg, float* kout
 cudaError_t launch_filter_red_tc(const RedLaunch& r, cudaStream_t s) {
   cudaError_t e = set_smem(tc::filter_tc_red_kernel, tc::kRedSmemBytes);
   if (e != cudaSuccess) return e;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   tc::RedArgs R{r.dh, r.scratch, r.zT, r.dW0, r.db0, r.dW1, r.db1, r.dW2, r.db2, r.dW3, r.dfreq, r.L, r.D, r.E};

@@ -5,7 +5,7 @@
 namespace hy {
 
 static int ln_grid(long long rows) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   long long want = (rows + ln::kWarps - 1) / ln::kWarps;

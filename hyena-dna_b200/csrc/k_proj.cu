@@ -1,4 +1,4 @@
-// Launchers of the tcgen05 projection GEMMs (proj_gemm.cuh).
+// Launchers of the wgmma projection GEMMs (proj_gemm.cuh).
 #include <cstdint>
 #include <cstring>
 
@@ -6,8 +6,6 @@
 #include "proj_gemm.cuh"
 
 namespace hy {
-
-long long* g_proj_dbg = nullptr;      // tools/dbg_proj_timing.py: device buffer for the per-role wait counters (debug)
 
 size_t proj_wimg_bytes(int N, int K) {
   const int NT = 128;
@@ -94,7 +92,7 @@ cudaError_t launch_proj_gemm(const float* act, int act_layout, const float* W, i
                              const float* fir, float* out, int out_layout, int B, int L, int K, int N, int l0, int ln,
                              float* wimg, cudaStream_t s) {
   const int NT = 128;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const size_t total = pg::wimg_floats(N, K, NT);
@@ -107,8 +105,6 @@ cudaError_t launch_proj_gemm(const float* act, int act_layout, const float* W, i
   if (e != cudaSuccess) return e;
   pg::Args a;
   a.act = act; a.wimg = wimg; a.out = out; a.bias = bias; a.fir = fir;
-  a.dbg = g_proj_dbg;
-  a.zero = 0;
   a.B = B; a.L = L; a.K = K; a.N = N; a.l0 = l0; a.ln = ln;
   // TMA needs 16-byte aligned rows (global stride a multiple of 16 bytes) and, for the channel-major box, a 16-byte
   // aligned first position
@@ -130,7 +126,7 @@ void proj_wgrad_plan(int M, int N, int sms, int* mtiles, int* ntiles, int* split
 }
 
 size_t proj_wgrad_scratch_bytes(int M, int N) {
-  int dev = 0, sms = 148, mt, nt, sp;
+  int dev = 0, sms = 132, mt, nt, sp;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   proj_wgrad_plan(M, N, sms, &mt, &nt, &sp);
@@ -139,11 +135,11 @@ size_t proj_wgrad_scratch_bytes(int M, int N) {
 
 cudaError_t launch_proj_wgrad(const float* X, const float* Y, const float* fir, float* dW, int transposed_out, float beta,
                               int B, int L, int M, int N, float* part, cudaStream_t s) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   wg::Args a;
-  a.X = X; a.Y = Y; a.fir = fir; a.part = part; a.dbg = g_proj_dbg; a.zero = 0; a.B = B; a.L = L; a.M = M; a.N = N;
+  a.X = X; a.Y = Y; a.fir = fir; a.part = part; a.zero = 0; a.B = B; a.L = L; a.M = M; a.N = N;
   a.chunks_per_b = (L + 31) / 32;
   proj_wgrad_plan(M, N, sms, &a.mtiles, &a.ntiles, &a.splits);
   const long long total_chunks = (long long)B * a.chunks_per_b;

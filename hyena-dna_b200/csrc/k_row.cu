@@ -5,8 +5,7 @@
 namespace hy {
 
 // The batch-1 backward kernel at two CTAs per SM (up to 255 registers, no spills) instead of row_pass_kernel's three CTAs
-// at <= 170 registers with ~80 registers spilled: same body, 3.52 ms instead of 3.94-4.00 ms at large-1m
-// (profiles/r1_config_sweep.txt).  Default; HYENA_B200_ROW_BWD1_CTAS=3 selects the three-CTA form.
+// at <= 170 registers with ~80 registers spilled: same body.  Default; HYENA_B200_ROW_BWD1_CTAS=3 selects the three-CTA form.
 template <int LOGM2>
 __global__ void __launch_bounds__(128, 2) row_pass_bwd1_2cta_kernel(const PassArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];

@@ -36,7 +36,7 @@ cudaError_t launch_filter_red_tc(const RedLaunch& r, cudaStream_t s);   // k_fil
 cudaError_t launch_filter_bwd(const FilterParams& P, const float* dk, const FilterGrads& G, cudaStream_t s);
 cudaError_t launch_short_bwd(const ShortBwdArgs& a, int B, cudaStream_t s);
 cudaError_t launch_twiddle_init(float2* tw1024, float2* twlo, cudaStream_t s);
-// k_proj.cu: projection GEMMs on tcgen05 (3xTF32)
+// k_proj.cu: projection GEMMs on wgmma (3xTF32)
 size_t proj_wimg_bytes(int N, int K);
 cudaError_t launch_proj_gemm(const float* act, int act_layout, const float* W, int ldw, int w_transposed, const float* bias,
                              const float* fir, float* out, int out_layout, int B, int L, int K, int N, int l0, int ln,

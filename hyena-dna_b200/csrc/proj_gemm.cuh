@@ -1,4 +1,4 @@
-// Projection GEMMs of the operator on the 5th-generation tensor cores (tcgen05 / TMEM), fp32 accuracy via 3xTF32.
+// Projection GEMMs of the operator on the Hopper tensor cores (wgmma), fp32 accuracy via 3xTF32.
 //
 // in_proj / out_proj and their input gradients (src/models/sequence/hyena.py:350-351, :391, :440) are all of the form
 //     OUT[pos][n] = sum_k ACT[pos][k] * W[n][k]            pos = up to 2^20 sequence positions, K <= 768, N <= 768
@@ -6,23 +6,17 @@
 // channel-major (n, pos) (p, dy_pre: what the FFT passes read) or row-major (pos, n) (y, du).  One persistent,
 // warp-specialised kernel (proj_gemm_kernel):
 //
-//   tile      128 positions (UMMA M = 128, one TMEM lane per position) x NT outputs, K streamed in chunks of 32
-//   A operand the activation chunk: global -> shared-memory ring by TMA bulk copies issued by a producer warp (one copy per
-//             row of the chunk, four chunks in flight) -> registers -> (hi, lo) tf32 split -> TENSOR MEMORY (tcgen05.st).  The MMAs
-//             read A from TMEM: the shared-memory port is the scarce resource of a tf32 MMA (an SS-mode M128 N256 K8
-//             instruction reads 12 KB per 128 cycles), so only B goes through it.
+//   tile      128 positions x 128 outputs, K streamed in chunks of 32; two consumer warpgroups of 64 positions each
+//   A operand the activation chunk: global -> shared-memory staging ring by TMA (one tiled copy per chunk, issued by a
+//             producer warp, four chunks in flight) -> registers in the wgmma A-fragment layout -> (hi, lo) tf32 split.
+//             The MMAs read A from registers, so only B goes through the shared-memory port.
 //   B operand the weights, pre-split once per call into hi / lo images in the canonical no-swizzle K-major
-//             core-matrix layout (proj_prep_kernel), streamed by TMA bulk copies (cp.async.bulk, SASS UBLKCP) into a
-//             ring of shared-memory stages guarded by mbarriers
-//   D         fp32 accumulators in TMEM, two buffers used in turn for every PAIR of K chunks (24 MMAs, the 16 small correction products
-//             first so that only the 8 hi*hi MMAs truncate at full scale); the epilogue
-//             warps drain each pair into per-thread fp32 registers (round-to-nearest adds) while the next pair is being
-//             multiplied.  Reason: the tensor core adds into its accumulator with truncation, so a long chain biases the
-//             result by ~(number of MMAs) x 2^-24 towards zero -- measured here: 96 chained MMAs (K = 256) cost 4x the
-//             error of cuBLASLt's BF16x9 on y at L = 2^20, the 2^20-position weight gradients lost four digits.
+//             core-matrix layout (proj_prep_kernel), streamed by TMA bulk copies into the same ring of stages
+//   D         fp32 accumulators in registers, restarted for every K chunk (12 MMAs, the 8 small correction products
+//             first so that only the 4 hi*hi MMAs add at full scale) and added into a second register set with
+//             round-to-nearest adds.  Reason: the tensor core adds into its accumulator with truncation, so a long chain
+//             biases the result by ~(number of MMAs) x 2^-24 towards zero.
 //   3xTF32    x = hi + lo, hi = rna_tf32(x), lo = rna_tf32(x - hi);  D += Ahi Bhi + Alo Bhi + Ahi Blo   (lo*lo < 2^-22)
-//
-// Warp roles: see the comment above proj_gemm_kernel.
 //
 // Optional fused prologue (FIR): the activation is ds (B, C, L) and the GEMM consumes dp = transposed 3-tap depthwise
 // filter of ds (dp[t] = w2 ds[t] + w1 ds[t+1] + w0 ds[t+2], hyena.py:363-369 backward), so dp never exists in HBM.
@@ -38,7 +32,7 @@ namespace hy {
 namespace pg {
 
 constexpr int kKC = 32;                 // K chunk (one chunk = 4 MMAs of K = 8 per product)
-constexpr int kThreads = 512;          // 16 warps: 4 convert, 8 epilogue, 2 TMA producers (weights / activations), 2 MMA issuers
+constexpr int kThreads = 288;           // 9 warps: 0-7 two consumer warpgroups, 8 TMA producer
 constexpr uint32_t kSBO = 1024, kLBO = 128;
 constexpr uint32_t kAPitchCh = 132 * 4; // ACT_CH staging row: 128 positions + one look-ahead quad (fused FIR)
 constexpr uint32_t kAStageBytes = 32 * kAPitchCh;      // 16.5 KB (>= the 16 KB an ACT_ROW tile needs)
@@ -63,8 +57,6 @@ struct Args {
   int ntiles_n;          // ceil(N / NT)
   int mtiles_per_b;      // ceil(ln / 128)
   int vec;               // 1: the activation qualifies for TMA (16-byte aligned rows): `tmap` is valid
-  unsigned zero;         // 0 at run time (tc::mbar_arrive_after_loads)
-  long long* dbg;        // optional (tools/dbg_proj_timing.py): per-role wait / work cycle counters of CTA 0, or null
 };
 
 // ------------------------------------------------------------------------------------------------ weight images
@@ -95,101 +87,49 @@ __host__ __device__ constexpr size_t wimg_floats(int N, int K, int NT) {
 
 // ------------------------------------------------------------------------------------------------ the kernel
 // Activation staging slot (17 KB, 1024-byte aligned):
-//   ACT_ROW  128 rows x 32 floats (128-byte rows), 16-byte pieces XOR-swizzled by the row (= TMA SWIZZLE_128B): LDS.128 of
-//            32 different rows at the same logical piece is bank-conflict free
+//   ACT_ROW  128 rows x 32 floats (128-byte rows), 16-byte pieces XOR-swizzled by the row (= TMA SWIZZLE_128B): the
+//            A-fragment loads (8 rows x 4 consecutive k per warp) are bank-conflict free
 //   ACT_CH   32 channel rows x 132 floats (128 positions + 4 look-ahead samples for the fused FIR), dense
 constexpr uint32_t kSStageBytes = 17408;
 static_assert(kSStageBytes >= 32 * kAPitchCh && kSStageBytes >= 128 * 128 && kSStageBytes % 1024 == 0, "staging slot");
 
 template <int NT> struct Cfg {
-  static constexpr int STAGES = 4;                                     // weight stages = A buffers = staging slots
+  static constexpr int STAGES = 4;                                     // weight stages = staging slots
   static constexpr uint32_t STAGE_BYTES = 2u * NT * kKC * 4u;          // hi + lo image of one K chunk
-  static constexpr uint32_t D_COLS = NT;                               // per accumulator buffer
-  static constexpr uint32_t A_COL0 = 2 * NT;                           // A buffers after the two accumulators
-  static constexpr uint32_t TMEM_COLS = 512;
   static constexpr size_t OFF_A = (size_t)STAGES * STAGE_BYTES;        // activation staging ring
   static constexpr size_t OFF_BAR = OFF_A + (size_t)STAGES * kSStageBytes;
   static constexpr size_t OFF_FIR = OFF_BAR + 256;
   static constexpr size_t SMEM = OFF_FIR;                              // + 12 K bytes of taps when the FIR is fused
-  static_assert(2 * NT + 4 * 64 <= 512, "two accumulators and four A (hi, lo) chunk buffers must fit tensor memory");
-  static_assert(NT == 128, "the epilogue keeps NT / 2 partial sums per thread in registers");
-  static_assert(STAGES == 4, "slot c uses weight stage / staging slot / A buffer c & 3: a chunk pair then owns stages "
-                             "{0,1} or {2,3}, i.e. each of the two MMA issuers sees its barriers' phases in order");
+  static_assert(NT == 128, "one m64n128 accumulator per consumer warpgroup");
 };
 
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-
-// Warp roles (512 threads):
-//   warps 0-3    convert: staged activation chunk -> registers (-> fused FIR) -> (hi, lo) split -> tensor memory
-//   warps 4-7    epilogue, output columns [0, 64)   } thread = position; drain every chunk pair into registers,
-//   warps 11-14  epilogue, output columns [64, 128) } store the tile at the end
-//   warp 8       producer: TMA bulk copies of the weight images (lane 0); stages the activation by hand when it does
-//                not qualify for TMA (all lanes)
-//   warp 15      producer: tiled TMA copies of the activation tiles (lane 0)
-//   warps 9, 10  MMA issuers (lane 0 each), alternate chunk pairs
+// Warp roles (288 threads):
+//   warps 0-3, 4-7  consumer warpgroups, positions [0, 64) and [64, 128) of the tile: staged activation -> A fragments
+//                   (-> fused FIR) -> (hi, lo) split -> wgmma against the weight stage -> register accumulators -> stores
+//   warp 8          producer: per chunk one TMA bulk copy of the weight images and one tiled TMA copy of the activation
+//                   tile (lane 0); stages the activation by hand when it does not qualify for TMA (all lanes)
 template <int NT, int ACT, int OUT>
 __global__ void __launch_bounds__(kThreads, 1) proj_gemm_kernel(const Args a, const __grid_constant__ CUtensorMap tmap) {
   using C = Cfg<NT>;
   extern __shared__ __align__(1024) unsigned char smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR);
-  // barrier map: b_full[4] b_empty[4] a_full[4] a_empty[4] s_full[4] s_empty[4] d_full[2] d_empty[2]
-  uint32_t* tmem_p = reinterpret_cast<uint32_t*>(bars + 28);
   float* fir_s = reinterpret_cast<float*>(smem + C::OFF_FIR);     // (K, 3) taps, FIR only
   const uint32_t sbase = tc::smem_u32(smem);
   const uint32_t bar0 = tc::smem_u32(bars);
-  auto B_FULL = [&](int s) { return bar0 + 8u * s; };
-  auto B_EMPTY = [&](int s) { return bar0 + 8u * (4 + s); };
-  auto A_FULL = [&](int j) { return bar0 + 8u * (8 + j); };
-  auto A_EMPTY = [&](int j) { return bar0 + 8u * (12 + j); };
-  auto S_FULL = [&](int j) { return bar0 + 8u * (16 + j); };
-  auto S_EMPTY = [&](int j) { return bar0 + 8u * (20 + j); };
-  auto D_FULL = [&](int j) { return bar0 + 8u * (24 + j); };
-  auto D_EMPTY = [&](int j) { return bar0 + 8u * (26 + j); };
+  auto FULL = [&](int s) { return bar0 + 8u * s; };
+  auto EMPTY = [&](int s) { return bar0 + 8u * (4 + s); };
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const bool use_fir = (ACT == ACT_CH) && a.fir != nullptr;
-  if (warp == 9) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc::smem_u32(tmem_p)), "r"(C::TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   if (use_fir)
     for (int i = tid; i < 3 * a.K; i += kThreads) fir_s[i] = __ldg(a.fir + i);
   if (tid == 0) {
-    for (int s = 0; s < 4; ++s) {
-      tc::mbar_init(B_FULL(s), 1); tc::mbar_init(B_EMPTY(s), 1);
-      tc::mbar_init(A_FULL(s), 128); tc::mbar_init(A_EMPTY(s), 1);
-      tc::mbar_init(S_FULL(s), 1); tc::mbar_init(S_EMPTY(s), 128);
-    }
-    for (int j = 0; j < 2; ++j) { tc::mbar_init(D_FULL(j), 1); tc::mbar_init(D_EMPTY(j), 256); }
+    for (int s = 0; s < 4; ++s) { tc::mbar_init(FULL(s), 1); tc::mbar_init(EMPTY(s), 8); }
   }
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = *tmem_p;
-
-  // debug timing: cycles spent in barrier waits, per role (CTA 0), see tools/dbg_proj_timing.py
-  const bool dbg_on = a.dbg != nullptr && blockIdx.x == 0;
-  long long dbg_t[4] = {0, 0, 0, 0};
-  auto timed_wait = [&](uint32_t bar, uint32_t parity, int slot) {
-    if (dbg_on) {
-      const long long t0 = clock64();
-      tc::mbar_wait_u(bar, parity);
-      dbg_t[slot] += clock64() - t0;
-    } else {
-      tc::mbar_wait_u(bar, parity);
-    }
-  };
-  const long long dbg_start = clock64();
 
   const int mtiles = a.B * a.mtiles_per_b;
   const int ntiles = mtiles * a.ntiles_n;
-  const int npairs = (a.kchunks + 1) / 2;
-  // slot numbering shared by all roles: tile ordinal T of this CTA owns slots [T * spt, (T + 1) * spt), spt = 2 * npairs
-  // (even: with an odd chunk count the last slot of a tile stays unused); slot -> stage / staging slot / A buffer slot & 3
-  const uint32_t spt = 2u * (uint32_t)npairs;
   const int lend = a.l0 + a.ln;
   auto tile_pos = [&](int tile, int& b, int& lt, int& nt) {
     const int mt = tile / a.ntiles_n;
@@ -198,300 +138,156 @@ __global__ void __launch_bounds__(kThreads, 1) proj_gemm_kernel(const Args a, co
     lt = a.l0 + (mt - b * a.mtiles_per_b) * 128;
   };
 
-  if (warp < 4) {
-    // ================================================================== converters: thread = position of the tile
-    const int row = tid;                                           // 0..127 == TMEM lane
-    const uint32_t lane_addr = tmem + ((uint32_t)(32 * warp) << 16);
-    uint32_t T = 0, parSf = 0u, parAe = 0xFu;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++T) {
-      for (int kc = 0; kc < a.kchunks; ++kc) {
-        const int s = (int)((T * spt + (uint32_t)kc) & 3u);
-        timed_wait(S_FULL(s), (parSf >> s) & 1u, 0);              // the producer's copies of this chunk have landed
-        parSf ^= 1u << s;
-        const unsigned char* st = smem + C::OFF_A + (size_t)s * kSStageBytes;
-        float x[kKC];
-        if constexpr (ACT == ACT_ROW) {
-#pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            const float4 v = *reinterpret_cast<const float4*>(st + row * 128 + ((c ^ (row & 7)) << 4));
-            x[4 * c] = v.x; x[4 * c + 1] = v.y; x[4 * c + 2] = v.z; x[4 * c + 3] = v.w;
-          }
-        } else {
-          if (!use_fir) {
-#pragma unroll
-            for (int j = 0; j < kKC; ++j) x[j] = *reinterpret_cast<const float*>(st + j * kAPitchCh + row * 4);
-          } else {
-            // dp[t] = w2 ds[t] + w1 ds[t+1] + w0 ds[t+2]; ds beyond the tensor end is staged as zero, a position beyond
-            // the processed range produces a value nobody stores; channels >= K are staged as zero
-            const int k0 = kc * kKC;
-            const bool kfull = k0 + kKC <= a.K;
-#pragma unroll
-            for (int j = 0; j < kKC; ++j) {
-              const float* sp = reinterpret_cast<const float*>(st + j * kAPitchCh) + row;
-              const float* w = fir_s + 3 * ((kfull || k0 + j < a.K) ? k0 + j : 0);
-              x[j] = fmaf(w[2], sp[0], fmaf(w[1], sp[1], w[0] * sp[2]));
-            }
-          }
-        }
-        {                                                          // staging slot read: the producer may refill it -- once the
-          uint32_t dep = 0;                                        // loads have actually returned (see mbar_arrive_after_loads)
-#pragma unroll
-          for (int j = 0; j < kKC; ++j) dep |= __float_as_uint(x[j]);
-          tc::mbar_arrive_after_loads(S_EMPTY(s), dep, a.zero);
-        }
-        uint32_t hi[kKC], lo[kKC];
-#pragma unroll
-        for (int j = 0; j < kKC; ++j) {
-          float hh, lw;
-          tc::split_tf32(x[j], hh, lw);
-          hi[j] = __float_as_uint(hh); lo[j] = __float_as_uint(lw);
-        }
-        timed_wait(A_EMPTY(s), (parAe >> s) & 1u, 1);             // MMAs of the previous use of this A buffer are done
-        parAe ^= 1u << s;
-        tc::fence_after_sync();
-        const uint32_t acol = C::A_COL0 + s * 64;
-        tc::tmem_st32(lane_addr + acol, hi);
-        tc::tmem_st32(lane_addr + acol + 32, lo);
-        tc::tmem_wait_st();
-        tc::fence_before_sync();
-        tc::mbar_arrive(A_FULL(s));
-      }
-    }
-    if (dbg_on && tid == 0) { a.dbg[0] = dbg_t[0]; a.dbg[1] = dbg_t[1]; a.dbg[2] = clock64() - dbg_start; }
-  } else if (warp == 8) {
-    // ================================================================== producer: weight images + activation tiles (TMA)
-    // One thread issues, per chunk, one bulk copy of the weight stage and ONE tiled TMA copy of the activation tile
-    // (tensor map: box 32 k x 128 positions, 128-byte swizzle, for a row-major activation; box 132 positions x 32
-    // channels for a channel-major one).  Out-of-range coordinates are zero-filled by the copy engine (end of the tensor:
-    // exactly the zero padding the fused FIR needs; K tail).  Activations that do not qualify for TMA (rows not 16-byte
-    // aligned) are staged by the 32 lanes with plain loads and stores instead.
+  if (warp == 8) {
+    // ================================================================== producer
+    // Out-of-range coordinates are zero-filled by the copy engine (end of the tensor: exactly the zero padding the fused
+    // FIR needs; K tail).  Activations that do not qualify for TMA (rows not 16-byte aligned) are staged by the 32 lanes
+    // with plain loads and stores instead.
     if (lane == 0 && a.vec) tc::tma_prefetch_desc(&tmap);
-    uint32_t T = 0, parBe = 0xFu, parSe = 0xFu;
-    if (a.vec) {
-      // Two independent issue loops (this lane: weights; warp 15: activation tiles): the activation copy of a chunk only needs its staging slot back (the
-      // converters release it as soon as they have read it), the weight copy needs the MMAs of four chunks ago to have
-      // completed.  Issued from one loop the activation stream ran a whole weight-stage wait late (measured: converters
-      // waiting ~970 of 1650 cycles per chunk for their tile).
-      if (lane == 0) {
-        for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++T) {
-          int b, lt, nt;
-          tile_pos(tile, b, lt, nt);
-          for (int kc = 0; kc < a.kchunks; ++kc) {
-            const int s = (int)((T * spt + (uint32_t)kc) & 3u);
-            timed_wait(B_EMPTY(s), (parBe >> s) & 1u, 0);
-            parBe ^= 1u << s;
-            tc::mbar_arrive_expect_tx(B_FULL(s), C::STAGE_BYTES);
-            const float* src = a.wimg + ((size_t)nt * a.kchunks + kc) * (C::STAGE_BYTES / 4);
-            tc::bulk_g2s(sbase + s * C::STAGE_BYTES, src, C::STAGE_BYTES, B_FULL(s));
-          }
-        }
-      }
-    } else
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++T) {
-      int b, lt, nt;
-      tile_pos(tile, b, lt, nt);
-      for (int kc = 0; kc < a.kchunks; ++kc) {
-        const int s = (int)((T * spt + (uint32_t)kc) & 3u);
-        const int k0 = kc * kKC;
-        if (lane == 0) {
-          timed_wait(B_EMPTY(s), (parBe >> s) & 1u, 0);
-          tc::mbar_arrive_expect_tx(B_FULL(s), C::STAGE_BYTES);
-          const float* src = a.wimg + ((size_t)nt * a.kchunks + kc) * (C::STAGE_BYTES / 4);
-          tc::bulk_g2s(sbase + s * C::STAGE_BYTES, src, C::STAGE_BYTES, B_FULL(s));
-          timed_wait(S_EMPTY(s), (parSe >> s) & 1u, 1);
-        }
-        parBe ^= 1u << s; parSe ^= 1u << s;
-        {
-          __syncwarp();
-          unsigned char* st = smem + C::OFF_A + (size_t)s * kSStageBytes;
-          if constexpr (ACT == ACT_ROW) {
-#pragma unroll 1
-            for (int i = 0; i < 4; ++i) {
-              const int r = lane + 32 * i, l = lt + r;
-              const float* src = a.act + ((size_t)b * a.L + (l < lend ? l : 0)) * a.K + k0;
-#pragma unroll
-              for (int c = 0; c < 8; ++c) {
-                float4 v;
-                v.x = (l < lend && k0 + 4 * c + 0 < a.K) ? __ldg(src + 4 * c + 0) : 0.f;
-                v.y = (l < lend && k0 + 4 * c + 1 < a.K) ? __ldg(src + 4 * c + 1) : 0.f;
-                v.z = (l < lend && k0 + 4 * c + 2 < a.K) ? __ldg(src + 4 * c + 2) : 0.f;
-                v.w = (l < lend && k0 + 4 * c + 3 < a.K) ? __ldg(src + 4 * c + 3) : 0.f;
-                *reinterpret_cast<float4*>(st + r * 128 + ((c ^ (r & 7)) << 4)) = v;
-              }
-            }
-          } else {
-            const int j = lane;
-            const bool kv = k0 + j < a.K;
-            const float* src = a.act + ((size_t)b * a.K + (kv ? k0 + j : 0)) * a.L + lt;
-            float* dst = reinterpret_cast<float*>(st + j * kAPitchCh);
-            for (int e = 0; e < 132; ++e) dst[e] = (kv && lt + e < a.L) ? __ldg(src + e) : 0.f;
-          }
-          __syncwarp();
-          if (lane == 0) tc::mbar_arrive(S_FULL(s));
-        }
-      }
-    }
-    if (dbg_on && lane == 0) { a.dbg[3] = dbg_t[0]; if (!a.vec) a.dbg[4] = dbg_t[1]; }
-  } else if (warp == 15) {
-    // ================================================================== producer: activation tiles (TMA), own warp
-    if (lane == 0 && a.vec) {
-      uint32_t T = 0, parSe = 0xFu;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++T) {
-        int b, lt, nt;
-        tile_pos(tile, b, lt, nt);
-        for (int kc = 0; kc < a.kchunks; ++kc) {
-          const int s = (int)((T * spt + (uint32_t)kc) & 3u);
-          const int k0 = kc * kKC;
-          const uint32_t st_u = sbase + (uint32_t)C::OFF_A + (uint32_t)s * kSStageBytes;
-          timed_wait(S_EMPTY(s), (parSe >> s) & 1u, 1);
-          parSe ^= 1u << s;
-          if constexpr (ACT == ACT_ROW) {
-            tc::mbar_arrive_expect_tx(S_FULL(s), 128u * 128u);
-            tc::tma_load_2d(st_u, &tmap, k0, b * a.L + lt, S_FULL(s));
-          } else {
-            tc::mbar_arrive_expect_tx(S_FULL(s), 32u * kAPitchCh);
-            tc::tma_load_2d(st_u, &tmap, lt, b * a.K + k0, S_FULL(s));
-          }
-        }
-      }
-      if (dbg_on) a.dbg[4] = dbg_t[1];
-    }
-  } else if (warp == 9 || warp == 10) {
-    // ================================================================== MMA issuers (one thread each of warps 9 and 10)
-    // Chunk pairs alternate between the two accumulator buffers, and between the two issuing threads: a pair starts a
-    // fresh accumulation (first MMA overwrites), so the pairs are independent and no ordering is needed between the two
-    // threads' instruction streams; with slot c on stage / A buffer c & 3 each issuer also owns its barriers (stages
-    // {0,1} or {2,3}), so their phases reach it in order.  While one thread sits in its barrier waits (~200 cycles each)
-    // the other one's MMAs keep the tensor pipe busy (measured with one issuer: 1800 cycles per chunk for 768 of MMA).
-    if (lane == 0) {
-      constexpr uint32_t idesc = tc::make_idesc(NT);
-      const uint32_t me = (uint32_t)(warp - 9);
-      uint32_t pp = 0, T = 0, parAf = 0u, parBf = 0u;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++T) {
-        for (int pr = 0; pr < npairs; ++pr, ++pp) {
-          if ((pp & 1u) != me) continue;
-          const int dbuf = pp & 1;
-          timed_wait(D_EMPTY(dbuf), ((pp >> 1) & 1) ^ 1, 0);       // the epilogue has drained this accumulator
-          tc::fence_after_sync();
-          const uint32_t dcol = tmem + dbuf * C::D_COLS;
-          const int kc_end = min(a.kchunks, 2 * pr + 2);
-          // Order inside a pair: the correction products (lo*hi, hi*lo; 2^-11 of the result) of BOTH chunks first, the
-          // hi*hi products last.  Every MMA truncates the accumulator it adds into (error ~ one-sided 2^-24 of the
-          // accumulator's magnitude), so only the 8 MMAs issued after the accumulator has reached full scale cost
-          // accuracy -- 24 did in chunk order (tools/acc_1m.py: the difference shows as a systematic shrink of y).
-          uint32_t bhi_[2], ahi_[2];
-          int ss_[2];
-          for (int kc = 2 * pr; kc < kc_end; ++kc) {
-            const int s = (int)((T * spt + (uint32_t)kc) & 3u);
-            timed_wait(B_FULL(s), (parBf >> s) & 1u, 1);
-            timed_wait(A_FULL(s), (parAf >> s) & 1u, 2);
-            parBf ^= 1u << s; parAf ^= 1u << s;
-            tc::fence_after_sync();
-            const uint32_t bhi = sbase + s * C::STAGE_BYTES, blo = bhi + C::STAGE_BYTES / 2;
-            const uint32_t ahi = tmem + C::A_COL0 + s * 64, alo = ahi + 32;
-            bhi_[kc - 2 * pr] = bhi; ahi_[kc - 2 * pr] = ahi; ss_[kc - 2 * pr] = s;
-#pragma unroll
-            for (int pass = 1; pass < 3; ++pass) {
-              const uint32_t aa = (pass == 1) ? alo : ahi;
-              const uint32_t bb = (pass == 2) ? blo : bhi;
-#pragma unroll
-              for (int ks = 0; ks < kKC / 8; ++ks)
-                tc::mma_tf32_ts(dcol, aa + 8 * ks, tc::make_desc_ls(bb + ks * 2 * kLBO, kLBO, kSBO), idesc,
-                                ((kc - 2 * pr) | (pass - 1) | ks) ? 1u : 0u);
-            }
-          }
-          for (int i = 0; i < kc_end - 2 * pr; ++i) {
-#pragma unroll
-            for (int ks = 0; ks < kKC / 8; ++ks)
-              tc::mma_tf32_ts(dcol, ahi_[i] + 8 * ks, tc::make_desc_ls(bhi_[i] + ks * 2 * kLBO, kLBO, kSBO), idesc, 1u);
-            tc::mma_commit(A_EMPTY(ss_[i]));                       // A chunk buffer free once these MMAs complete
-            tc::mma_commit(B_EMPTY(ss_[i]));                       // and so is the weight stage
-          }
-          tc::mma_commit(D_FULL(dbuf));
-        }
-      }
-      if (dbg_on && me == 0) { a.dbg[5] = dbg_t[0]; a.dbg[6] = dbg_t[1]; a.dbg[7] = dbg_t[2]; a.dbg[8] = clock64() - dbg_start;
-                               a.dbg[10] = (long long)((ntiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x) * a.kchunks; }
-    }
-  } else if (warp != 15) {
-    // ================================================================== epilogue: thread = position, 64 columns each
-    const int half = warp >= 11 ? 1 : 0;
-    const int lq = warp & 3;                                       // TMEM lane quadrant this warp may access
-    const int row = 32 * lq + lane;
-    const uint32_t lane_addr = tmem + ((uint32_t)(32 * lq) << 16);
-    uint32_t pp = 0;
+    uint32_t it = 0;
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
       int b, lt, nt;
       tile_pos(tile, b, lt, nt);
-      const int l = lt + row;
-      const bool pv = l < lend;
-      float acc[64];
-      for (int pr = 0; pr < npairs; ++pr, ++pp) {
-        const int dbuf = pp & 1;
-        timed_wait(D_FULL(dbuf), (pp >> 1) & 1, 0);
-        tc::fence_after_sync();
-#pragma unroll
-        for (int c0 = 0; c0 < 64; c0 += 32) {
-          uint32_t r[32];
-          tc::tmem_ld32_nowait(lane_addr + dbuf * C::D_COLS + 64 * half + c0, r);
-          tc::tmem_wait_ld();
-          if (pr == 0) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) acc[c0 + j] = __uint_as_float(r[j]);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) acc[c0 + j] += __uint_as_float(r[j]);
+      for (int kc = 0; kc < a.kchunks; ++kc, ++it) {
+        const int s = (int)(it & 3u);
+        const int k0 = kc * kKC;
+        tc::mbar_wait_u(EMPTY(s), ((it >> 2) & 1u) ^ 1u);
+        const float* wsrc = a.wimg + ((size_t)nt * a.kchunks + kc) * (C::STAGE_BYTES / 4);
+        const uint32_t st_u = sbase + (uint32_t)C::OFF_A + (uint32_t)s * kSStageBytes;
+        if (a.vec) {
+          if (lane == 0) {
+            const uint32_t abytes = (ACT == ACT_ROW) ? 128u * 128u : 32u * kAPitchCh;
+            tc::mbar_arrive_expect_tx(FULL(s), C::STAGE_BYTES + abytes);
+            tc::bulk_g2s(sbase + s * C::STAGE_BYTES, wsrc, C::STAGE_BYTES, FULL(s));
+            if constexpr (ACT == ACT_ROW) tc::tma_load_2d(st_u, &tmap, k0, b * a.L + lt, FULL(s));
+            else tc::tma_load_2d(st_u, &tmap, lt, b * a.K + k0, FULL(s));
           }
+          continue;
         }
-        tc::fence_before_sync();
-        tc::mbar_arrive(D_EMPTY(dbuf));
-      }
-      const int nbase = nt * NT + 64 * half;
-      if constexpr (OUT == OUT_CH) {
-        float* dst = a.out + ((size_t)b * a.N + nbase) * a.L + l;
-        if (nbase + 64 <= a.N && a.bias == nullptr) {               // full tile: plain strided stores (warp = 128 bytes each)
-          if (pv) {
+        unsigned char* st = smem + C::OFF_A + (size_t)s * kSStageBytes;
+        if constexpr (ACT == ACT_ROW) {
+#pragma unroll 1
+          for (int i = 0; i < 4; ++i) {
+            const int r = lane + 32 * i, l = lt + r;
+            const float* src = a.act + ((size_t)b * a.L + (l < lend ? l : 0)) * a.K + k0;
 #pragma unroll
-            for (int j = 0; j < 64; ++j) { *dst = acc[j]; dst += a.L; }
+            for (int c = 0; c < 8; ++c) {
+              float4 v;
+              v.x = (l < lend && k0 + 4 * c + 0 < a.K) ? __ldg(src + 4 * c + 0) : 0.f;
+              v.y = (l < lend && k0 + 4 * c + 1 < a.K) ? __ldg(src + 4 * c + 1) : 0.f;
+              v.z = (l < lend && k0 + 4 * c + 2 < a.K) ? __ldg(src + 4 * c + 2) : 0.f;
+              v.w = (l < lend && k0 + 4 * c + 3 < a.K) ? __ldg(src + 4 * c + 3) : 0.f;
+              *reinterpret_cast<float4*>(st + r * 128 + ((c ^ (r & 7)) << 4)) = v;
+            }
           }
         } else {
+          const int j = lane;
+          const bool kv = k0 + j < a.K;
+          const float* src = a.act + ((size_t)b * a.K + (kv ? k0 + j : 0)) * a.L + lt;
+          float* dst = reinterpret_cast<float*>(st + j * kAPitchCh);
+          for (int e = 0; e < 132; ++e) dst[e] = (kv && lt + e < a.L) ? __ldg(src + e) : 0.f;
+        }
+        __syncwarp();
+        if (lane == 0) {
+          tc::mbar_arrive_expect_tx(FULL(s), C::STAGE_BYTES);
+          tc::bulk_g2s(sbase + s * C::STAGE_BYTES, wsrc, C::STAGE_BYTES, FULL(s));
+        }
+      }
+    }
+    return;
+  }
+
+  // ================================================================== consumers: warpgroup wg = positions [64 wg, 64 wg + 64)
+  const int wg = warp >> 2, g = lane >> 2, t = lane & 3;
+  const int r0 = 64 * wg + 16 * (warp & 3) + g;                  // fragment rows r0, r0 + 8 of the tile
+  uint32_t it = 0;
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    int b, lt, nt;
+    tile_pos(tile, b, lt, nt);
+    float sum[64], acc[64];
+    for (int kc = 0; kc < a.kchunks; ++kc, ++it) {
+      const int s = (int)(it & 3u);
+      tc::mbar_wait_u(FULL(s), (it >> 2) & 1u);                    // weights and activation of this chunk have landed
+      const unsigned char* st = smem + C::OFF_A + (size_t)s * kSStageBytes;
+      const int k0 = kc * kKC;
+      uint32_t ahi[4][4], alo[4][4];
 #pragma unroll
-          for (int j = 0; j < 64; ++j) {
-            if (pv && nbase + j < a.N) {
-              float v = acc[j];
-              if (a.bias) v += __ldg(a.bias + nbase + j);
-              dst[(size_t)j * a.L] = v;
+      for (int ks = 0; ks < 4; ++ks) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int row = r0 + ((q & 1) ? 8 : 0), k = 8 * ks + t + ((q & 2) ? 4 : 0);
+          float x;
+          if constexpr (ACT == ACT_ROW) {
+            x = *reinterpret_cast<const float*>(st + row * 128 + (((k >> 2) ^ (row & 7)) << 4) + (k & 3) * 4);
+          } else {
+            const float* sp = reinterpret_cast<const float*>(st + k * kAPitchCh) + row;
+            if (!use_fir) {
+              x = sp[0];
+            } else {
+              // dp[t] = w2 ds[t] + w1 ds[t+1] + w0 ds[t+2]; ds beyond the tensor end is staged as zero, a position
+              // beyond the processed range produces a value nobody stores; channels >= K are staged as zero
+              const float* w = fir_s + 3 * (k0 + k < a.K ? k0 + k : 0);
+              x = fmaf(w[2], sp[0], fmaf(w[1], sp[1], w[0] * sp[2]));
             }
           }
+          float hh, lw;
+          tc::split_tf32(x, hh, lw);
+          ahi[ks][q] = __float_as_uint(hh); alo[ks][q] = __float_as_uint(lw);
         }
+      }
+      // a fresh accumulation per chunk: the correction products (lo*hi, hi*lo; 2^-11 of the result) first, the four
+      // hi*hi products last, so that only those add at full scale; chunks are summed with round-to-nearest adds
+      const uint32_t bhi = sbase + s * C::STAGE_BYTES, blo = bhi + C::STAGE_BYTES / 2;
+      tc::wgmma_fence();
+      tc::fence_regs(acc);
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+        tc::wgmma_rs_n128(acc, alo[ks], tc::make_desc_ls(bhi + ks * 2 * kLBO, kLBO, kSBO), ks ? 1u : 0u);
+        tc::wgmma_rs_n128(acc, ahi[ks], tc::make_desc_ls(blo + ks * 2 * kLBO, kLBO, kSBO), 1u);
+      }
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks)
+        tc::wgmma_rs_n128(acc, ahi[ks], tc::make_desc_ls(bhi + ks * 2 * kLBO, kLBO, kSBO), 1u);
+      tc::wgmma_commit();
+      tc::wgmma_wait<0>();
+      tc::fence_regs(acc);
+      __syncwarp();
+      if (lane == 0) tc::mbar_arrive(EMPTY(s));                    // weight stage and staging slot are free
+      if (kc == 0) {
+#pragma unroll
+        for (int i = 0; i < 64; ++i) sum[i] = acc[i];
       } else {
-        float* dst = a.out + ((size_t)b * a.L + l) * a.N + nbase;
-        if (pv) {
-          if (nbase + 64 <= a.N && (a.N & 3) == 0) {
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              float4 v = make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]);
-              if (a.bias) {
-                const float4 bb = __ldg(reinterpret_cast<const float4*>(a.bias + nbase) + j);
-                v.x += bb.x; v.y += bb.y; v.z += bb.z; v.w += bb.w;
-              }
-              reinterpret_cast<float4*>(dst)[j] = v;
-            }
-          } else {
+        for (int i = 0; i < 64; ++i) sum[i] += acc[i];
+      }
+    }
+    // epilogue: element i of the fragment = (row r0 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 t + (i & 1))
 #pragma unroll
-            for (int j = 0; j < 64; ++j)
-              if (nbase + j < a.N) dst[j] = acc[j] + (a.bias ? __ldg(a.bias + nbase + j) : 0.f);
+    for (int h = 0; h < 2; ++h) {
+      const int l = lt + r0 + 8 * h;
+      if (l >= lend) continue;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int n = nt * NT + 8 * j + 2 * t;
+        float v0 = sum[4 * j + 2 * h], v1 = sum[4 * j + 2 * h + 1];
+        if constexpr (OUT == OUT_CH) {
+          float* dst = a.out + ((size_t)b * a.N + n) * a.L + l;
+          if (n < a.N) dst[0] = v0 + (a.bias ? __ldg(a.bias + n) : 0.f);
+          if (n + 1 < a.N) dst[a.L] = v1 + (a.bias ? __ldg(a.bias + n + 1) : 0.f);
+        } else {
+          float* dst = a.out + ((size_t)b * a.L + l) * a.N + n;
+          if (a.bias) {
+            if (n < a.N) v0 += __ldg(a.bias + n);
+            if (n + 1 < a.N) v1 += __ldg(a.bias + n + 1);
+          }
+          if (n + 1 < a.N && (a.N & 1) == 0) *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
+          else {
+            if (n < a.N) dst[0] = v0;
+            if (n + 1 < a.N) dst[1] = v1;
           }
         }
       }
     }
-    if (dbg_on && warp == 4 && lane == 0) a.dbg[9] = dbg_t[0];
-  }
-
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 9) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(C::TMEM_COLS) : "memory");
   }
 }
 
@@ -500,25 +296,23 @@ __global__ void __launch_bounds__(kThreads, 1) proj_gemm_kernel(const Args a, co
 // ================================================================================================ weight gradients
 // dW[m][n] = sum_{b,pos} X[b][m][pos] * Y[b][pos][n]: the reduction runs over the (up to 2^20) sequence positions.
 // Computed as its transpose, T[n][m] = sum_pos Y[pos][n] X[m][pos], so that both operands sit in their natural layout
-// (a probe on the B200, tools/ubench/mma_mn.cu, showed the MN-major shared-memory descriptor of kind::tf32 returning
-// zeros with either LBO/SBO assignment, so no transposed operand is used):
-//   A operand = Y^T: 128 columns n of Y per tile = TMEM lanes; thread n reads Y[pos][n] of 32 staged positions
-//               (consecutive threads = consecutive n: conflict free), (hi, lo) split, tcgen05.st
+// (wgmma takes tf32 operands K-major only):
+//   A operand = Y^T: 128 columns n of Y per tile, two consumer warpgroups of 64; each thread loads its A fragments
+//               (Y[pos][n] of the staged chunk), (hi, lo) split in registers
 //   B operand = X:   128 rows m per tile, K = position contiguous in memory = K-major; four converter warps turn the
 //               staged rows into hi / lo K-major core-matrix images (one 16-byte piece = four consecutive positions of
 //               one row; optional transposed short filter on the fly from six staged samples)
-//   staging   both chunks arrive by cp.async into shared-memory rings, three chunks in flight
+//   staging   both tiles of a chunk arrive by TMA into shared-memory rings, four chunks in flight
 //   split-K   CTA = (n tile, m tile, slice of the position chunks), one partial per CTA, summed in fixed order by
 //             wgrad_reduce_kernel (deterministic, no atomics).
 //   accuracy  the tensor core adds into its accumulator with truncation: a chain of n MMAs biases the sum by ~n 2^-24
-//             towards zero, and a slice here is ~8000 MMAs long (measured: four digits lost).  So (i) the hi*hi products
-//             go to a MAIN accumulator that is restarted every kSeg chunks (two TMEM buffers in turn) and drained by four
-//             extra warps into the CTA's partial in L2 with round-to-nearest adds, (ii) the lo*hi + hi*lo products go to a
-//             separate CORRECTION accumulator, 2^-11 times smaller, whose own bias is negligible over the whole slice.
+//             towards zero, and a slice here is thousands of MMAs long.  So the accumulator is restarted every kSeg chunks
+//             (the correction products of a chunk first, its hi*hi products last) and added into the CTA's partial in
+//             L2 with round-to-nearest adds.
 namespace wg {
 
-constexpr int kThreads = 448;             // warps 0-3 Y -> A conversion, 4-7 X -> B images, 8 MMA, 9-12 drain, 13 TMA producer
-constexpr int kSeg = 8;                   // chunks per accumulation segment (32 chained main MMAs)
+constexpr int kThreads = 416;             // warps 0-7 two consumer warpgroups, 8-11 X -> B images, 12 TMA producer
+constexpr int kSeg = 4;                   // chunks per accumulation segment (48 chained MMAs)
 constexpr int kStg = 4;                   // staged chunks in flight
 constexpr uint32_t kYPitch = 128 * 4;     // staged Y row: 128 columns, dense (= the TMA box)
 constexpr uint32_t kYStage = 32 * kYPitch;            // 32 positions
@@ -537,7 +331,6 @@ struct Args {
   const float* X;       // (B, M, L)
   const float* Y;       // (B, L, N)
   const float* fir;     // (M, 3) or null
-  long long* dbg;       // optional per-role cycle counters of CTA 0 (tools/dbg_proj_timing.py), or null
   float* part;          // (splits, N, M) partial sums of the TRANSPOSED product
   int B, L, M, N;
   int chunks_per_b;     // ceil(L / 32)
@@ -548,113 +341,107 @@ struct Args {
 
 // Staging: one producer thread issues, per chunk of 32 positions, ONE tiled TMA copy of the Y tile (box 128 n x 32 pos of
 // the (N, L, B) tensor) and one of the X tile (box 36 pos x 128 m of the (L, M, B) tensor; four look-ahead samples for
-// the fused FIR), four chunks in flight, completion on an mbarrier per stage.  Out-of-range rows / columns / positions
-// are zero-filled by the copy engine (tails of M, N and L; the 3-D maps keep a tile from running into the next batch).
-// Round 2 measured why: staged with per-thread cp.async the kernel sat at ~3100 cycles per chunk for 800 of MMA, both
-// staging loops waiting ~900 cycles just to ISSUE their copies (the SM's outstanding-miss tracking was full);
-// bulk tensor copies do not go through it.
+// the fused FIR), completion on an mbarrier per stage.  Out-of-range rows / columns / positions are zero-filled by the
+// copy engine (tails of M, N and L; the 3-D maps keep a tile from running into the next batch).
 __global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const Args a, const __grid_constant__ CUtensorMap tmapX,
                                                             const __grid_constant__ CUtensorMap tmapY) {
   extern __shared__ __align__(1024) unsigned char smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBar);
-  // barriers: b_full[2] b_empty[2] a_full[2] a_empty[2] dm_full[2] dm_empty[2] dc_full s_full[4] y_empty[4] x_empty[4]
-  uint32_t* tmem_p = reinterpret_cast<uint32_t*>(bars + 25);
+  // barriers: b_full[2] b_empty[2] s_full[4] y_empty[4] x_empty[4]
   const uint32_t sbase = tc::smem_u32(smem), bar0 = tc::smem_u32(bars);
   auto B_FULL = [&](int s) { return bar0 + 8u * s; };
   auto B_EMPTY = [&](int s) { return bar0 + 8u * (2 + s); };
-  auto A_FULL = [&](int j) { return bar0 + 8u * (4 + j); };
-  auto A_EMPTY = [&](int j) { return bar0 + 8u * (6 + j); };
-  auto DM_FULL = [&](int j) { return bar0 + 8u * (8 + j); };
-  auto DM_EMPTY = [&](int j) { return bar0 + 8u * (10 + j); };
-  const uint32_t DC_FULL = bar0 + 8u * 12;
-  auto S_FULL = [&](int j) { return bar0 + 8u * (13 + j); };
-  auto Y_EMPTY = [&](int j) { return bar0 + 8u * (17 + j); };
-  auto X_EMPTY = [&](int j) { return bar0 + 8u * (21 + j); };
+  auto S_FULL = [&](int j) { return bar0 + 8u * (4 + j); };
+  auto Y_EMPTY = [&](int j) { return bar0 + 8u * (8 + j); };
+  auto X_EMPTY = [&](int j) { return bar0 + 8u * (12 + j); };
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  // tensor memory map (columns): main accumulators [0,128) [128,256), correction accumulator [256,384), A chunks [384,512)
-  constexpr uint32_t kColDC = 256, kColA = 384;
 
-  if (warp == 8) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc::smem_u32(tmem_p)), "r"(512)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   if (tid == 0) {
-    for (int s = 0; s < 2; ++s) {
-      tc::mbar_init(B_FULL(s), 128); tc::mbar_init(B_EMPTY(s), 1);
-      tc::mbar_init(A_FULL(s), 128); tc::mbar_init(A_EMPTY(s), 1);
-      tc::mbar_init(DM_FULL(s), 1); tc::mbar_init(DM_EMPTY(s), 128);
-    }
-    tc::mbar_init(DC_FULL, 1);
-    for (int j = 0; j < kStg; ++j) { tc::mbar_init(S_FULL(j), 1); tc::mbar_init(Y_EMPTY(j), 128); tc::mbar_init(X_EMPTY(j), 128); }
+    for (int s = 0; s < 2; ++s) { tc::mbar_init(B_FULL(s), 128); tc::mbar_init(B_EMPTY(s), 8); }
+    for (int j = 0; j < kStg; ++j) { tc::mbar_init(S_FULL(j), 1); tc::mbar_init(Y_EMPTY(j), 256); tc::mbar_init(X_EMPTY(j), 128); }
   }
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = *tmem_p;
-
-  const bool dbg_on = a.dbg != nullptr && blockIdx.x == 0;
-  long long dbg_t[4] = {0, 0, 0, 0};
-  auto timed_wait = [&](uint32_t bar, uint32_t parity, int slot) {
-    if (dbg_on) { const long long t0 = clock64(); tc::mbar_wait_u(bar, parity); dbg_t[slot] += clock64() - t0; }
-    else tc::mbar_wait_u(bar, parity);
-  };
-  const long long dbg_start = clock64();
 
   // work item of this CTA
   const int split = blockIdx.x % a.splits;
   const int tile = blockIdx.x / a.splits;
   const int nt = tile / a.mtiles, mt = tile - nt * a.mtiles;
   const int n0 = nt * 128, m0 = mt * 128;
-  const int nrows = min(128, a.N - n0);                                 // valid accumulator rows (TMEM lanes)
+  const int nrows = min(128, a.N - n0);                                 // valid accumulator rows
   const int mcols = min(128, a.M - m0);                                 // valid accumulator columns
   const long long total_chunks = (long long)a.B * a.chunks_per_b;
   const long long c_begin = total_chunks * split / a.splits, c_end = total_chunks * (split + 1) / a.splits;
   const long long nchunks = c_end - c_begin;
 
-  if (warp < 4) {
-    // ---------------------------------------------------------------- A side: thread = column n of Y = TMEM lane
-    const uint32_t lane_addr = tmem + ((uint32_t)(32 * warp) << 16);
+  if (warp < 8) {
+    // ---------------------------------------------------------------- consumers: rows n [64 wg, 64 wg + 64) of the tile
+    const int wgi = warp >> 2, g = lane >> 2, t = lane & 3;
+    const int nl0 = 64 * wgi + 16 * (warp & 3) + g;                     // fragment rows nl0, nl0 + 8
+    float acc[64];
+    auto drain = [&](bool first) {                                      // partial += acc (round-to-nearest adds)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int nl = nl0 + 8 * h;
+        if (nl >= nrows) continue;
+        float* dst = a.part + ((size_t)split * a.N + n0 + nl) * a.M + m0;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int ml = 8 * j + 2 * t;
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+            if (ml + e < mcols) dst[ml + e] = acc[4 * j + 2 * h + e] + (first ? 0.f : dst[ml + e]);
+        }
+      }
+    };
+    if (nchunks == 0) {
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+      drain(true);
+    }
     for (long long q = 0; q < nchunks; ++q) {
       const int ss = (int)(q % kStg);
-      {
-        const long long tS = dbg_on ? clock64() : 0;
-        tc::mbar_wait_u(S_FULL(ss), (uint32_t)(q / kStg) & 1u);         // the producer's copies of this chunk have landed
-        if (dbg_on) dbg_t[1] += clock64() - tS;
-      }
-      const long long tC = dbg_on ? clock64() : 0;
+      tc::mbar_wait_u(S_FULL(ss), (uint32_t)(q / kStg) & 1u);            // the producer's copies of this chunk have landed
       const unsigned char* st = smem + kOffY + (size_t)ss * kYStage;
-      uint32_t hi[32], lo[32];
+      uint32_t ahi[4][4], alo[4][4];
+      uint32_t dep = 0;
 #pragma unroll
-      for (int k = 0; k < 32; ++k) {
-        const float v = *reinterpret_cast<const float*>(st + k * kYPitch + tid * 4);
-        float h, lw;
-        tc::split_tf32(v, h, lw);
-        hi[k] = __float_as_uint(h); lo[k] = __float_as_uint(lw);
-      }
-      {                                                                 // staged tile consumed (loads returned): the producer may
-        uint32_t dep = 0;                                               // refill the slot
+      for (int ks = 0; ks < 4; ++ks) {
 #pragma unroll
-        for (int k = 0; k < 32; ++k) dep |= hi[k];
-        tc::mbar_arrive_after_loads(Y_EMPTY(ss), dep, a.zero);
+        for (int e = 0; e < 4; ++e) {
+          const int nl = nl0 + ((e & 1) ? 8 : 0), k = 8 * ks + t + ((e & 2) ? 4 : 0);
+          const float v = *reinterpret_cast<const float*>(st + k * kYPitch + nl * 4);
+          dep |= __float_as_uint(v);
+          float h, lw;
+          tc::split_tf32(v, h, lw);
+          ahi[ks][e] = __float_as_uint(h); alo[ks][e] = __float_as_uint(lw);
+        }
       }
+      tc::mbar_arrive_after_loads(Y_EMPTY(ss), dep, a.zero);            // staged Y tile consumed: the producer may refill it
       const uint32_t it = (uint32_t)q;
-      const int buf = it & 1;
-      if (dbg_on) dbg_t[2] += clock64() - tC;
-      timed_wait(A_EMPTY(buf), ((it >> 1) & 1) ^ 1, 0);
-      tc::fence_after_sync();
-      const uint32_t acol = kColA + buf * 64;
-      tc::tmem_st32(lane_addr + acol, hi);
-      tc::tmem_st32(lane_addr + acol + 32, lo);
-      tc::tmem_wait_st();
-      tc::fence_before_sync();
-      tc::mbar_arrive(A_FULL(buf));
+      const int s = it & 1;
+      tc::mbar_wait_u(B_FULL(s), (it >> 1) & 1);
+      const uint32_t bhi = sbase + kOffImg + s * 2 * kImg, blo = bhi + kImg;
+      const uint32_t cont = (it % kSeg) != 0;                           // 0: this chunk starts a segment
+      tc::wgmma_fence();
+      tc::fence_regs(acc);
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {                                  // corrections: lo * hi, hi * lo
+        tc::wgmma_rs_n128(acc, alo[ks], tc::make_desc_ls(bhi + ks * 2 * pg::kLBO, pg::kLBO, pg::kSBO), (cont | ks) ? 1u : 0u);
+        tc::wgmma_rs_n128(acc, ahi[ks], tc::make_desc_ls(blo + ks * 2 * pg::kLBO, pg::kLBO, pg::kSBO), 1u);
+      }
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks)                                    // main: hi * hi
+        tc::wgmma_rs_n128(acc, ahi[ks], tc::make_desc_ls(bhi + ks * 2 * pg::kLBO, pg::kLBO, pg::kSBO), 1u);
+      tc::wgmma_commit();
+      tc::wgmma_wait<0>();
+      tc::fence_regs(acc);
+      __syncwarp();
+      if (lane == 0) tc::mbar_arrive(B_EMPTY(s));                       // the image pair is free
+      if (it % kSeg == kSeg - 1 || q + 1 == nchunks) drain(it < kSeg);
     }
-    if (dbg_on && tid == 0) { a.dbg[0] = dbg_t[0]; a.dbg[1] = dbg_t[1]; a.dbg[2] = dbg_t[2]; a.dbg[15] = nchunks;
-                              a.dbg[14] = clock64() - dbg_start; }
-  } else if (warp < 8) {
+  } else if (warp < 12) {
     // ---------------------------------------------------------------- B side: X rows -> K-major hi / lo images
-    const int t = tid - 128;
+    const int t = tid - 256;
     const bool use_fir = a.fir != nullptr;
     // this thread converts pieces (row r, quad k4) with r % 8 == t % 8: the eight lanes of a quarter warp then write one
     // contiguous 128-byte core matrix (bank-conflict free); 1024 pieces per chunk, 8 per thread
@@ -670,16 +457,11 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const Args a, const 
     }
     for (long long q = 0; q < nchunks; ++q) {
       const int ss = (int)(q % kStg);
-      {
-        const long long tS = dbg_on ? clock64() : 0;
-        tc::mbar_wait_u(S_FULL(ss), (uint32_t)(q / kStg) & 1u);
-        if (dbg_on) dbg_t[1] += clock64() - tS;
-      }
+      tc::mbar_wait_u(S_FULL(ss), (uint32_t)(q / kStg) & 1u);
       const unsigned char* st = smem + kOffX + (size_t)ss * kXStage;
       const uint32_t it = (uint32_t)q;
       const int s = it & 1;
-      timed_wait(B_EMPTY(s), ((it >> 1) & 1) ^ 1, 0);                   // the MMAs that read this image pair are done
-      const long long tV = dbg_on ? clock64() : 0;
+      tc::mbar_wait_u(B_EMPTY(s), ((it >> 1) & 1) ^ 1);                 // the MMAs that read this image pair are done
       unsigned char* hi_img = smem + kOffImg + (size_t)s * 2 * kImg;
       unsigned char* lo_img = hi_img + kImg;
 #pragma unroll
@@ -707,46 +489,8 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const Args a, const 
       tc::mbar_arrive(X_EMPTY(ss));                                     // staged rows consumed
       tc::fence_async_smem();
       tc::mbar_arrive(B_FULL(s));
-      if (dbg_on) dbg_t[2] += clock64() - tV;
     }
-    if (dbg_on && t == 0) { a.dbg[3] = dbg_t[0]; a.dbg[4] = dbg_t[1]; a.dbg[5] = dbg_t[2]; }
   } else {
-    // ---------------------------------------------------------------- MMA issuer
-    if (warp == 8 && lane == 0) {
-      constexpr uint32_t idesc = tc::make_idesc(128);
-      for (long long q = 0; q < nchunks; ++q) {
-        const uint32_t it = (uint32_t)q;
-        const int s = it & 1;
-        const uint32_t seg = it / kSeg, sb = seg & 1;
-        if (it % kSeg == 0) {                                           // new segment: its main accumulator must be drained
-          timed_wait(DM_EMPTY(sb), ((seg >> 1) & 1) ^ 1, 0);
-          tc::fence_after_sync();
-        }
-        timed_wait(B_FULL(s), (it >> 1) & 1, 1);
-        timed_wait(A_FULL(s), (it >> 1) & 1, 2);
-        tc::fence_after_sync();
-        const uint32_t bhi = sbase + kOffImg + s * 2 * kImg, blo = bhi + kImg;
-        const uint32_t ahi = tmem + kColA + s * 64, alo = ahi + 32;
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks)                                  // main: hi * hi
-          tc::mma_tf32_ts(tmem + sb * 128, ahi + 8 * ks, tc::make_desc_ls(bhi + ks * 2 * pg::kLBO, pg::kLBO, pg::kSBO), idesc,
-                          ((it % kSeg) | ks) ? 1u : 0u);
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks)                                  // correction: lo * hi
-          tc::mma_tf32_ts(tmem + kColDC, alo + 8 * ks, tc::make_desc_ls(bhi + ks * 2 * pg::kLBO, pg::kLBO, pg::kSBO), idesc,
-                          (it | ks) ? 1u : 0u);
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks)                                  //             hi * lo
-          tc::mma_tf32_ts(tmem + kColDC, ahi + 8 * ks, tc::make_desc_ls(blo + ks * 2 * pg::kLBO, pg::kLBO, pg::kSBO), idesc, 1u);
-        tc::mma_commit(A_EMPTY(s));
-        tc::mma_commit(B_EMPTY(s));
-        if (it % kSeg == kSeg - 1 || q + 1 == nchunks) tc::mma_commit(DM_FULL(sb));
-      }
-      if (nchunks > 0) tc::mma_commit(DC_FULL);
-      if (dbg_on) { a.dbg[6] = dbg_t[0]; a.dbg[7] = dbg_t[1]; a.dbg[8] = dbg_t[2]; a.dbg[9] = clock64() - dbg_start; }
-    }
-  }
-  if (warp == 13) {
     // ---------------------------------------------------------------- producer: Y and X tiles of every chunk (TMA)
     if (lane == 0 && a.vec) { tc::tma_prefetch_desc(&tmapX); tc::tma_prefetch_desc(&tmapY); }
     int sb_ = (int)(c_begin / a.chunks_per_b), sl_ = (int)(c_begin - (long long)sb_ * a.chunks_per_b) * 32;
@@ -780,65 +524,6 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const Args a, const 
         if (lane == 0) tc::mbar_arrive(S_FULL(ss));
       }
     }
-  } else if (warp >= 9) {
-    // ---------------------------------------------------------------- drain warps: thread = accumulator row (TMEM lane)
-    const int w4 = warp - 9, row = 32 * w4 + lane;                      // warps 9..12 -> lane quadrants 1,2,3,0
-    const int lq = warp & 3;
-    const int n = 32 * lq + lane;                                       // accumulator row of this thread
-    (void)w4; (void)row;
-    const uint32_t lane_addr = tmem + ((uint32_t)(32 * lq) << 16);
-    const bool nv = n < nrows;
-    float* dst = a.part + ((size_t)split * a.N + (nv ? n0 + n : 0)) * a.M + m0;
-    const bool v4 = ((a.M & 3) == 0) && (mcols == 128);
-    const uint32_t nseg = (uint32_t)((nchunks + kSeg - 1) / kSeg);
-    auto add_cols = [&](uint32_t col0, bool first) {
-#pragma unroll 1
-      for (int c0 = 0; c0 < 128; c0 += 32) {
-        uint32_t r[32];
-        tc::tmem_ld32_nowait(lane_addr + col0 + c0, r);
-        tc::tmem_wait_ld();
-        if (!nv) continue;
-        if (v4) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            float4 v = make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]), __uint_as_float(r[4 * j + 2]),
-                                   __uint_as_float(r[4 * j + 3]));
-            float4* pd = reinterpret_cast<float4*>(dst + c0) + j;
-            if (!first) { const float4 o = *pd; v.x += o.x; v.y += o.y; v.z += o.z; v.w += o.w; }
-            *pd = v;
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (c0 + j < mcols) dst[c0 + j] = __uint_as_float(r[j]) + (first ? 0.f : dst[c0 + j]);
-        }
-      }
-    };
-    if (nchunks == 0) {
-      if (nv)
-        for (int c = 0; c < mcols; ++c) dst[c] = 0.f;
-    } else {
-      for (uint32_t seg = 0; seg < nseg; ++seg) {
-        const int sb = seg & 1;
-        timed_wait(DM_FULL(sb), (seg >> 1) & 1, 0);
-        tc::fence_after_sync();
-        const long long tD = dbg_on ? clock64() : 0;
-        add_cols(sb * 128, seg == 0);
-        tc::fence_before_sync();
-        tc::mbar_arrive(DM_EMPTY(sb));
-        if (dbg_on) dbg_t[1] += clock64() - tD;
-      }
-      tc::mbar_wait_u(DC_FULL, 0);
-      tc::fence_after_sync();
-      add_cols(kColDC, false);
-      tc::fence_before_sync();
-      if (dbg_on && warp == 9 && lane == 0) { a.dbg[10] = dbg_t[0]; a.dbg[11] = dbg_t[1]; }
-    }
-  }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 8) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512) : "memory");
   }
 }
 

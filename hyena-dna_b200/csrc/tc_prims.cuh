@@ -1,4 +1,4 @@
-// tcgen05 / TMEM / mbarrier / bulk-copy PTX wrappers shared by the tensor-core kernels (filter_tc.cuh, proj_gemm.cuh).
+// wgmma / mbarrier / TMA PTX wrappers shared by the tensor-core kernels (filter_tc.cuh, proj_gemm.cuh), sm_90a.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -7,8 +7,7 @@ namespace hy {
 namespace tc {
 
 // Round-to-nearest (ties away) to tf32 by integer arithmetic: add half an ulp of the 10-bit mantissa, clear the 13 low
-// bits.  Same result as cvt.rna.tf32.f32 for finite inputs (Inf stays Inf, NaN stays NaN); ptxas expands that PTX
-// instruction into five SASS instructions (add, |x| < Inf test, select, mask), this is two.
+// bits.  Same result as cvt.rna.tf32.f32 for finite inputs (Inf stays Inf, NaN stays NaN) in two instructions.
 __device__ __forceinline__ float to_tf32(float x) {
   return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
 }
@@ -20,131 +19,95 @@ __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
 // ---------------------------------------------------------------------------------------------- PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// shared-memory matrix descriptor, no swizzle: start address, leading byte offset, stride byte offset (16-byte units)
+// wgmma shared-memory matrix descriptor, no swizzle (canonical K-major core-matrix layout: 8 rows x 16 bytes per core
+// matrix): start address, leading byte offset (next core matrix along K), stride byte offset (next 8-row group)
 __device__ __forceinline__ uint64_t make_desc_ls(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);            // start address, 16-byte units, bits [0,14)
   d |= (uint64_t)(lbo >> 4) << 16;                     // leading byte offset, bits [16,30)
   d |= (uint64_t)(sbo >> 4) << 32;                     // stride byte offset, bits [32,46)
-  d |= (uint64_t)1 << 46;                              // descriptor version 1 (Blackwell)
   return d;                                            // base_offset 0, layout_type 0 (no swizzle)
 }
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr) { return make_desc_ls(saddr, 128u, 2048u); }
-// kind::tf32, fp32 accumulate, A and B K-major, M = 128
-__host__ __device__ constexpr uint32_t make_idesc(int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
+
+// ---------------------------------------------------------------------------------------------- wgmma
+// All wrappers are warpgroup-wide (.sync.aligned): every thread of the 128-thread warpgroup executes them.
+// D (64 x N, fp32) += A (64 x 8, tf32) * B^T (N x 8, tf32); A from shared memory (ss) or registers (rs), B from shared
+// memory, both K-major.  Accumulator fragment of thread (warp w of the warpgroup, lane = 4 g + t), n8 block j:
+//   d[4j] = (16w + g, 8j + 2t)   d[4j+1] = (16w + g, 8j + 2t + 1)   d[4j+2] = (16w + g + 8, 8j + 2t)   d[4j+3] = (.. + 8, .. + 1)
+// Register A fragment (rs), k8 block:  a[0] = (16w + g, t)  a[1] = (16w + g + 8, t)  a[2] = (16w + g, t + 4)  a[3] = (16w + g + 8, t + 4)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of accumulator registers across wgmma issue / wait points
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// same with the B operand MN-major (bit 16) and/or the A operand MN-major (bit 15)
-__host__ __device__ constexpr uint32_t make_idesc_major(int N, bool a_mn, bool b_mn) {
-  return make_idesc(N) | (a_mn ? (1u << 15) : 0u) | (b_mn ? (1u << 16) : 0u);
-}
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
+
+__device__ __forceinline__ void wgmma_ss_n8(float (&d)[4], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n8k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3}, %4, %5, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
-__device__ __forceinline__ void mma_commit(uint32_t mbar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(mbar) : "memory");
+__device__ __forceinline__ void wgmma_ss_n32(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
+__device__ __forceinline__ void wgmma_ss_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_ss_n72(float (&d)[36], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %38, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n72k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35}, %36, %37, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_rs_n128(float (&d)[64], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+
+// overloads by accumulator size (N / 2 registers per thread)
+__device__ __forceinline__ void wgmma_ss(float (&d)[4], uint64_t da, uint64_t db, uint32_t sc) { wgmma_ss_n8(d, da, db, sc); }
+__device__ __forceinline__ void wgmma_ss(float (&d)[16], uint64_t da, uint64_t db, uint32_t sc) { wgmma_ss_n32(d, da, db, sc); }
+__device__ __forceinline__ void wgmma_ss(float (&d)[32], uint64_t da, uint64_t db, uint32_t sc) { wgmma_ss_n64(d, da, db, sc); }
+__device__ __forceinline__ void wgmma_ss(float (&d)[36], uint64_t da, uint64_t db, uint32_t sc) { wgmma_ss_n72(d, da, db, sc); }
+
+// ---------------------------------------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint32_t mbar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(mbar), "r"(count) : "memory");
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-__device__ __forceinline__ void mbar_wait(uint32_t mbar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred P1;\n\t"
-      "LAB_WAIT:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t"
-      "@P1 bra DONE;\n\t"
-      "bra LAB_WAIT;\n\t"
-      "DONE:\n\t}\n"
-      ::"r"(mbar), "r"(parity)
-      : "memory");
-}
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-// 32 consecutive accumulator columns of this thread's TMEM lane
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// ---------------------------------------------------------------------------------------------- more wrappers
-// A operand in tensor memory (lane = row, one 32-bit column per tf32 element), B from shared memory
-__device__ __forceinline__ void mma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(db), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// 32 consecutive columns of this thread's TMEM lane <- registers
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};\n"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-        "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-        "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// tcgen05.ld without the wait (callers batch several loads, then tmem_wait_ld once)
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 __device__ __forceinline__ void mbar_arrive(uint32_t mbar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(mbar) : "memory");
 }
 // Release of a shared-memory slot whose contents this thread has just LOADED into registers: the arrive must not be performed
 // before those loads have returned.  A plain arrive is issued right behind the LDS instructions (no register dependency) and is
-// handled by the barrier unit, not queued behind them in the load pipe -- measured: with the refilling TMA copy issued as soon
-// as the barrier completes, ~1e-6 of the runs read rows the copy engine had already overwritten (tools/determinism_proj.py).
-// `dep` must be computed from every loaded register; `zero` is a run-time 0 the assembler cannot fold, so the arrive count
-// (always 1) carries a true data dependency on the loads.
+// handled by the barrier unit, not queued behind them in the load pipe, so a refilling TMA copy issued as soon as the barrier
+// completes could overwrite rows that are still being read.  `dep` must be computed from every loaded register; `zero` is a
+// run-time 0 the assembler cannot fold, so the arrive count (always 1) carries a true data dependency on the loads.
 __device__ __forceinline__ void mbar_arrive_after_loads(uint32_t mbar, uint32_t dep, uint32_t zero) {
   const uint32_t cnt = 1u + (dep & zero);
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" ::"r"(mbar), "r"(cnt) : "memory");
@@ -152,14 +115,14 @@ __device__ __forceinline__ void mbar_arrive_after_loads(uint32_t mbar, uint32_t 
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t mbar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mbar), "r"(bytes) : "memory");
 }
-// TMA bulk copy (no tensor map): global -> shared, completion on an mbarrier (SASS: UBLKCP)
+// TMA bulk copy (no tensor map): global -> shared, completion on an mbarrier
 __device__ __forceinline__ void bulk_g2s(uint32_t smem_dst, const void* gsrc, uint32_t bytes, uint32_t mbar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(smem_dst), "l"(gsrc), "r"(bytes), "r"(mbar)
                : "memory");
 }
 // TMA tiled copy through a tensor map (cuTensorMapEncodeTiled): box at coordinates (c0 fastest, c1) -> shared memory,
-// completion on an mbarrier (SASS: UTMALDG).  `tmap` must live in param / const / global space (__grid_constant__).
+// completion on an mbarrier.  `tmap` must live in param / const / global space (__grid_constant__).
 __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const void* tmap, int c0, int c1, uint32_t mbar) {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                ::"r"(smem_dst), "l"(tmap), "r"(mbar), "r"(c0), "r"(c1)
@@ -175,22 +138,11 @@ __device__ __forceinline__ void tma_prefetch_desc(const void* tmap) {
 }
 
 // wait (no PTX labels: may be inlined any number of times); traps after ~2 s of waiting instead of hanging the GPU --
-// a protocol bug then surfaces as a launch failure.  No suspend-time hint: with the 10 ms hint round 1 used, ptxas emits
-// SYNCS.PHASECHK + NANOSLEEP 0x989680 and the sleeping warp wakes late -- ncu put 16-32 % of all stall samples of the
-// projection kernels on that NANOSLEEP (profiles/r2_ncu_proj_staged_stalls.txt)
+// a protocol bug then surfaces as a launch failure.
 __device__ __forceinline__ void mbar_wait_u(uint32_t mbar, uint32_t parity) {
   uint32_t done = 0;
   const long long t0 = clock64();
   while (!done) {
-#if defined(HY_WAIT_HINT_NS) && HY_WAIT_HINT_NS > 0
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}\n"
-        : "=r"(done)
-        : "r"(mbar), "r"(parity), "r"((uint32_t)HY_WAIT_HINT_NS)
-        : "memory");
-#else
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
         "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
@@ -198,7 +150,6 @@ __device__ __forceinline__ void mbar_wait_u(uint32_t mbar, uint32_t parity) {
         : "=r"(done)
         : "r"(mbar), "r"(parity)
         : "memory");
-#endif
     if (!done && clock64() - t0 > 4000000000LL) __trap();
   }
 }

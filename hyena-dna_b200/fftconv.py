@@ -1,4 +1,4 @@
-"""The reference's long-convolution op surface on top of the sm_100a library.
+"""The reference's long-convolution op surface on top of the sm_90a library.
 
 Mirrors /root/reference/src/ops/fftconv.py (``fftconv_func``, ``FFTConvFunc``) and the pybind
 module ``fftconv`` it imports (csrc/fftconv/fftconv.cpp:238-241: ``fftconv_fwd`` / ``fftconv_bwd``),
@@ -15,7 +15,7 @@ from ._lib import HyenaB200Error
 def _reject(**flags):
     bad = [k for k, v in flags.items() if v]
     if bad:
-        raise HyenaB200Error(f"fftconv options not supported by the sm_100a hot path (no fallback): {bad}")
+        raise HyenaB200Error(f"fftconv options not supported by the sm_90a hot path (no fallback): {bad}")
 
 
 def _is_packed(filter, H, L):
@@ -172,7 +172,7 @@ def fftconv_func(u, k, D, dropout_mask=None, gelu=True, force_fp16_output=False,
 
 
 def fftconv_ref(u, k, D, dropout_mask=None, gelu=True, k_rev=None, bidirectional=False):
-    """Same call as the reference's ``fftconv_ref`` (src/models/sequence/hyena.py:59-88) on the sm_100a kernels.
+    """Same call as the reference's ``fftconv_ref`` (src/models/sequence/hyena.py:59-88) on the sm_90a kernels.
 
     ``bidirectional`` there pads the input by ~L/2 on both sides -- to exactly the 2L points of the transform, so nothing is
     left to absorb the wrap-around (:67-73) -- and convolves cyclically with the L-tap filter:

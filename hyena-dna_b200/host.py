@@ -22,9 +22,9 @@ from ._lib import HyenaB200Error
 
 class HostStep:
     def __init__(self, op, batch, seqlen, chunks=4):
-        self.tc = ops.proj_mode() == "tc"               # own tcgen05 projections (default) or cuBLASLt slices
+        self.tc = ops.proj_mode() == "tc"               # own wgmma projections (default) or cuBLASLt slices
         if not self.tc and ops.gemm_mode() != "bf16x9":
-            raise HyenaB200Error("HostStep needs the tcgen05 projections or the cuBLASLt 12.9 projection path")
+            raise HyenaB200Error("HostStep needs the wgmma projections or the cuBLASLt 12.9 projection path")
         self.op = op
         dev = op.in_proj.weight.device
         self.dev = dev

@@ -1,4 +1,4 @@
-"""Drop-in HyenaOperator / HyenaFilter backed by the sm_100a library.
+"""Drop-in HyenaOperator / HyenaFilter backed by the sm_90a library.
 
 Mirrors the public surface of /root/reference/src/models/sequence/hyena.py (same class names,
 constructor keywords, state_dict keys and shapes, ``_optim`` attributes, ``filter(L)`` /
@@ -88,7 +88,7 @@ class HyenaFilter(OptimModule):
         super().__init__()
         if linear_mixer or num_inner_mlps != 2 or dropout != 0.0:
             raise HyenaB200Error("HyenaFilter: linear_mixer / num_inner_mlps != 2 / "
-                                 "dropout are outside the sm_100a hot path (no fallback)")
+                                 "dropout are outside the sm_90a hot path (no fallback)")
         if order != 64:
             raise HyenaB200Error(f"HyenaFilter: filter order {order} not supported by the fused kernel (64 only)")
         assert emb_dim % 2 != 0 and emb_dim >= 3, "emb_dim must be odd and greater or equal to 3 (time, sine and cosine)"
@@ -297,7 +297,7 @@ class _OutProj(torch.autograd.Function):
 
 
 class HyenaOperator(nn.Module):
-    """Hyena operator (hyena.py:270-448): order 2 as one fused pass on sm_100a, order >= 3 as a chain of its kernels.
+    """Hyena operator (hyena.py:270-448): order 2 as one fused pass on sm_90a, order >= 3 as a chain of its kernels.
 
     forward(u: (B, L, D)) -> (B, L, D) (or ``(y, None)`` when return_state).  Unknown keyword arguments
     (layer_idx, device, dtype, ...) fall through to the filter exactly as in the reference."""
@@ -315,7 +315,7 @@ class HyenaOperator(nn.Module):
                        "filter_cls": filter_cls != "hyena-filter", "fused_bias_fc": fused_bias_fc}
         bad = [k for k, v in unsupported.items() if v]
         if bad:
-            raise HyenaB200Error(f"HyenaOperator options outside the sm_100a hot path (no fallback): {bad}")
+            raise HyenaB200Error(f"HyenaOperator options outside the sm_90a hot path (no fallback): {bad}")
         self.d_model, self.l_max, self.order = d_model, l_max, order
         self.num_heads, self.inner_factor, self.num_blocks = num_heads, inner_factor, num_blocks
         self.block_dim, self.head_dim = l_max // num_blocks, d_model // num_heads
@@ -335,7 +335,7 @@ class HyenaOperator(nn.Module):
 
     def forward(self, u, *args, **kwargs):
         if not u.is_cuda:
-            raise HyenaB200Error("HyenaOperator (hyena_b200) runs on CUDA sm_100a only; there is no CPU fallback")
+            raise HyenaB200Error("HyenaOperator (hyena_b200) runs on CUDA sm_90a only; there is no CPU fallback")
         in_dtype = u.dtype
         u = u.to(torch.float32)
         l = u.size(-2)
@@ -372,7 +372,7 @@ class HyenaOperator(nn.Module):
     def _forward_chained(self, u, k, fb, l_filter):
         """order >= 3 (the shipped HyenaDNA layer default is 3, configs/model/layer/hyena_dna.yaml:3): the recurrence of
         hyena.py:414-423 as a chain of this library's long convolutions.  Projections and every FFT convolution
-        (forward and backward) run on the sm_100a kernels; the gates and the 3-tap short filter between them are
+        (forward and backward) run on the sm_90a kernels; the gates and the 3-tap short filter between them are
         plain elementwise / depthwise torch ops here -- the fully fused pass exists for order 2 only."""
         D, O1 = self.d_model, self.order - 1
         from .fftconv import fftconv_func

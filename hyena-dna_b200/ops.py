@@ -79,7 +79,7 @@ def filter_forward(z, t, W0, b0, W1, b1, W2, b2, W3, freq, deltas, shift, modula
 
 
 def _filter_backward_tc(z, t, W0, b0, W1, b1, W2, b2, W3, freq, deltas, shift, modulate, L, dk, need_dz):
-    """Tensor-core backward: stage 1 on tcgen05 (csrc/filter_tc.cuh), stage 2 = sequence-length reductions."""
+    """Tensor-core backward: stage 1 on wgmma (csrc/filter_tc.cuh), stage 2 = sequence-length reductions."""
     zz, tt, E, N, D = _filter_args(z, t, W0, b0, W1, b1, W2, b2, W3, freq, deltas, shift, modulate, L)
     ws = [x.contiguous() for x in (W0, b0, W1, b1, W2, b2, W3)]
     fr = freq.reshape(-1).contiguous()
@@ -346,7 +346,7 @@ class HyenaCoreFn(torch.autograd.Function):
 
 
 class HyenaInCoreFn(torch.autograd.Function):
-    """in_proj + operator core as ONE autograd node (tcgen05 projections): u (B, L, D) -> y_pre (B, D, L).
+    """in_proj + operator core as ONE autograd node (wgmma projections): u (B, L, D) -> y_pre (B, D, L).
 
     Forward: p = W u^T channel-major (proj_gemm), then the fused core.  Backward: the core returns ds (gradient w.r.t. the
     short-filter outputs) and the two projection-backward GEMMs apply the transposed 3-tap filter to it on the fly, so
@@ -457,7 +457,7 @@ _proj_mode = None
 
 
 def proj_mode():
-    """'tc': the projections run on this library's tcgen05 3xTF32 kernels (csrc/proj_gemm.cuh) -- the default;
+    """'tc': the projections run on this library's wgmma 3xTF32 kernels (csrc/proj_gemm.cuh) -- the default;
     'lt': cuBLASLt 12.9 BF16x9 (csrc/gemm.cu; also what runs when the user opted into TF32 via
     torch.backends.cuda.matmul.allow_tf32); 'torch': torch.bmm.  HYENA_B200_PROJ selects."""
     global _proj_mode
@@ -474,7 +474,7 @@ def proj_mode():
 
 
 def proj_gemm(act, act_layout, W, w_transposed, out_layout, bias=None, fir=None, out=None, l_range=None):
-    """OUT[pos][n] = sum_k ACT[pos][k] Wl[n][k] (+ bias) on this library's tcgen05 kernel (csrc/proj_gemm.cuh, 3xTF32).
+    """OUT[pos][n] = sum_k ACT[pos][k] Wl[n][k] (+ bias) on this library's wgmma kernel (csrc/proj_gemm.cuh, 3xTF32).
     act_layout 0: act (B, L, K); 1: act (B, K, L).  out_layout 0: (B, N, L); 1: (B, L, N).  Wl = W.T if w_transposed."""
     _need_cuda(act, W, bias, fir)
     if act.dim() != 3 or W.dim() != 2 or not act.is_contiguous() or not W.is_contiguous():
@@ -516,7 +516,7 @@ def fuse_fir():
 
 def proj_wgrad(X, Y, fir=None, transposed_out=False):
     """dW (M, N) [(N, M) if transposed_out] = sum_{b,pos} X[b][m][pos] Y[b][pos][n]; X (B, M, L), Y (B, L, N)
-    (csrc/proj_gemm.cuh wgrad_kernel: tcgen05 3xTF32, split-K, deterministic)."""
+    (csrc/proj_gemm.cuh wgrad_kernel: wgmma 3xTF32, split-K, deterministic)."""
     _need_cuda(X, Y, fir)
     if X.dim() != 3 or Y.dim() != 3 or not X.is_contiguous() or not Y.is_contiguous() or X.shape[0] != Y.shape[0] \
             or X.shape[2] != Y.shape[1]:
@@ -543,8 +543,7 @@ _side_streams = {}
 def side_stream(device):
     """A second stream per device for work that is independent of the main chain (weight-gradient GEMMs run there
     while the input-gradient GEMM runs on the caller's stream: one op's cuBLASLt input scan overlaps the other's
-    tensor-core phase).  Measured on B200 at L = 2^20: no gain (39.3 vs 38.8 ms/step; both GEMMs want the whole
-    chip), so it is OFF unless HYENA_B200_SIDE_STREAM=1."""
+    tensor-core phase).  Both GEMMs want the whole chip, so it is OFF unless HYENA_B200_SIDE_STREAM=1."""
     import os
     if os.environ.get("HYENA_B200_SIDE_STREAM", "0") != "1":
         return None

@@ -1,4 +1,4 @@
-/* hyena_b200 -- C ABI of the sm_100a Hyena long-convolution library (libhyena_b200.so).
+/* hyena_b200 -- C ABI of the sm_90a Hyena long-convolution library (libhyena_b200.so).
  *
  * This is the drop-in boundary for the HyenaOperator hot path of HazyResearch/hyena-dna.  The
  * reference's own FFI for this path is the pybind11 module `fftconv`
@@ -35,7 +35,8 @@
 extern "C" {
 #endif
 
-#define HYENA_B200_ABI_VERSION 1
+/* 2: hyena_b200_proj_debug_buffer removed (the wgmma projection kernels keep no per-role counters) */
+#define HYENA_B200_ABI_VERSION 2
 #if defined(__GNUC__)
 #define HY_API __attribute__((visibility("default")))
 #else
@@ -84,10 +85,10 @@ HY_API int hyena_b200_filter_bwd(const float* z, int z_stride, const float* t,
                           float* dW0, float* db0, float* dW1, float* db1, float* dW2, float* db2,
                           float* dW3, float* dfreq, float* dz, int dz_stride, void* stream);
 
-/* Tensor-core (tcgen05, 3xTF32) backward in two stages.  Stage 1: per position, recompute the activations and back-
+/* Tensor-core (wgmma, 3xTF32) backward in two stages.  Stage 1: per position, recompute the activations and back-
  * propagate through the MLP, writing dh = dk * modulation (D,L) and seven feature-major (64,L) arrays into `scratch`
  * (7*64*L floats, 16-byte aligned): a1, a2, a3, dp1, dp2, dp3, X.  Stage 2: the parameter gradients are reductions
- * over the sequence, done as accumulating tcgen05 GEMMs with K = position (all outputs (+=); zT is z transposed,
+ * over the sequence, done as accumulating wgmma GEMMs with K = position (all outputs (+=); zT is z transposed,
  * (E,L)); D <= 256, E <= 8:
  *   dW3 = dh a3^T, dW2 = dp3 a2^T, dW1 = dp2 a1^T, dW0 = dp1 z, db_l = rowsum(dp_{l+1}), dfreq = rowsum(X) */
 HY_API int hyena_b200_filter_bwd_stage1(const float* z, int z_stride, const float* t,
@@ -164,8 +165,8 @@ HY_API int hyena_b200_spectrum_to_rfft(const float* dk, int fft_size, float* dfi
 HY_API int hyena_b200_gemm_available(void);
 
 /* ---- projections on this library's own tensor-core kernel (csrc/proj_gemm.cuh) --------------------
- * The same GEMMs as above without the library call: tcgen05 / TMEM, fp32 accuracy through 3xTF32, weights streamed by
- * TMA bulk copies, the activation converted on the fly into tensor memory.  Computes, for every batch b,
+ * The same GEMMs as above without the library call: wgmma, fp32 accuracy through 3xTF32, weights streamed by
+ * TMA bulk copies, the activation converted on the fly into wgmma register fragments.  Computes, for every batch b,
  *     OUT[pos][n] = sum_k ACT[pos][k] * Wl[n][k] (+ bias[n]),    Wl[n][k] = w_transposed ? W[k*ldw + n] : W[n*ldw + k]
  *   act_layout 0: ACT is (B, L, K) row-major (u, dy: hyena.py:391, :440 backward)
  *              1: ACT is (B, K, L) channel-major (y_pre, ds: hyena.py:432-440)
@@ -186,8 +187,6 @@ HY_API size_t hyena_b200_proj_wgrad_scratch_bytes(int M, int N);
 HY_API int hyena_b200_proj_wgrad(const float* X, const float* Y, const float* fir, float* dW, int transposed_out, float beta,
                           int B, int L, int M, int N, void* scratch, size_t scratch_bytes, void* stream);
 HY_API size_t hyena_b200_proj_wimg_bytes(int N, int K);
-/* debug aid (tools/dbg_proj_timing.py): device buffer of >= 16 int64 receiving per-role barrier-wait cycle counters */
-HY_API int hyena_b200_proj_debug_buffer(void* buf);
 HY_API int hyena_b200_proj_gemm(const float* act, int act_layout, const float* W, int ldw, int w_transposed,
                          const float* bias, const float* fir, float* out, int out_layout, int B, int L, int K, int N,
                          int l_begin, int l_len, void* wimg, size_t wimg_bytes, void* stream);

@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE ONLY -- numpy model of the FFT decomposition used by the CUDA kernels.
 
 Not part of the product path: only tests/ may import this file.  It restates, in
-vectorised numpy, the exact algebra the sm_100a kernels in
+vectorised numpy, the exact algebra the sm_90a kernels in
 ``hyena-dna_b200/csrc/`` implement, so the index bookkeeping (4-step layout, row
 pairing, even/odd polyphase pointwise product, scaling) can be checked on a CPU
 against ``numpy.fft`` before any GPU time is spent.

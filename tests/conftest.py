@@ -9,12 +9,12 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def pytest_sessionstart(session):
-    # the oracle runs on the host: 128 hardware threads of a shared B200 host made torch CPU ops up to 40x slower
-    # than 8-16 threads do (bench.py cpu_baseline note); keep the CPU side of the tests predictable
+    # the oracle runs on the host: on a large shared host, a hundred-odd threads make torch CPU ops much slower than
+    # 8-16 threads do; keep the CPU side of the tests predictable
     import torch
     torch.set_num_threads(min(16, os.cpu_count() or 1))
 

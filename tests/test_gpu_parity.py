@@ -1,4 +1,4 @@
-"""GPU parity tests: the sm_100a path (through the C ABI) against the CPU oracle and the committed
+"""GPU parity tests: the sm_90a path (through the C ABI) against the CPU oracle and the committed
 reference-generated golden vectors.  Tolerance from BASELINE.json north_star: 1e-3 rel / 1e-5 abs
 in fp32 (applied elementwise, with the abs term scaled by the tensor's magnitude where outputs are
 far from unit scale -- see SURVEY.md S8(c) for why)."""
@@ -314,7 +314,7 @@ def test_host_step_matches_autograd(B, L, D):
     import hyena_dna_b200 as H
     dev = _dev()
     if H.ops.proj_mode() != "tc" and H.ops.gemm_mode() != "bf16x9":
-        pytest.skip("needs the tcgen05 or the cuBLASLt 12.9 projection path")
+        pytest.skip("needs the wgmma or the cuBLASLt 12.9 projection path")
     torch.manual_seed(5)
     op = H.HyenaOperator(D, L, emb_dim=5, w=10.0, lr_pos_emb=0.0).to(dev)
     u = torch.randn(B, L, D); dy = torch.randn(B, L, D)
@@ -480,7 +480,7 @@ def test_validation_of_spectrum_and_filter_shapes():
 @pytest.mark.parametrize("B,L,K,N", [(1, 128, 32, 128), (2, 1000, 64, 192), (1, 4096, 256, 768), (2, 777, 24, 8),
                                      (1, 2048, 768, 256), (1, 333, 40, 200)])
 def test_proj_gemm_tcgen05_matches_fp64(B, L, K, N):
-    """csrc/proj_gemm.cuh (tcgen05, 3xTF32, A operand in tensor memory) against float64 matmuls, all four layout
+    """csrc/proj_gemm.cuh (wgmma, 3xTF32, A operand in registers) against float64 matmuls, all four layout
     combinations, bias epilogue, ragged shapes, and the fused transposed short filter."""
     import hyena_dna_b200 as H
     dev = _dev()
@@ -512,7 +512,7 @@ def test_proj_gemm_tcgen05_matches_fp64(B, L, K, N):
 @pytest.mark.parametrize("B,L,M,N", [(1, 64, 128, 256), (2, 1000, 192, 64), (1, 40000, 768, 256), (2, 777, 24, 8),
                                      (1, 5000, 256, 256), (1, 333, 200, 320)])
 def test_proj_wgrad_tcgen05_matches_fp64(B, L, M, N):
-    """Split-K weight-gradient GEMM (MN-major B operand, A in tensor memory) against float64, plain and with the fused
+    """Split-K weight-gradient GEMM (A operand = Y^T in registers, B = X images in shared memory) against float64, plain and with the fused
     transposed short filter, normal and transposed output."""
     import hyena_dna_b200 as H
     dev = _dev()
@@ -619,7 +619,7 @@ def test_checkpointed_stack_reuses_filter_and_matches_plain_autograd():
     prof2 = H._lib.profile_end()
     assert "filter_tc_fwd" in prof2
     plan = H.memory_plan(1, 1 << 20, 256, 8)
-    assert plan["total"] < 180e9
+    assert plan["total"] < 80e9                     # an 8-layer stack at L = 2^20 fits one 80 GB H100
 
 
 # ------------------------------------------------------------------------------------------ fftconv variants (S8 f4)

@@ -1,6 +1,6 @@
 """CPU checks of the fftconv variants (k_rev, bidirectional): the oracle's restatement against the golden vectors generated
 from the unmodified reference fftconv_ref (tests/golden/make_golden_fftconv.py), and the time-domain decomposition the
-sm_100a host side uses (hyena_dna_b200/fftconv.py: RevCorrFunc, fftconv_ref) against that restatement."""
+sm_90a host side uses (hyena_dna_b200/fftconv.py: RevCorrFunc, fftconv_ref) against that restatement."""
 import os
 
 import numpy as np
