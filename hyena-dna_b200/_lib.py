@@ -49,6 +49,9 @@ SIGNATURES = {
     "hyena_b200_proj_wgrad_scratch_bytes": (_sz, [_i, _i]),
     "hyena_b200_proj_wgrad": (_i, [c_fp, c_fp, c_fp, c_fp, _i, _f, _i, _i, _i, _i, _vp, _sz, _vp]),
     "hyena_b200_proj_gemm": (_i, [c_fp, _i, c_fp, _i, _i, c_fp, c_fp, c_fp, _i, _i, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
+    "hyena_b200_proj_gemm_gelu": (_i, [c_fp, c_fp, _i, _i, c_fp, _i, c_fp, _i, _i, _i, _i, _vp, _sz, _vp]),
+    "hyena_b200_proj_gemm_dgelu": (_i, [c_fp, c_fp, _i, _i, c_fp, _i, c_fp, _i, _i, _i, _i, _vp, _sz, _vp]),
+    "hyena_b200_proj_wgrad_gelu": (_i, [c_fp, c_fp, _i, c_fp, _i, _f, _i, _i, _i, _i, _vp, _sz, _vp]),
     "hyena_b200_filter_ddelta": (_i, [c_fp, c_fp, c_fp, c_fp, _f, _i, _i, c_fp, _vp]),
     "hyena_b200_filter_l1norm_fwd": (_i, [c_fp, c_fp, c_fp, _i, _i, _vp]),
     "hyena_b200_filter_l1norm_bwd": (_i, [c_fp, c_fp, c_fp, c_fp, _i, _i, _vp]),

@@ -278,7 +278,8 @@ HY_API const char* hyena_b200_kind_name(int kind) {
       "row_pass<filter>", "row_pass<conv_fwd>", "row_pass<conv_bwd>",
       "filter_fwd", "filter_bwd", "short_conv_bwd", "twiddle_init", "filter_tc_prep", "filter_tc_fwd", "filter_tc_bwd", "filter_tc_red", "fused_conv_fwd",
       "spectrum_convert", "proj_prep", "proj_gemm", "proj_wgrad",
-      "conv_fwd<pipelined>", "conv_bwd<pipelined>", "filter_spectrum<pipelined>", "add_layer_norm", "filter_extra"};
+      "conv_fwd<pipelined>", "conv_bwd<pipelined>", "filter_spectrum<pipelined>", "add_layer_norm", "filter_extra",
+      "proj_gemm<gelu>", "proj_gemm<dgelu>", "proj_wgrad<gelu>"};
   return (kind >= 0 && kind < K_COUNT) ? names[kind] : "?";
 }
 
@@ -617,6 +618,57 @@ HY_API int hyena_b200_proj_wgrad(const float* X, const float* Y, const float* fi
            proj_wgrad_scratch_bytes(M, N));
   HY_CUDA(launch_proj_wgrad(X, Y, fir, dW, transposed_out, beta, B, L, M, N, reinterpret_cast<float*>(scratch),
                             (cudaStream_t)stream));
+  return 0;
+}
+
+/* block MLP (fc1 -> gelu -> fc2) on the projection kernels with the GELU fused in; see include/hyena_b200.h */
+static int check_gelu(int activation) {
+  HY_CHECK(activation == HYENA_B200_GELU_TANH || activation == HYENA_B200_GELU_ERF,
+           "activation %d: expected HYENA_B200_GELU_TANH (%d) or HYENA_B200_GELU_ERF (%d)", activation, HYENA_B200_GELU_TANH,
+           HYENA_B200_GELU_ERF);
+  return 0;
+}
+
+HY_API int hyena_b200_proj_gemm_gelu(const float* act, const float* W, int ldw, int w_transposed, const float* bias,
+                                     int activation, float* out, int B, int L, int K, int N, void* wimg, size_t wimg_bytes,
+                                     void* stream) {
+  if (check_gelu(activation)) return 1;
+  HY_CHECK(act && W && out && wimg, "null pointer");
+  HY_CHECK(B >= 1 && L >= 1 && K >= 1 && N >= 1, "bad shape B=%d L=%d K=%d N=%d", B, L, K, N);
+  HY_CHECK(aligned16(act) && aligned16(out) && aligned16(wimg) && (!bias || aligned16(bias)), "pointers must be 16-byte aligned");
+  HY_CHECK(wimg_bytes >= proj_wimg_bytes(N, K), "weight image scratch too small: %zu < %zu", wimg_bytes, proj_wimg_bytes(N, K));
+  HY_CHECK(ldw >= (w_transposed ? N : K), "ldw %d too small", ldw);
+  HY_CUDA(launch_proj_gemm(act, 1, W, ldw, w_transposed, bias, nullptr, out, 1, B, L, K, N, 0, L, reinterpret_cast<float*>(wimg),
+                           (cudaStream_t)stream, activation, nullptr));
+  return 0;
+}
+
+HY_API int hyena_b200_proj_gemm_dgelu(const float* act, const float* W, int ldw, int w_transposed, const float* pre,
+                                      int activation, float* out, int B, int L, int K, int N, void* wimg, size_t wimg_bytes,
+                                      void* stream) {
+  if (check_gelu(activation)) return 1;
+  HY_CHECK(act && W && pre && out && wimg, "null pointer");
+  HY_CHECK(B >= 1 && L >= 1 && K >= 1 && N >= 1, "bad shape B=%d L=%d K=%d N=%d", B, L, K, N);
+  HY_CHECK(aligned16(act) && aligned16(out) && aligned16(wimg), "pointers must be 16-byte aligned");
+  HY_CHECK(wimg_bytes >= proj_wimg_bytes(N, K), "weight image scratch too small: %zu < %zu", wimg_bytes, proj_wimg_bytes(N, K));
+  HY_CHECK(ldw >= (w_transposed ? N : K), "ldw %d too small", ldw);
+  const size_t n_out = (size_t)B * N * L;
+  HY_CHECK(pre + n_out <= out || out + n_out <= pre, "pre and out must not overlap");
+  HY_CUDA(launch_proj_gemm(act, 0, W, ldw, w_transposed, nullptr, nullptr, out, 0, B, L, K, N, 0, L, reinterpret_cast<float*>(wimg),
+                           (cudaStream_t)stream, activation, pre));
+  return 0;
+}
+
+HY_API int hyena_b200_proj_wgrad_gelu(const float* X, const float* Y, int activation, float* dW, int transposed_out, float beta,
+                                      int B, int L, int M, int N, void* scratch, size_t scratch_bytes, void* stream) {
+  if (check_gelu(activation)) return 1;
+  HY_CHECK(X && Y && dW && scratch, "null pointer");
+  HY_CHECK(B >= 1 && L >= 1 && M >= 1 && N >= 1, "bad shape B=%d L=%d M=%d N=%d", B, L, M, N);
+  HY_CHECK(aligned16(X) && aligned16(Y) && aligned16(scratch), "pointers must be 16-byte aligned");
+  HY_CHECK(scratch_bytes >= proj_wgrad_scratch_bytes(M, N), "scratch too small: %zu < %zu", scratch_bytes,
+           proj_wgrad_scratch_bytes(M, N));
+  HY_CUDA(launch_proj_wgrad(X, Y, nullptr, dW, transposed_out, beta, B, L, M, N, reinterpret_cast<float*>(scratch),
+                            (cudaStream_t)stream, activation));
   return 0;
 }
 

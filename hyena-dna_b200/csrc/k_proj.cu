@@ -2,10 +2,13 @@
 #include <cstdint>
 #include <cstring>
 
+#include "../../include/hyena_b200.h"
 #include "launch.h"
 #include "proj_gemm.cuh"
 
 namespace hy {
+
+static_assert(FN_GELU_TANH == HYENA_B200_GELU_TANH && FN_GELU_ERF == HYENA_B200_GELU_ERF, "activation codes of the C ABI");
 
 size_t proj_wimg_bytes(int N, int K) {
   const int NT = 128;
@@ -56,9 +59,9 @@ static bool make_tmap3(CUtensorMap* m, const float* base, unsigned long long d0,
            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-template <int NT, int ACT, int OUT>
-static cudaError_t go(pg::Args a, int sms, cudaStream_t s) {
-  auto kern = pg::proj_gemm_kernel<NT, ACT, OUT>;
+template <int NT, int ACT, int OUT, int FN = FN_NONE>
+static cudaError_t go(pg::Args a, int sms, cudaStream_t s, int kind = K_PROJ_GEMM) {
+  auto kern = pg::proj_gemm_kernel<NT, ACT, OUT, FN>;
   CUtensorMap tmap;
   memset(&tmap, 0, sizeof(tmap));
   if (a.vec) {
@@ -73,9 +76,9 @@ static cudaError_t go(pg::Args a, int sms, cudaStream_t s) {
   if (e != cudaSuccess) return e;
   const long long ntiles = (long long)a.B * a.mtiles_per_b * a.ntiles_n;
   const int grid = (int)(ntiles < sms ? ntiles : sms);
-  prof_begin(K_PROJ_GEMM, s);
+  prof_begin(kind, s);
   kern<<<grid, pg::kThreads, smem, s>>>(a, tmap);
-  prof_end(K_PROJ_GEMM, s);
+  prof_end(kind, s);
   return cudaGetLastError();
 }
 
@@ -90,7 +93,7 @@ static cudaError_t by_layout(const pg::Args& a, int act_layout, int out_layout, 
 
 cudaError_t launch_proj_gemm(const float* act, int act_layout, const float* W, int ldw, int w_transposed, const float* bias,
                              const float* fir, float* out, int out_layout, int B, int L, int K, int N, int l0, int ln,
-                             float* wimg, cudaStream_t s) {
+                             float* wimg, cudaStream_t s, int fn, const float* aux) {
   const int NT = 128;
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
@@ -104,7 +107,7 @@ cudaError_t launch_proj_gemm(const float* act, int act_layout, const float* W, i
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   pg::Args a;
-  a.act = act; a.wimg = wimg; a.out = out; a.bias = bias; a.fir = fir;
+  a.act = act; a.wimg = wimg; a.out = out; a.bias = bias; a.fir = fir; a.aux = aux;
   a.B = B; a.L = L; a.K = K; a.N = N; a.l0 = l0; a.ln = ln;
   // TMA needs 16-byte aligned rows (global stride a multiple of 16 bytes) and, for the channel-major box, a 16-byte
   // aligned first position
@@ -113,7 +116,16 @@ cudaError_t launch_proj_gemm(const float* act, int act_layout, const float* W, i
   a.kchunks = (K + pg::kKC - 1) / pg::kKC;
   a.ntiles_n = (N + NT - 1) / NT;
   a.mtiles_per_b = (ln + 127) / 128;
-  return by_layout<128>(a, act_layout, out_layout, sms, s);
+  if (fn == FN_NONE) return by_layout<128>(a, act_layout, out_layout, sms, s);
+  if (act_layout == pg::ACT_CH && out_layout == pg::OUT_ROW) {          // GELU prologue (MLP fc2 forward)
+    if (fn == FN_GELU_TANH) return go<128, pg::ACT_CH, pg::OUT_ROW, FN_GELU_TANH>(a, sms, s, K_PROJ_GEMM_GELU);
+    if (fn == FN_GELU_ERF) return go<128, pg::ACT_CH, pg::OUT_ROW, FN_GELU_ERF>(a, sms, s, K_PROJ_GEMM_GELU);
+  }
+  if (act_layout == pg::ACT_ROW && out_layout == pg::OUT_CH) {          // GELU-gradient epilogue (MLP fc2 input gradient)
+    if (fn == FN_GELU_TANH) return go<128, pg::ACT_ROW, pg::OUT_CH, FN_GELU_TANH>(a, sms, s, K_PROJ_GEMM_DGELU);
+    if (fn == FN_GELU_ERF) return go<128, pg::ACT_ROW, pg::OUT_CH, FN_GELU_ERF>(a, sms, s, K_PROJ_GEMM_DGELU);
+  }
+  return cudaErrorInvalidValue;
 }
 
 
@@ -134,7 +146,7 @@ size_t proj_wgrad_scratch_bytes(int M, int N) {
 }
 
 cudaError_t launch_proj_wgrad(const float* X, const float* Y, const float* fir, float* dW, int transposed_out, float beta,
-                              int B, int L, int M, int N, float* part, cudaStream_t s) {
+                              int B, int L, int M, int N, float* part, cudaStream_t s, int fn) {
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
@@ -153,19 +165,23 @@ cudaError_t launch_proj_wgrad(const float* X, const float* Y, const float* fir, 
                     make_tmap3(&tmy, Y, (unsigned long long)N, (unsigned long long)L, (unsigned long long)B, 128, 32);
     if (!ok) a.vec = 0;                  // no driver entry point / unencodable shape: the producer warp stages by hand
   }
-  cudaError_t e = cudaFuncSetAttribute(wg::wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wg::kSmem);
+  auto kern = fn == FN_GELU_TANH ? wg::wgrad_kernel<FN_GELU_TANH>
+            : fn == FN_GELU_ERF  ? wg::wgrad_kernel<FN_GELU_ERF> : wg::wgrad_kernel<FN_NONE>;
+  if (fn != FN_NONE && (fir || (fn != FN_GELU_TANH && fn != FN_GELU_ERF))) return cudaErrorInvalidValue;
+  const int kind = fn == FN_NONE ? K_PROJ_WGRAD : K_PROJ_WGRAD_GELU;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wg::kSmem);
   if (e != cudaSuccess) return e;
-  prof_begin(K_PROJ_WGRAD, s);
-  wg::wgrad_kernel<<<a.mtiles * a.ntiles * a.splits, wg::kThreads, wg::kSmem, s>>>(a, tmx, tmy);
-  prof_end(K_PROJ_WGRAD, s);
+  prof_begin(kind, s);
+  kern<<<a.mtiles * a.ntiles * a.splits, wg::kThreads, wg::kSmem, s>>>(a, tmx, tmy);
+  prof_end(kind, s);
   e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   const size_t total = (size_t)M * N;
   int blocks = (int)((total + 255) / 256);
   if (blocks > 2 * sms) blocks = 2 * sms;
-  prof_begin(K_PROJ_WGRAD, s);
+  prof_begin(kind, s);
   wg::wgrad_reduce_kernel<<<blocks, 256, 0, s>>>(part, dW, a.splits, M, N, transposed_out, beta);
-  prof_end(K_PROJ_WGRAD, s);
+  prof_end(kind, s);
   return cudaGetLastError();
 }
 

@@ -17,7 +17,8 @@ enum Kind {
   K_PIPE_FWD = 25, K_PIPE_BWD = 26, K_PIPE_FILTER = 27,   // whole pipelined calls (api.cu PipeRun): kernels of different groups overlap
   K_ADD_LN = 28,            // residual add + LayerNorm (block glue, layernorm.cuh)
   K_FILTER_EXTRA = 29,      // deltas gradient / channel L1 normalisation (filter_extra.cuh; non-default filter options)
-  K_COUNT = 30
+  K_PROJ_GEMM_GELU = 30, K_PROJ_GEMM_DGELU = 31, K_PROJ_WGRAD_GELU = 32,   // block MLP: projection GEMMs with fused GELU
+  K_COUNT = 33
 };
 void prof_begin(int kind, cudaStream_t s);     // api.cu: records an event when profiling is on
 void prof_end(int kind, cudaStream_t s);       // api.cu: records an event when profiling is on; counts the launch
@@ -40,10 +41,10 @@ cudaError_t launch_twiddle_init(float2* tw1024, float2* twlo, cudaStream_t s);
 size_t proj_wimg_bytes(int N, int K);
 cudaError_t launch_proj_gemm(const float* act, int act_layout, const float* W, int ldw, int w_transposed, const float* bias,
                              const float* fir, float* out, int out_layout, int B, int L, int K, int N, int l0, int ln,
-                             float* wimg, cudaStream_t s);
+                             float* wimg, cudaStream_t s, int fn = 0 /* ActFn */, const float* aux = nullptr);
 size_t proj_wgrad_scratch_bytes(int M, int N);
 cudaError_t launch_proj_wgrad(const float* X, const float* Y, const float* fir, float* dW, int transposed_out, float beta,
-                              int B, int L, int M, int N, float* part, cudaStream_t s);
+                              int B, int L, int M, int N, float* part, cudaStream_t s, int fn = 0);
 // k_filter.cu: filter_extra.cuh
 cudaError_t launch_filter_ddelta(const float* dk, const float* k, const float* t, const float* deltas, float shift, int D,
                                  int L, float* ddelta, cudaStream_t s);

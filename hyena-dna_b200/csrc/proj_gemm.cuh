@@ -21,6 +21,12 @@
 // Optional fused prologue (FIR): the activation is ds (B, C, L) and the GEMM consumes dp = transposed 3-tap depthwise
 // filter of ds (dp[t] = w2 ds[t] + w1 ds[t+1] + w0 ds[t+2], hyena.py:363-369 backward), so dp never exists in HBM.
 //
+// Optional GELU transforms (template argument FN, the block MLP fc1 -> gelu -> fc2 with the hidden activation `a` kept
+// channel-major (B, H, L); hyena-dna_b200/mlp.py):
+//   ACT_CH  prologue: the GEMM consumes gelu(act)            (fc2 forward: gelu(a) never exists in HBM)
+//   OUT_CH  epilogue: OUT = acc * gelu'(aux), aux (B, N, L)  (fc2 input gradient: da = (dy W2) o gelu'(a))
+//   wgrad   the converter warps build the B images from gelu(X)  (fc2 weight gradient)
+//
 // Weight gradients (wgrad_kernel) at the end of the file.
 #pragma once
 #include <cuda.h>      // CUtensorMap (types only: the encode function is looked up at run time, no libcuda link)
@@ -29,6 +35,42 @@
 #include "tc_prims.cuh"
 
 namespace hy {
+
+// Elementwise activations fused into the projection GEMMs: torch's fp32 GELU (approximate="tanh" / "none") and its
+// analytic derivative, in the same formulas (ATen ActivationGeluKernel.cu) with the accurate tanhf / erff / expf.
+enum ActFn { FN_NONE = 0, FN_GELU_TANH = 1, FN_GELU_ERF = 2 };
+
+template <int FN>
+__device__ __forceinline__ float act_fn(float x) {
+  static_assert(FN == FN_GELU_TANH || FN == FN_GELU_ERF, "GELU variant");
+  if constexpr (FN == FN_GELU_TANH) {
+    constexpr float kBeta = (float)(M_SQRT2 * M_2_SQRTPI * 0.5), kKappa = 0.044715f;
+    const float inner = kBeta * (x + kKappa * (x * x * x));
+    return 0.5f * x * (1.f + tanhf(inner));
+  } else {
+    return x * 0.5f * (1.f + erff(x * (float)M_SQRT1_2));
+  }
+}
+
+template <int FN>
+__device__ __forceinline__ float act_grad(float x) {
+  static_assert(FN == FN_GELU_TANH || FN == FN_GELU_ERF, "GELU variant");
+  if constexpr (FN == FN_GELU_TANH) {
+    constexpr float kBeta = (float)(M_SQRT2 * M_2_SQRTPI * 0.5), kKappa = 0.044715f;
+    const float x_sq = x * x;
+    const float th = tanhf(kBeta * (x + kKappa * (x_sq * x)));
+    const float left = 0.5f * x, right = 1.f + th;
+    const float left_derivative = 0.5f * right;
+    const float right_derivative = left * (1.f - th * th) * (kBeta * (1.f + 3.f * kKappa * x_sq));
+    return left_derivative + right_derivative;
+  } else {
+    constexpr float kBeta = (float)(M_2_SQRTPI * M_SQRT1_2 * 0.5);
+    const float cdf = 0.5f * (1.f + erff(x * (float)M_SQRT1_2));
+    const float pdf = expf(-0.5f * x * x) * kBeta;
+    return cdf + x * pdf;
+  }
+}
+
 namespace pg {
 
 constexpr int kKC = 32;                 // K chunk (one chunk = 4 MMAs of K = 8 per product)
@@ -57,6 +99,7 @@ struct Args {
   int ntiles_n;          // ceil(N / NT)
   int mtiles_per_b;      // ceil(ln / 128)
   int vec;               // 1: the activation qualifies for TMA (16-byte aligned rows): `tmap` is valid
+  const float* aux;      // (B, N, L) pre-activation read by the gradient epilogue (OUT_CH with FN != FN_NONE), or null
 };
 
 // ------------------------------------------------------------------------------------------------ weight images
@@ -108,8 +151,11 @@ template <int NT> struct Cfg {
 //                   (-> fused FIR) -> (hi, lo) split -> wgmma against the weight stage -> register accumulators -> stores
 //   warp 8          producer: per chunk one TMA bulk copy of the weight images and one tiled TMA copy of the activation
 //                   tile (lane 0); stages the activation by hand when it does not qualify for TMA (all lanes)
-template <int NT, int ACT, int OUT>
+// FN != FN_NONE: GELU prologue (ACT_CH -> OUT_ROW) or GELU-gradient epilogue (ACT_ROW -> OUT_CH), see the top of the file
+template <int NT, int ACT, int OUT, int FN = FN_NONE>
 __global__ void __launch_bounds__(kThreads, 1) proj_gemm_kernel(const Args a, const __grid_constant__ CUtensorMap tmap) {
+  static_assert(FN == FN_NONE || (ACT == ACT_CH && OUT == OUT_ROW) || (ACT == ACT_ROW && OUT == OUT_CH),
+                "the GELU transforms exist for the fc2 forward and input-gradient layouts only");
   using C = Cfg<NT>;
   extern __shared__ __align__(1024) unsigned char smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR);
@@ -221,7 +267,9 @@ __global__ void __launch_bounds__(kThreads, 1) proj_gemm_kernel(const Args a, co
             x = *reinterpret_cast<const float*>(st + row * 128 + (((k >> 2) ^ (row & 7)) << 4) + (k & 3) * 4);
           } else {
             const float* sp = reinterpret_cast<const float*>(st + k * kAPitchCh) + row;
-            if (!use_fir) {
+            if constexpr (FN != FN_NONE) {
+              x = act_fn<FN>(sp[0]);       // zero-filled staging (tails of K and L) stays zero: gelu(0) = 0
+            } else if (!use_fir) {
               x = sp[0];
             } else {
               // dp[t] = w2 ds[t] + w1 ds[t+1] + w0 ds[t+2]; ds beyond the tensor end is staged as zero, a position
@@ -266,11 +314,27 @@ __global__ void __launch_bounds__(kThreads, 1) proj_gemm_kernel(const Args a, co
     for (int h = 0; h < 2; ++h) {
       const int l = lt + r0 + 8 * h;
       if (l >= lend) continue;
+      float pre[16];
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
+        if constexpr (OUT == OUT_CH && FN != FN_NONE) {
+          // gradient epilogue: the pre-activation values of eight column pairs are fetched together, so that their
+          // loads are in flight at once instead of each one stalling the multiply that consumes it
+          if (j % 8 == 0) {
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+              const int n = nt * NT + 8 * (j + (i >> 1)) + 2 * t + (i & 1);
+              pre[i] = n < a.N ? __ldg(a.aux + ((size_t)b * a.N + n) * a.L + l) : 0.f;
+            }
+          }
+        }
         const int n = nt * NT + 8 * j + 2 * t;
         float v0 = sum[4 * j + 2 * h], v1 = sum[4 * j + 2 * h + 1];
-        if constexpr (OUT == OUT_CH) {
+        if constexpr (OUT == OUT_CH && FN != FN_NONE) {
+          float* dst = a.out + ((size_t)b * a.N + n) * a.L + l;
+          if (n < a.N) dst[0] = v0 * act_grad<FN>(pre[2 * (j % 8)]);
+          if (n + 1 < a.N) dst[a.L] = v1 * act_grad<FN>(pre[2 * (j % 8) + 1]);
+        } else if constexpr (OUT == OUT_CH) {
           float* dst = a.out + ((size_t)b * a.N + n) * a.L + l;
           if (n < a.N) dst[0] = v0 + (a.bias ? __ldg(a.bias + n) : 0.f);
           if (n + 1 < a.N) dst[a.L] = v1 + (a.bias ? __ldg(a.bias + n + 1) : 0.f);
@@ -343,6 +407,8 @@ struct Args {
 // the (N, L, B) tensor) and one of the X tile (box 36 pos x 128 m of the (L, M, B) tensor; four look-ahead samples for
 // the fused FIR), completion on an mbarrier per stage.  Out-of-range rows / columns / positions are zero-filled by the
 // copy engine (tails of M, N and L; the 3-D maps keep a tile from running into the next batch).
+// FN != FN_NONE: the product is taken with gelu(X) (fir must be null), applied by the converter warps.
+template <int FN = FN_NONE>
 __global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const Args a, const __grid_constant__ CUtensorMap tmapX,
                                                             const __grid_constant__ CUtensorMap tmapY) {
   extern __shared__ __align__(1024) unsigned char smem[];
@@ -478,6 +544,9 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const Args a, const 
           o.z = fmaf(w[i][2], v.z, fmaf(w[i][1], v.w, w[i][0] * x4));
           o.w = fmaf(w[i][2], v.w, fmaf(w[i][1], x4, w[i][0] * x5));
           v = o;
+        }
+        if constexpr (FN != FN_NONE) {                                 // zero fill outside the tensor stays zero
+          v.x = act_fn<FN>(v.x); v.y = act_fn<FN>(v.y); v.z = act_fn<FN>(v.z); v.w = act_fn<FN>(v.w);
         }
         float4 h, lw;
         tc::split_tf32(v.x, h.x, lw.x); tc::split_tf32(v.y, h.y, lw.y);

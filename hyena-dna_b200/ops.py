@@ -473,10 +473,24 @@ def proj_mode():
     return _proj_mode
 
 
-def proj_gemm(act, act_layout, W, w_transposed, out_layout, bias=None, fir=None, out=None, l_range=None):
+_GELU_CODES = {"tanh": 1, "none": 2}        # F.gelu(approximate=...) -> HYENA_B200_GELU_TANH / HYENA_B200_GELU_ERF
+
+
+def _gelu_code(approximate):
+    if approximate not in _GELU_CODES:
+        raise _lib.HyenaB200Error(f"GELU approximate must be 'tanh' or 'none', got {approximate!r}")
+    return _GELU_CODES[approximate]
+
+
+def proj_gemm(act, act_layout, W, w_transposed, out_layout, bias=None, fir=None, out=None, l_range=None, gelu=None,
+              gelu_pre=None):
     """OUT[pos][n] = sum_k ACT[pos][k] Wl[n][k] (+ bias) on this library's wgmma kernel (csrc/proj_gemm.cuh, 3xTF32).
-    act_layout 0: act (B, L, K); 1: act (B, K, L).  out_layout 0: (B, N, L); 1: (B, L, N).  Wl = W.T if w_transposed."""
-    _need_cuda(act, W, bias, fir)
+    act_layout 0: act (B, L, K); 1: act (B, K, L).  out_layout 0: (B, N, L); 1: (B, L, N).  Wl = W.T if w_transposed.
+
+    gelu ('tanh' | 'none', F.gelu's ``approximate``) fuses the block MLP's activation: with act_layout 1 / out_layout 1 the
+    GEMM consumes gelu(act); with act_layout 0 / out_layout 0 and ``gelu_pre`` (B, N, L) the output is multiplied by
+    gelu'(gelu_pre)."""
+    _need_cuda(act, W, bias, fir, gelu_pre)
     if act.dim() != 3 or W.dim() != 2 or not act.is_contiguous() or not W.is_contiguous():
         raise _lib.HyenaB200Error("proj_gemm: act must be contiguous 3-D, W contiguous 2-D")
     B = act.shape[0]
@@ -497,6 +511,28 @@ def proj_gemm(act, act_layout, W, w_transposed, out_layout, bias=None, fir=None,
     if wimg is None or wimg.numel() < need:
         wimg = torch.empty(max(need, 4 << 20), dtype=torch.uint8, device=dev)
         _wimg_cache[key] = wimg
+    if gelu is not None:
+        code = _gelu_code(gelu)
+        if fir is not None or l_range is not None:
+            raise _lib.HyenaB200Error("proj_gemm: the fused GELU takes no short filter and no position range")
+        if act_layout == 1 and out_layout == 1 and gelu_pre is None:
+            with torch.cuda.device(dev):
+                _lib.check(_lib.lib().hyena_b200_proj_gemm_gelu(
+                    _ptr(act), _ptr(W), W.shape[1], int(bool(w_transposed)), _ptr(bias), code, _ptr(out), B, L, K, N,
+                    _ptr(wimg), wimg.numel(), _stream()))
+            return out
+        if act_layout == 0 and out_layout == 0 and bias is None and gelu_pre is not None:
+            if tuple(gelu_pre.shape) != oshape or not gelu_pre.is_contiguous():
+                raise _lib.HyenaB200Error(f"proj_gemm: gelu_pre must be contiguous {oshape}")
+            with torch.cuda.device(dev):
+                _lib.check(_lib.lib().hyena_b200_proj_gemm_dgelu(
+                    _ptr(act), _ptr(W), W.shape[1], int(bool(w_transposed)), _ptr(gelu_pre), code, _ptr(out), B, L, K, N,
+                    _ptr(wimg), wimg.numel(), _stream()))
+            return out
+        raise _lib.HyenaB200Error("proj_gemm: the fused GELU runs as (act_layout 1, out_layout 1) or, with gelu_pre and "
+                                  "no bias, as (act_layout 0, out_layout 0)")
+    if gelu_pre is not None:
+        raise _lib.HyenaB200Error("proj_gemm: gelu_pre needs gelu")
     with torch.cuda.device(dev):
         _lib.check(_lib.lib().hyena_b200_proj_gemm(
             _ptr(act), int(act_layout), _ptr(W), W.shape[1], int(bool(w_transposed)), _ptr(bias), _ptr(fir), _ptr(out),
@@ -514,9 +550,10 @@ def fuse_fir():
     return os.environ.get("HYENA_B200_FUSE_FIR", "1") != "0"
 
 
-def proj_wgrad(X, Y, fir=None, transposed_out=False):
+def proj_wgrad(X, Y, fir=None, transposed_out=False, gelu=None):
     """dW (M, N) [(N, M) if transposed_out] = sum_{b,pos} X[b][m][pos] Y[b][pos][n]; X (B, M, L), Y (B, L, N)
-    (csrc/proj_gemm.cuh wgrad_kernel: wgmma 3xTF32, split-K, deterministic)."""
+    (csrc/proj_gemm.cuh wgrad_kernel: wgmma 3xTF32, split-K, deterministic).  gelu ('tanh' | 'none'): the product is
+    taken with gelu(X) instead of X (block MLP fc2 weight gradient)."""
     _need_cuda(X, Y, fir)
     if X.dim() != 3 or Y.dim() != 3 or not X.is_contiguous() or not Y.is_contiguous() or X.shape[0] != Y.shape[0] \
             or X.shape[2] != Y.shape[1]:
@@ -532,9 +569,57 @@ def proj_wgrad(X, Y, fir=None, transposed_out=False):
         sc = torch.empty(need, dtype=torch.uint8, device=dev)
         _wgrad_cache[key] = sc
     with torch.cuda.device(dev):
-        _lib.check(_lib.lib().hyena_b200_proj_wgrad(_ptr(X), _ptr(Y), _ptr(fir), _ptr(dW), int(bool(transposed_out)), 0.0,
-                                                    B, L, M, N, _ptr(sc), sc.numel(), _stream()))
+        if gelu is not None:
+            if fir is not None:
+                raise _lib.HyenaB200Error("proj_wgrad: the fused GELU takes no short filter")
+            _lib.check(_lib.lib().hyena_b200_proj_wgrad_gelu(_ptr(X), _ptr(Y), _gelu_code(gelu), _ptr(dW),
+                                                             int(bool(transposed_out)), 0.0, B, L, M, N, _ptr(sc), sc.numel(),
+                                                             _stream()))
+        else:
+            _lib.check(_lib.lib().hyena_b200_proj_wgrad(_ptr(X), _ptr(Y), _ptr(fir), _ptr(dW), int(bool(transposed_out)),
+                                                        0.0, B, L, M, N, _ptr(sc), sc.numel(), _stream()))
     return dW
+
+
+class MlpFn(torch.autograd.Function):
+    """Block MLP y = fc2(gelu(fc1(x))) as ONE autograd node on the wgmma projection kernels, fp32 (3xTF32).
+
+    Replaces flash_attn/modules/mlp.py:26-30 (the Mlp that src/models/sequence/long_conv_lm.py:102-123 builds).  x is
+    (B, L, D); the hidden activation a = fc1(x) is written channel-major (B, H, L), the layout in which every GEMM of the
+    MLP is one the projection kernels already run.  GELU is applied in fc2's operand prologue, gelu' in the epilogue of
+    the fc2 input gradient and gelu again in the converter warps of the fc2 weight gradient, so the saved state is x, a
+    and the two weights: one hidden-sized tensor instead of autograd's two (fc1 output and gelu output)."""
+
+    @staticmethod
+    def forward(ctx, x, W1, b1, W2, b2, approximate):
+        x = x.contiguous(); W1 = W1.contiguous(); W2 = W2.contiguous()
+        b1 = b1.contiguous() if b1 is not None else None
+        b2 = b2.contiguous() if b2 is not None else None
+        if x.dim() != 3 or W1.dim() != 2 or W2.dim() != 2 or W1.shape[1] != x.shape[2] or W2.shape[1] != W1.shape[0]:
+            raise _lib.HyenaB200Error(f"MlpFn: x (B, L, D), W1 (H, D), W2 (Do, H) expected; got {tuple(x.shape)}, "
+                                      f"{tuple(W1.shape)}, {tuple(W2.shape)}")
+        a = proj_gemm(x, 0, W1, False, 0, bias=b1)                                  # (B, H, L) = W1 x^T + b1
+        y = proj_gemm(a, 1, W2, False, 1, bias=b2, gelu=approximate)                # (B, L, Do) = gelu(a)^T W2^T + b2
+        ctx.save_for_backward(x, a, W1, W2)
+        ctx.approximate, ctx.has_b1, ctx.has_b2 = approximate, b1 is not None, b2 is not None
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, a, W1, W2 = ctx.saved_tensors
+        dy = dy.contiguous()
+        _need_cuda(dy)
+        approx = ctx.approximate
+        need_x, need_w1, need_b1, need_w2, need_b2 = (ctx.needs_input_grad[i] for i in range(5))
+        dW2 = proj_wgrad(a, dy, transposed_out=True, gelu=approx) if need_w2 else None    # (Do, H) = sum dy^T gelu(a)
+        db2 = dy.sum((0, 1)) if (ctx.has_b2 and need_b2) else None
+        dx = dW1 = db1 = None
+        if need_x or need_w1 or need_b1:
+            da = proj_gemm(dy, 0, W2, True, 0, gelu=approx, gelu_pre=a)                 # (B, H, L) = (dy W2)^T o gelu'(a)
+            dx = proj_gemm(da, 1, W1, True, 1) if need_x else None                      # (B, L, D) = da^T W1
+            dW1 = proj_wgrad(da, x) if need_w1 else None                                # (H, D) = sum da x
+            db1 = da.sum((0, 2)) if (ctx.has_b1 and need_b1) else None
+        return dx, dW1, db1, dW2, db2, None
 
 
 _side_streams = {}

@@ -190,6 +190,27 @@ HY_API size_t hyena_b200_proj_wimg_bytes(int N, int K);
 HY_API int hyena_b200_proj_gemm(const float* act, int act_layout, const float* W, int ldw, int w_transposed,
                          const float* bias, const float* fir, float* out, int out_layout, int B, int L, int K, int N,
                          int l_begin, int l_len, void* wimg, size_t wimg_bytes, void* stream);
+/* ---- block MLP: fc1 -> gelu -> fc2 with the GELU fused into the projection kernels ------------------
+ * replaces flash_attn/modules/mlp.py:26-30 (Mlp.forward: fc1, activation, fc2) as src/models/sequence/long_conv_lm.py:102-123
+ * (create_mlp_cls) builds it, and its autograd.  The hidden activation a = fc1(x) is kept channel-major (B, H, L): fc1
+ * and its gradients are plain hyena_b200_proj_gemm / hyena_b200_proj_wgrad calls, and the three products of fc2 below apply
+ * the activation (or its derivative) in registers, so gelu(a) and gelu'(a) never exist in HBM.  activation:
+ * HYENA_B200_GELU_TANH = F.gelu(approximate="tanh"), HYENA_B200_GELU_ERF = F.gelu(approximate="none"), fp32 as torch
+ * computes them.  Shapes, weights (W, ldw, w_transposed), wimg and scratch as for proj_gemm / proj_wgrad.
+ *   proj_gemm_gelu   OUT (B, L, N) = gelu(ACT) Wl^T (+ bias),  ACT (B, K, L) channel-major        (fc2 forward)
+ *   proj_gemm_dgelu  OUT (B, N, L) = (ACT Wl^T)^T o gelu'(pre), ACT (B, L, K) row-major, pre (B, N, L) the
+ *                    pre-activation, not overlapping OUT                                          (fc2 input gradient)
+ *   proj_wgrad_gelu  dW[m][n] (= or +=) sum_{b,pos} gelu(X[b][m][pos]) Y[b][pos][n]               (fc2 weight gradient) */
+#define HYENA_B200_GELU_TANH 1
+#define HYENA_B200_GELU_ERF 2
+HY_API int hyena_b200_proj_gemm_gelu(const float* act, const float* W, int ldw, int w_transposed, const float* bias,
+                                     int activation, float* out, int B, int L, int K, int N, void* wimg, size_t wimg_bytes,
+                                     void* stream);
+HY_API int hyena_b200_proj_gemm_dgelu(const float* act, const float* W, int ldw, int w_transposed, const float* pre,
+                                      int activation, float* out, int B, int L, int K, int N, void* wimg, size_t wimg_bytes,
+                                      void* stream);
+HY_API int hyena_b200_proj_wgrad_gelu(const float* X, const float* Y, int activation, float* dW, int transposed_out, float beta,
+                                      int B, int L, int M, int N, void* scratch, size_t scratch_bytes, void* stream);
 HY_API int hyena_b200_gemm(int transa, int transb, int m, int n, int k, float alpha, const float* A, int lda,
                            long long strideA, const float* B, int ldb, long long strideB, float beta, float* C,
                            int ldc, long long strideC, int batch, const float* bias, int emulate, void* workspace,
