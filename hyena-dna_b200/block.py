@@ -15,6 +15,7 @@ import torch.nn as nn
 
 from . import ops
 from ._lib import HyenaB200Error
+from .decode import DecodeCache
 
 
 class Block(nn.Module):
@@ -59,9 +60,29 @@ class Block(nn.Module):
         """(hidden_states, residual) -> (mlp(LN2(.)) or mixer output, new residual); block.py:111-180, prenorm branch."""
         if mixer_subset is not None:
             raise HyenaB200Error("Block: mixer_subset is not supported")
+        return self._run(hidden_states, residual, lambda y: self.mixer(y, **(mixer_kwargs or {})))
+
+    def prefill(self, hidden_states, residual, cache):
+        """forward over the first positions, filling the mixer's DecodeCache (HyenaOperator.prefill)."""
+        return self._decode(hidden_states, residual, lambda y: self.mixer.prefill(y, cache))
+
+    def step(self, hidden_states, residual, cache):
+        """forward of one position (B, 1, D) from the mixer's DecodeCache (HyenaOperator.step).  The residual stream of a
+        position depends on that position only, so the block keeps no state of its own."""
+        return self._decode(hidden_states, residual, lambda y: self.mixer.step(y, cache))
+
+    def _decode(self, hidden_states, residual, mix):
+        if not hasattr(self.mixer, "step"):
+            raise HyenaB200Error(f"Block: the mixer {type(self.mixer).__name__} has no incremental decoding")
+        if hidden_states.requires_grad or (residual is not None and residual.requires_grad):
+            raise HyenaB200Error("decoding is inference only: the input requires grad (run under torch.no_grad())")
+        with torch.no_grad():
+            return self._run(hidden_states, residual, mix)
+
+    def _run(self, hidden_states, residual, mix):
         in_dtype = hidden_states.dtype
         y, residual = self._add_norm(hidden_states, residual, self.norm1)
-        hidden_states = self.mixer(y.to(in_dtype), **(mixer_kwargs or {}))
+        hidden_states = mix(y.to(in_dtype))
         if isinstance(hidden_states, tuple):                # mixers built with return_state
             hidden_states = hidden_states[0]
         if not isinstance(self.mlp, nn.Identity):
@@ -90,3 +111,25 @@ class Backbone(nn.Module):
             hidden_states, residual = layer(hidden_states, residual)
         y, _ = Block._add_norm(hidden_states, residual, self.ln_f)
         return y.to(hidden_states.dtype)
+
+    def allocate_decode_cache(self, batch_size, max_seqlen):
+        """One DecodeCache holding the state of every layer's mixer (decode.py)."""
+        return DecodeCache.stack(layer.mixer.allocate_decode_cache(batch_size, max_seqlen) for layer in self.layers)
+
+    def prefill(self, hidden_states, cache):
+        """forward over the first P positions (B, P, D), filling ``cache`` for step()."""
+        return self._decode(hidden_states, cache, "prefill")
+
+    def step(self, hidden_states, cache):
+        """The output of one more position (B, 1, D)."""
+        return self._decode(hidden_states, cache, "step")
+
+    def _decode(self, hidden_states, cache, how):
+        if hidden_states.requires_grad:
+            raise HyenaB200Error("decoding is inference only: the input requires grad (run under torch.no_grad())")
+        with torch.no_grad():
+            residual = None
+            for layer in self.layers:
+                hidden_states, residual = getattr(layer, how)(hidden_states, residual, cache)
+            y, _ = Block._add_norm(hidden_states, residual, self.ln_f)
+            return y.to(hidden_states.dtype)

@@ -279,7 +279,7 @@ HY_API const char* hyena_b200_kind_name(int kind) {
       "filter_fwd", "filter_bwd", "short_conv_bwd", "twiddle_init", "filter_tc_prep", "filter_tc_fwd", "filter_tc_bwd", "filter_tc_red", "fused_conv_fwd",
       "spectrum_convert", "proj_prep", "proj_gemm", "proj_wgrad",
       "conv_fwd<pipelined>", "conv_bwd<pipelined>", "filter_spectrum<pipelined>", "add_layer_norm", "filter_extra",
-      "proj_gemm<gelu>", "proj_gemm<dgelu>", "proj_wgrad<gelu>"};
+      "proj_gemm<gelu>", "proj_gemm<dgelu>", "proj_wgrad<gelu>", "decode_hist", "decode_step"};
   return (kind >= 0 && kind < K_COUNT) ? names[kind] : "?";
 }
 
@@ -772,6 +772,45 @@ HY_API int hyena_b200_add_layernorm_bwd(const float* dy, const float* dres, cons
   HY_CHECK(scratch_bytes >= hyena_b200_add_layernorm_scratch_bytes(rows, D), "scratch too small (%zu bytes)", scratch_bytes);
   ln::BwdArgs a{dy, dres, r, w, mean, rstd, dx, reinterpret_cast<float*>(scratch), rows, D};
   HY_CUDA(launch_add_ln_bwd(a, dw, db, (cudaStream_t)stream));
+  return 0;
+}
+
+/* incremental decoding of the causal operator (the reference's HyenaOperator.recurrence hook, hyena.py:384-386) */
+static int check_decode_shape(int B, int cache_B, int D, int order, int Lcap) {
+  HY_CHECK(B >= 1 && D >= 1 && Lcap >= 1, "bad shape B=%d D=%d Lcap=%d", B, D, Lcap);
+  HY_CHECK(B == cache_B, "batch size %d differs from the decode cache's %d", B, cache_B);
+  HY_CHECK(order >= 2 && order <= dec::kMaxOrder, "order %d outside [2, %d]", order, dec::kMaxOrder);
+  HY_CHECK(Lcap <= (1 << 20), "cache length %d exceeds the supported maximum %d", Lcap, 1 << 20);
+  return 0;
+}
+
+HY_API int hyena_b200_decode_hist(const float* p, const float* in_bias, const float* sw, const float* sb, float* h,
+                                  float* tail, int B, int cache_B, int D, int order, int P, int Lcap, void* stream) {
+  if (check_decode_shape(B, cache_B, D, order, Lcap)) return 1;
+  HY_CHECK(p && sw && sb && h && tail, "null pointer");
+  HY_CHECK(P >= 1 && P <= Lcap, "prefill of %d positions outside [1, %d]", P, Lcap);
+  dec::HistArgs a{p, in_bias, sw, sb, h, tail, B, D, (order + 1) * D, P, dec::ld_for(Lcap), (order - 1) * D};
+  HY_CUDA(launch_decode_hist(a, (cudaStream_t)stream));
+  return 0;
+}
+
+HY_API int hyena_b200_decode_step(const float* p_t, const float* in_bias, const float* sw, const float* sb, const float* k,
+                                  const float* fbias, float* h, float* tail, float* s_t, const float* v_in, float* out,
+                                  float* part, int B, int cache_B, int D, int order, int o, int t, int Lcap, void* stream) {
+  if (check_decode_shape(B, cache_B, D, order, Lcap)) return 1;
+  HY_CHECK(k && fbias && h && s_t && out && part, "null pointer");
+  HY_CHECK(o >= 0 && o < order - 1, "recurrence %d outside [0, %d)", o, order - 1);
+  HY_CHECK(o == 0 ? (p_t && sw && sb && tail && !v_in) : (v_in != nullptr),
+           o == 0 ? "null pointer: recurrence 0 needs p_t, sw, sb, tail (and no v_in)" : "null pointer: v_in");
+  HY_CHECK(t >= 0 && t < Lcap, "position %d outside the decode cache [0, %d)", t, Lcap);
+  const int ld = dec::ld_for(Lcap);
+  HY_CHECK(aligned16(k) && aligned16(h), "k and h must be 16-byte aligned");
+  const int F = order - 1;
+  dec::DotArgs dot{h, k + (size_t)o * ld, part, B, D, t, ld, F * ld, dec::chunks_for(Lcap)};
+  dec::StepArgs st{part, (t + dec::kChunk - 1) / dec::kChunk, dec::chunks_for(Lcap), k + (size_t)o * ld, fbias + o, F * ld, F,
+                   ld, p_t, in_bias, sw, sb, tail, s_t, v_in, h, out, B, D, (order + 1) * D, order, t, (order - 1 - o) * D,
+                   o == order - 2};
+  HY_CUDA(launch_decode_step(dot, st, (cudaStream_t)stream));
   return 0;
 }
 

@@ -1,0 +1,47 @@
+// Launchers of the incremental-decoding kernels (decode.cuh).
+#include "launch.h"
+#include "decode.cuh"
+
+namespace hy {
+
+cudaError_t launch_decode_hist(const dec::HistArgs& a, cudaStream_t s) {
+  const int per_row = (a.P + 255) / 256;
+  dim3 grid(per_row < 64 ? per_row : 64, a.B * a.D);
+  prof_begin(K_DECODE_HIST, s);
+  dec::decode_hist_kernel<<<grid, 256, 0, s>>>(a);
+  prof_end(K_DECODE_HIST, s);
+  return cudaGetLastError();
+}
+
+template <int BG>
+static cudaError_t dot_bg(const dec::DotArgs& a, int R, dim3 grid, cudaStream_t s) {
+  const int threads = 32 * dec::kDotWarps;
+  switch (R) {
+    case 0: dec::decode_dot_kernel<BG, 0><<<grid, threads, 0, s>>>(a); break;
+    case 1: dec::decode_dot_kernel<BG, 1><<<grid, threads, 0, s>>>(a); break;
+    case 2: dec::decode_dot_kernel<BG, 2><<<grid, threads, 0, s>>>(a); break;
+    default: dec::decode_dot_kernel<BG, 3><<<grid, threads, 0, s>>>(a); break;
+  }
+  return cudaGetLastError();
+}
+
+// one recurrence of one step: the split dot product over the history (skipped at t = 0), then the combine kernel
+cudaError_t launch_decode_step(const dec::DotArgs& dot, const dec::StepArgs& st, cudaStream_t s) {
+  if (st.nchunk > 0) {
+    const int BG = dot.B <= 1 ? 1 : dot.B <= 2 ? 2 : dot.B <= 4 ? 4 : 8;
+    const int R = (dot.ld - 1 - dot.t) & 3;
+    dim3 grid(st.nchunk, (dot.D + dec::kDotWarps - 1) / dec::kDotWarps, (dot.B + BG - 1) / BG);
+    prof_begin(K_DECODE_STEP, s);
+    cudaError_t e = BG == 1 ? dot_bg<1>(dot, R, grid, s) : BG == 2 ? dot_bg<2>(dot, R, grid, s)
+                  : BG == 4 ? dot_bg<4>(dot, R, grid, s) : dot_bg<8>(dot, R, grid, s);
+    prof_end(K_DECODE_STEP, s);
+    if (e != cudaSuccess) return e;
+  }
+  const int rows = st.B * st.D;
+  prof_begin(K_DECODE_STEP, s);
+  dec::decode_step_kernel<<<(rows + dec::kStepWarps - 1) / dec::kStepWarps, 32 * dec::kStepWarps, 0, s>>>(st);
+  prof_end(K_DECODE_STEP, s);
+  return cudaGetLastError();
+}
+
+}  // namespace hy

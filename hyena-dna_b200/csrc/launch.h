@@ -4,6 +4,7 @@
 #include "filter_mlp.cuh"
 #include "short_conv.cuh"
 #include "layernorm_args.h"
+#include "decode_args.h"
 
 namespace hy {
 
@@ -18,7 +19,8 @@ enum Kind {
   K_ADD_LN = 28,            // residual add + LayerNorm (block glue, layernorm.cuh)
   K_FILTER_EXTRA = 29,      // deltas gradient / channel L1 normalisation (filter_extra.cuh; non-default filter options)
   K_PROJ_GEMM_GELU = 30, K_PROJ_GEMM_DGELU = 31, K_PROJ_WGRAD_GELU = 32,   // block MLP: projection GEMMs with fused GELU
-  K_COUNT = 33
+  K_DECODE_HIST = 33, K_DECODE_STEP = 34,   // incremental decoding (decode.cuh): history fill, one-position step
+  K_COUNT = 35
 };
 void prof_begin(int kind, cudaStream_t s);     // api.cu: records an event when profiling is on
 void prof_end(int kind, cudaStream_t s);       // api.cu: records an event when profiling is on; counts the launch
@@ -54,6 +56,9 @@ cudaError_t launch_l1norm_bwd(const float* dout, const float* out, const float* 
 int ln_partials(long long rows);                     // CTAs (= rows of the dw/db partial scratch) the kernels use for `rows`
 cudaError_t launch_add_ln_fwd(const ln::FwdArgs& a, cudaStream_t s);
 cudaError_t launch_add_ln_bwd(ln::BwdArgs a, float* dw, float* db, cudaStream_t s);
+// k_decode.cu: incremental decoding (decode.cuh)
+cudaError_t launch_decode_hist(const dec::HistArgs& a, cudaStream_t s);
+cudaError_t launch_decode_step(const dec::DotArgs& dot, const dec::StepArgs& st, cudaStream_t s);
 // k_convert.cu: reference filter-spectrum convention (rfft(k, fft_size), natural order) <-> packed spectrum
 cudaError_t launch_rfft_to_packed(const float2* X, float2* Z, int H, int logM, int logM1, cudaStream_t s);
 cudaError_t launch_packed_to_rfft(const float2* Z, float2* X, int H, int logM, int logM1, float scale, cudaStream_t s);

@@ -1,0 +1,120 @@
+"""Incremental decoding state of the causal Hyena operator (the reference leaves HyenaOperator.recurrence unimplemented,
+src/models/sequence/hyena.py:384-386, and ignores the ``inference_params`` that LMBackbone threads through,
+src/models/sequence/long_conv_lm.py:375-376).
+
+Output t of the causal recurrence o (hyena.py:414-423) is
+    out_o[t] = sum_{s<=t} k_o[t-s] g_o[s] + bias_o g_o[t],    g_o = v_o * x_{O-1-o},
+so extending a sequence by one position needs the gated inputs g_o of every earlier position, the filter k and the last
+two in_proj outputs (the state of the 3-tap short filter) -- not a forward over the whole sequence.  ``DecodeCache`` holds
+exactly that; ``HyenaOperator.prefill`` / ``step`` fill and use it (csrc/decode.cuh).
+
+The filter is generated once, at allocation, for Lcap = min(max_seqlen, l_max) positions.  That is valid for any shorter
+prefix: k[j] depends on position j only -- z and t are sliced per position, the modulation is per position and the
+``normalized`` option divides by the L1 norm over channels at each position (hyena.py:235-236).
+"""
+import torch
+
+from ._lib import HyenaB200Error
+
+CHUNK = 1024          # positions per partial dot product of a step (csrc/decode_args.h kChunk)
+
+
+def _ld(lcap):
+    return (lcap + 3) // 4 * 4
+
+
+def _chunks(lcap):
+    return (lcap + CHUNK - 1) // CHUNK
+
+
+class DecodeCache:
+    """Decoding state of one HyenaOperator (``HyenaOperator.allocate_decode_cache``), or of every mixer of a stack
+    (``Backbone.allocate_decode_cache``: ``layers`` holds one per layer, looked up by module identity).
+
+    Per operator, with O = order, D = d_model, F = (O-1) D filter channels, C = (O+1) D in_proj channels and ld = Lcap
+    rounded up to a multiple of 4 (all fp32, on the operator's device):
+      k     (F * ld + 4,)       the filter, each row time-reversed (k[c][j] at c*ld + ld-1-j) so that the step kernel streams
+                                history and filter in ascending order; 4 floats of padding
+      bias  (F,)                the effective filter bias (0 * bias when use_bias is false, as in forward)
+      h     (O-1, B, D, ld)     g_o of every recurrence by position
+      tail  (B, C, 2)           in_proj outputs (with bias) of the last two positions
+      s_t   (B, C)              short-filter outputs of the current position
+      part  (B, D, ceil(Lcap / 1024))  partial dot products of one step
+    ``t`` is the number of positions consumed so far."""
+
+    def __init__(self, owner=None, batch_size=0, max_seqlen=0, lcap=0, k=None, bias=None, h=None, tail=None, s_t=None,
+                 part=None, layers=None):
+        self.owner = owner
+        self.batch_size, self.max_seqlen, self.lcap = int(batch_size), int(max_seqlen), int(lcap)
+        self.k, self.bias, self.h, self.tail, self.s_t, self.part = k, bias, h, tail, s_t, part
+        self.layers = list(layers) if layers is not None else []
+        self._t = 0
+        if owner is not None:
+            self.d_model, self.order = owner.d_model, owner.order
+
+    @classmethod
+    def allocate(cls, op, batch_size, max_seqlen):
+        """Decoding state of ``op`` for ``batch_size`` rows and up to min(max_seqlen, op.l_max) positions."""
+        if op.filter_fn.bidirectional:
+            raise HyenaB200Error("decoding needs a causal filter; this HyenaFilter is bidirectional")
+        if batch_size < 1 or max_seqlen < 1:
+            raise HyenaB200Error(f"allocate_decode_cache: batch_size {batch_size} and max_seqlen {max_seqlen} must be >= 1")
+        w = op.in_proj.weight
+        if not w.is_cuda:
+            raise HyenaB200Error("decoding runs on CUDA sm_90a only; the operator's parameters are on the CPU")
+        B, D, O = int(batch_size), op.d_model, op.order
+        lcap = min(int(max_seqlen), op.l_max)
+        ld = _ld(lcap)
+        F = (O - 1) * D
+        dev = w.device
+        with torch.no_grad():
+            k = op.filter_fn.filter_channel_major(lcap)                  # (F, lcap)
+            krev = torch.zeros(F * ld + 4, dtype=torch.float32, device=dev)
+            krev[:F * ld].view(F, ld)[:, ld - lcap:] = k.flip(-1)
+            fb = op.filter_fn.bias if op.filter_fn.use_bias else 0 * op.filter_fn.bias
+            fb = fb.detach().reshape(-1).to(torch.float32).contiguous().clone()
+        h = torch.zeros(O - 1, B, D, ld, dtype=torch.float32, device=dev)
+        tail = torch.zeros(B, (O + 1) * D, 2, dtype=torch.float32, device=dev)
+        s_t = torch.zeros(B, (O + 1) * D, dtype=torch.float32, device=dev)
+        part = torch.zeros(B, D, _chunks(lcap), dtype=torch.float32, device=dev)
+        return cls(op, B, max_seqlen, lcap, krev, fb, h, tail, s_t, part)
+
+    @classmethod
+    def stack(cls, caches):
+        """One cache for several operators (one per layer of a stack), each found by ``for_module``."""
+        caches = list(caches)
+        if not caches:
+            raise HyenaB200Error("DecodeCache.stack needs at least one operator cache")
+        return cls(None, caches[0].batch_size, caches[0].max_seqlen, min(c.lcap for c in caches), layers=caches)
+
+    @staticmethod
+    def layout_nbytes(batch_size, d_model, order, lcap):
+        """Bytes one operator's cache takes (the layout in the class docstring)."""
+        B, D, O = batch_size, d_model, order
+        ld, F, C = _ld(lcap), (order - 1) * d_model, (order + 1) * d_model
+        return 4 * ((F * ld + 4) + F + (O - 1) * B * D * ld + B * C * 2 + B * C + B * D * _chunks(lcap))
+
+    @property
+    def nbytes(self):
+        if self.layers:
+            return sum(c.nbytes for c in self.layers)
+        return sum(x.numel() * x.element_size() for x in (self.k, self.bias, self.h, self.tail, self.s_t, self.part))
+
+    @property
+    def t(self):
+        return self.layers[0].t if self.layers else self._t
+
+    @t.setter
+    def t(self, value):
+        if self.layers:
+            raise HyenaB200Error("the position of a stack's cache is advanced by its layers")
+        self._t = int(value)
+
+    def for_module(self, module):
+        """The state of ``module`` (this cache itself, or the layer cache allocated for it)."""
+        if self.owner is module:
+            return self
+        for c in self.layers:
+            if c.owner is module:
+                return c
+        raise HyenaB200Error("this DecodeCache was not allocated for this HyenaOperator")

@@ -13,6 +13,7 @@ import torch.nn as nn
 
 from . import ops
 from ._lib import HyenaB200Error
+from .decode import DecodeCache
 
 
 class OptimModule(nn.Module):
@@ -334,6 +335,13 @@ class HyenaOperator(nn.Module):
                                      channels=1, dropout=filter_dropout, **filter_args)
 
     def forward(self, u, *args, **kwargs):
+        cache = kwargs.get("inference_params")
+        if isinstance(cache, DecodeCache):
+            # incremental decoding driven by the caller's model (LMBackbone passes inference_params to every mixer,
+            # long_conv_lm.py:375-376); any other inference_params object is ignored, as the reference does
+            c = cache.for_module(self)
+            y = self.prefill(u, c) if (c.t == 0 and u.shape[-2] > 1) else self.step(u, c)
+            return (y, None) if self.return_state else y
         if not u.is_cuda:
             raise HyenaB200Error("HyenaOperator (hyena_b200) runs on CUDA sm_90a only; there is no CPU fallback")
         in_dtype = u.dtype
@@ -369,14 +377,17 @@ class HyenaOperator(nn.Module):
             return y, None
         return y
 
-    def _forward_chained(self, u, k, fb, l_filter):
+    def _forward_chained(self, u, k, fb, l_filter, capture=None):
         """order >= 3 (the shipped HyenaDNA layer default is 3, configs/model/layer/hyena_dna.yaml:3): the recurrence of
         hyena.py:414-423 as a chain of this library's long convolutions.  Projections and every FFT convolution
         (forward and backward) run on the sm_90a kernels; the gates and the 3-tap short filter between them are
-        plain elementwise / depthwise torch ops here -- the fully fused pass exists for order 2 only."""
+        plain elementwise / depthwise torch ops here -- the fully fused pass exists for order 2 only.
+        ``capture`` (a dict) receives the in_proj output "p" and the gated input "g" of every recurrence (prefill)."""
         D, O1 = self.d_model, self.order - 1
         from .fftconv import fftconv_func
         p = _InProj.apply(u, self.in_proj.weight)                                   # (B, (order+1) D, l)
+        if capture is not None:
+            capture["p"], capture["g"] = p, []
         if l_filter < p.shape[-1]:
             p = p[..., :l_filter]
         p = p + self.in_proj.bias[None, :, None]
@@ -387,13 +398,93 @@ class HyenaOperator(nn.Module):
         bb = fb.reshape(D, O1)
         bidir = self.filter_fn.bidirectional
         for o, x_i in enumerate(reversed(x[1:])):
+            g = (v * x_i).contiguous()
+            if capture is not None:
+                capture["g"].append(g)
             if bidir:
                 from .fftconv import fftconv_ref
-                v = fftconv_ref((v * x_i).contiguous(), kk[:, o].contiguous(), bb[:, o].contiguous(), None, gelu=False,
-                                bidirectional=True)
+                v = fftconv_ref(g, kk[:, o].contiguous(), bb[:, o].contiguous(), None, gelu=False, bidirectional=True)
             else:
-                v = fftconv_func((v * x_i).contiguous(), kk[:, o].contiguous(), bb[:, o].contiguous(), gelu=False)
+                v = fftconv_func(g, kk[:, o].contiguous(), bb[:, o].contiguous(), gelu=False)
         return (v * x[0]).contiguous()
+
+    # ------------------------------------------------------------------------------ incremental decoding
+    def allocate_decode_cache(self, batch_size, max_seqlen):
+        """A DecodeCache for ``batch_size`` rows and up to min(max_seqlen, l_max) positions (decode.py)."""
+        return DecodeCache.allocate(self, batch_size, max_seqlen)
+
+    def _decode_checks(self, u, cache, n, fresh=False):
+        if not isinstance(cache, DecodeCache):
+            raise HyenaB200Error(f"decoding needs a DecodeCache (allocate_decode_cache), got {type(cache).__name__}")
+        c = cache.for_module(self)
+        if u.requires_grad:
+            raise HyenaB200Error("decoding is inference only: the input requires grad (run under torch.no_grad())")
+        if self.filter_fn.bidirectional:
+            raise HyenaB200Error("decoding needs a causal filter; this HyenaFilter is bidirectional")
+        if u.dim() != 3 or u.shape[-1] != self.d_model or u.shape[1] != n:
+            raise HyenaB200Error(f"decoding input must be (B, {n}, {self.d_model}); got {tuple(u.shape)}")
+        if u.shape[0] != c.batch_size:
+            raise HyenaB200Error(f"batch size {u.shape[0]} differs from the decode cache's {c.batch_size}")
+        if fresh and c.t != 0:
+            raise HyenaB200Error(f"prefill needs a fresh cache; this one is at position {c.t}")
+        if c.t + n > c.lcap:
+            raise HyenaB200Error(f"decoding past the cache: positions [{c.t}, {c.t + n}) exceed Lcap = min(max_seqlen, "
+                                 f"l_max) = {c.lcap} (l_max = {self.l_max}: the filter has no taps beyond it)")
+        if not u.is_cuda or not c.k.is_cuda:
+            raise HyenaB200Error("decoding runs on CUDA sm_90a only; there is no CPU fallback")
+        return c
+
+    def _decode_params(self):
+        C = self.short_filter.weight.shape[0]
+        return (self.in_proj.bias.detach().contiguous() if self.in_proj.bias is not None else None,
+                self.short_filter.weight.detach().reshape(C, -1).contiguous(), self.short_filter.bias.detach().contiguous())
+
+    def prefill(self, u, cache):
+        """Run the first P positions, u (B, P, D), and fill ``cache`` (which must be fresh) for stepping.  The output is
+        the one ``forward(u)`` gives, bit for bit: the same kernels run in the same order."""
+        c = self._decode_checks(u, cache, u.shape[1] if u.dim() == 3 else -1, fresh=True)
+        with torch.no_grad():
+            in_dtype = u.dtype
+            u32 = u.to(torch.float32)
+            P = u32.shape[1]
+            if self.order == 2:
+                y = self.forward(u)
+                y = y[0] if isinstance(y, tuple) else y
+                # the in_proj output the forward consumed (the projections are deterministic: same bits)
+                if ops.proj_mode() == "tc":
+                    p = ops.proj_gemm(u32.contiguous(), 0, self.in_proj.weight.contiguous(), False, 0)
+                else:
+                    p = _InProj.apply(u32, self.in_proj.weight)
+                gs = []
+            else:                               # forward's order >= 3 route, keeping its intermediates
+                k = self.filter_fn.filter_channel_major(P)
+                fb = self.filter_fn.bias if self.filter_fn.use_bias else 0 * self.filter_fn.bias
+                cap = {}
+                y_pre = self._forward_chained(u32, k, fb, P, capture=cap)
+                y = _OutProj.apply(y_pre, self.out_proj.weight, self.out_proj.bias).to(in_dtype)
+                p, gs = cap["p"], cap["g"]
+            ib, sw, sb = self._decode_params()
+            ops.decode_hist(p.contiguous(), ib, sw, sb, c)
+            for o in range(1, self.order - 1):
+                c.h[o, :, :, :P].copy_(gs[o])
+            c.t = P
+        return y
+
+    def step(self, u_t, cache):
+        """One position: u_t (B, 1, D) -> y (B, 1, D), the output at position ``cache.t``; advances the cache.  Stepping a
+        fresh cache starts the sequence (empty history).  The in_proj / out_proj products of one position are fp32
+        matrix-vector products (F.linear); the operator itself runs in csrc/decode.cuh, two launches per recurrence."""
+        c = self._decode_checks(u_t, cache, 1)
+        with torch.no_grad():
+            in_dtype = u_t.dtype
+            B, D = u_t.shape[0], self.d_model
+            u = u_t.to(torch.float32).reshape(B, D)
+            p_t = torch.nn.functional.linear(u, self.in_proj.weight).contiguous()          # bias added in the kernel
+            ib, sw, sb = self._decode_params()
+            y_pre = ops.decode_step(p_t, ib, sw, sb, c)
+            y = torch.nn.functional.linear(y_pre, self.out_proj.weight, self.out_proj.bias)
+            c.t += 1
+        return y.reshape(B, 1, D).to(in_dtype)
 
     @property
     def d_output(self):

@@ -700,3 +700,37 @@ class AddLayerNormFn(torch.autograd.Function):
 
 def add_layer_norm(x, res, weight, bias, eps):
     return AddLayerNormFn.apply(x, res, weight, bias, eps)
+
+
+# ------------------------------------------------------------------------------------------ incremental decoding
+def decode_hist(p, in_bias, sw, sb, cache):
+    """After a prefill of P positions: g_0 = short(v) * short(x_{O-1}) of positions [0, P) into cache.h[0] and the last two
+    in_proj outputs (with bias) into cache.tail (csrc/decode.cuh).  p (B, (O+1) D, P) without in_proj.bias."""
+    _need_cuda(p, in_bias, sw, sb)
+    B, C, P = p.shape
+    if not p.is_contiguous() or C != (cache.order + 1) * cache.d_model:
+        raise _lib.HyenaB200Error(f"decode_hist: p must be contiguous (B, {(cache.order + 1) * cache.d_model}, P)")
+    with torch.cuda.device(p.device):
+        _lib.check(_lib.lib().hyena_b200_decode_hist(
+            _ptr(p), _ptr(in_bias), _ptr(sw), _ptr(sb), _ptr(cache.h), _ptr(cache.tail), B, cache.batch_size,
+            cache.d_model, cache.order, P, cache.lcap, _stream()))
+
+
+def decode_step(p_t, in_bias, sw, sb, cache):
+    """One position: y_pre (B, D) of position cache.t from p_t (B, (O+1) D), the in_proj output without its bias.  Runs
+    the O-1 recurrences in order, two launches each (csrc/decode.cuh); does not advance cache.t."""
+    _need_cuda(p_t, in_bias, sw, sb)
+    B = p_t.shape[0]
+    D, O = cache.d_model, cache.order
+    if not p_t.is_contiguous() or tuple(p_t.shape) != (B, (O + 1) * D):
+        raise _lib.HyenaB200Error(f"decode_step: p_t must be contiguous (B, {(O + 1) * D})")
+    out = [torch.empty(B, D, dtype=torch.float32, device=p_t.device) for _ in range(O - 1)]
+    with torch.cuda.device(p_t.device):
+        for o in range(O - 1):
+            first = o == 0
+            _lib.check(_lib.lib().hyena_b200_decode_step(
+                _ptr(p_t) if first else 0, _ptr(in_bias) if first else 0, _ptr(sw) if first else 0,
+                _ptr(sb) if first else 0, _ptr(cache.k), _ptr(cache.bias), _ptr(cache.h[o]), _ptr(cache.tail) if first else 0,
+                _ptr(cache.s_t), 0 if first else _ptr(out[o - 1]), _ptr(out[o]), _ptr(cache.part), B, cache.batch_size, D, O,
+                o, int(cache.t), cache.lcap, _stream()))
+    return out[-1]

@@ -243,6 +243,29 @@ HY_API int hyena_b200_add_layernorm_bwd(const float* dy, const float* dres, cons
                                  const float* rstd, float* dx, float* dw, float* db, long long rows, int D, void* scratch,
                                  size_t scratch_bytes, void* stream);
 
+/* ---- incremental decoding of the causal operator -------------------------------------------------
+ * The reference leaves HyenaOperator.recurrence unimplemented (hyena.py:384-386).  Output t of recurrence o is
+ *     out_o[t] = sum_{s<=t} k_o[t-s] g_o[s] + fbias_o g_o[t],   g_o = v_o * x_{O-1-o},  v_0 = short(v),  v_{o+1} = out_o,
+ * and y_pre[t] = out_{O-2}[t] * x_0[t] (hyena.py:404-432, filter channels ordered (d o), :408-412).  O = order, C = (O+1) D,
+ * F = (O-1) D, Lcap = positions the cache holds (<= 2^20), ld = Lcap rounded up to a multiple of 4.  Cache buffers:
+ *   k     F * ld + 4 floats, 16-byte aligned: filter row c time-reversed, k_c[j] at k[c*ld + ld-1-j] (padding zero)
+ *   fbias (F) effective filter bias (0 * bias when use_bias is false)
+ *   h     (O-1, B, D, ld), 16-byte aligned: g_o by position       tail (B, C, 2): in_proj outputs (with bias) of the last two positions
+ *   s_t   (B, C) short-filter outputs of the current position      part (B, D, ceil(Lcap/1024)) scratch of one step
+ * cache_B is the batch size the cache was allocated for; a different B fails.
+ *   decode_hist: after a prefill of P positions, p (B, C, P) channel-major WITHOUT in_proj.bias (as for core_fwd):
+ *                g_0[0..P) -> h (recurrence 0's rows) and the tail.  Later recurrences' history is copied in by the caller.
+ *   decode_step: recurrence o of position t < Lcap.  o = 0 takes p_t (B, C) (in_proj output of position t without its
+ *                bias), runs the short filter from the tail, writes s_t and shifts the tail; v_in must be NULL.  o > 0 takes
+ *                v_in (B, D) = out of recurrence o-1.  h points at recurrence o's rows; g_o[t] is written there.  out (B, D)
+ *                = out_o[t], times x_0[t] for the last recurrence (= y_pre[t]).  Two launches (one at t = 0): a split dot
+ *                product over the history into part, then a fixed-order reduction and the epilogue; deterministic. */
+HY_API int hyena_b200_decode_hist(const float* p, const float* in_bias, const float* sw, const float* sb, float* h,
+                                  float* tail, int B, int cache_B, int D, int order, int P, int Lcap, void* stream);
+HY_API int hyena_b200_decode_step(const float* p_t, const float* in_bias, const float* sw, const float* sb, const float* k,
+                                  const float* fbias, float* h, float* tail, float* s_t, const float* v_in, float* out,
+                                  float* part, int B, int cache_B, int D, int order, int o, int t, int Lcap, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
