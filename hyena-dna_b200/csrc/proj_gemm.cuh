@@ -371,11 +371,16 @@ __global__ void __launch_bounds__(kThreads, 1) proj_gemm_kernel(const Args a, co
 //             wgrad_reduce_kernel (deterministic, no atomics).
 //   accuracy  the tensor core adds into its accumulator with truncation: a chain of n MMAs biases the sum by ~n 2^-24
 //             towards zero, and a slice here is thousands of MMAs long.  So the accumulator is restarted every kSeg chunks
-//             (the correction products of a chunk first, its hi*hi products last) and added into the CTA's partial in
-//             L2 with round-to-nearest adds.
+//             (the correction products of a chunk first, its hi*hi products last) and added into a running sum in
+//             registers with round-to-nearest adds; the CTA writes its partial once, at the end of its slice.
+//   registers acc 64 + sum 64 + A fragments 32 + next chunk's Y 16 per consumer thread: whole warpgroups, and moves
+//             registers from the converter and producer warpgroups to the consumers (setmaxnreg).
+//   overlap   the next chunk's Y values are loaded while this chunk's MMAs run; the converters fill the other image pair.
 namespace wg {
 
-constexpr int kThreads = 416;             // warps 0-7 two consumer warpgroups, 8-11 X -> B images, 12 TMA producer
+constexpr int kThreads = 512;             // warpgroups: 0, 1 consumers; 2 X -> B images; 3 TMA producer (one warp)
+constexpr int kRegConsumer = 184, kRegConvert = 88, kRegProducer = 56;   // setmaxnreg; 128 each at launch
+static_assert(2 * kRegConsumer + kRegConvert + kRegProducer <= 4 * 128, "register file of one CTA");
 constexpr int kSeg = 4;                   // chunks per accumulation segment (48 chained MMAs)
 constexpr int kStg = 4;                   // staged chunks in flight
 constexpr uint32_t kYPitch = 128 * 4;     // staged Y row: 128 columns, dense (= the TMA box)
@@ -441,48 +446,41 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const Args a, const 
 
   if (warp < 8) {
     // ---------------------------------------------------------------- consumers: rows n [64 wg, 64 wg + 64) of the tile
+    tc::setmaxnreg_inc<kRegConsumer>();
     const int wgi = warp >> 2, g = lane >> 2, t = lane & 3;
     const int nl0 = 64 * wgi + 16 * (warp & 3) + g;                     // fragment rows nl0, nl0 + 8
-    float acc[64];
-    auto drain = [&](bool first) {                                      // partial += acc (round-to-nearest adds)
+    float acc[64], sum[64], yv[4][4];
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int nl = nl0 + 8 * h;
-        if (nl >= nrows) continue;
-        float* dst = a.part + ((size_t)split * a.N + n0 + nl) * a.M + m0;
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const int ml = 8 * j + 2 * t;
-#pragma unroll
-          for (int e = 0; e < 2; ++e)
-            if (ml + e < mcols) dst[ml + e] = acc[4 * j + 2 * h + e] + (first ? 0.f : dst[ml + e]);
-        }
-      }
-    };
-    if (nchunks == 0) {
-#pragma unroll
-      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-      drain(true);
-    }
-    for (long long q = 0; q < nchunks; ++q) {
+    for (int i = 0; i < 64; ++i) sum[i] = 0.f;
+    // this thread's A-fragment values of chunk q from the staged Y tile; the slot is released once they have arrived
+    auto load_y = [&](long long q) {
       const int ss = (int)(q % kStg);
       tc::mbar_wait_u(S_FULL(ss), (uint32_t)(q / kStg) & 1u);            // the producer's copies of this chunk have landed
       const unsigned char* st = smem + kOffY + (size_t)ss * kYStage;
-      uint32_t ahi[4][4], alo[4][4];
       uint32_t dep = 0;
 #pragma unroll
       for (int ks = 0; ks < 4; ++ks) {
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
           const int nl = nl0 + ((e & 1) ? 8 : 0), k = 8 * ks + t + ((e & 2) ? 4 : 0);
-          const float v = *reinterpret_cast<const float*>(st + k * kYPitch + nl * 4);
-          dep |= __float_as_uint(v);
-          float h, lw;
-          tc::split_tf32(v, h, lw);
-          ahi[ks][e] = __float_as_uint(h); alo[ks][e] = __float_as_uint(lw);
+          yv[ks][e] = *reinterpret_cast<const float*>(st + k * kYPitch + nl * 4);
+          dep |= __float_as_uint(yv[ks][e]);
         }
       }
       tc::mbar_arrive_after_loads(Y_EMPTY(ss), dep, a.zero);            // staged Y tile consumed: the producer may refill it
+    };
+    if (nchunks > 0) load_y(0);
+    for (long long q = 0; q < nchunks; ++q) {
+      uint32_t ahi[4][4], alo[4][4];
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          float h, lw;
+          tc::split_tf32(yv[ks][e], h, lw);
+          ahi[ks][e] = __float_as_uint(h); alo[ks][e] = __float_as_uint(lw);
+        }
+      }
       const uint32_t it = (uint32_t)q;
       const int s = it & 1;
       tc::mbar_wait_u(B_FULL(s), (it >> 1) & 1);
@@ -499,14 +497,35 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const Args a, const 
       for (int ks = 0; ks < 4; ++ks)                                    // main: hi * hi
         tc::wgmma_rs_n128(acc, ahi[ks], tc::make_desc_ls(bhi + ks * 2 * pg::kLBO, pg::kLBO, pg::kSBO), 1u);
       tc::wgmma_commit();
+      if (q + 1 < nchunks) load_y(q + 1);                               // under this chunk's MMAs
       tc::wgmma_wait<0>();
       tc::fence_regs(acc);
+      tc::fence_frags(ahi);                                             // read by the MMAs up to here
+      tc::fence_frags(alo);
       __syncwarp();
       if (lane == 0) tc::mbar_arrive(B_EMPTY(s));                       // the image pair is free
-      if (it % kSeg == kSeg - 1 || q + 1 == nchunks) drain(it < kSeg);
+      if (it % kSeg == kSeg - 1 || q + 1 == nchunks) {                  // end of a segment: sum += acc (round to nearest)
+#pragma unroll
+        for (int i = 0; i < 64; ++i) sum[i] = acc[i] + sum[i];
+      }
+    }
+    // the CTA's partial, written once (zero for an empty slice)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int nl = nl0 + 8 * h;
+      if (nl >= nrows) continue;
+      float* dst = a.part + ((size_t)split * a.N + n0 + nl) * a.M + m0;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int ml = 8 * j + 2 * t;
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (ml + e < mcols) dst[ml + e] = sum[4 * j + 2 * h + e];
+      }
     }
   } else if (warp < 12) {
     // ---------------------------------------------------------------- B side: X rows -> K-major hi / lo images
+    tc::setmaxnreg_dec<kRegConvert>();
     const int t = tid - 256;
     const bool use_fir = a.fir != nullptr;
     // this thread converts pieces (row r, quad k4) with r % 8 == t % 8: the eight lanes of a quarter warp then write one
@@ -561,6 +580,8 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const Args a, const 
     }
   } else {
     // ---------------------------------------------------------------- producer: Y and X tiles of every chunk (TMA)
+    tc::setmaxnreg_dec<kRegProducer>();
+    if (warp != 12) return;
     if (lane == 0 && a.vec) { tc::tma_prefetch_desc(&tmapX); tc::tma_prefetch_desc(&tmapY); }
     int sb_ = (int)(c_begin / a.chunks_per_b), sl_ = (int)(c_begin - (long long)sb_ * a.chunks_per_b) * 32;
     for (long long q = 0; q < nchunks; ++q) {

@@ -46,6 +46,22 @@ __device__ __forceinline__ void fence_regs(float (&d)[R]) {
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+// same for register A fragments read by wgmma in flight: keeps them (and their registers) live up to this point
+template <int R, int C>
+__device__ __forceinline__ void fence_frags(uint32_t (&a)[R][C]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i)
+#pragma unroll
+    for (int j = 0; j < C; ++j) asm volatile("" : "+r"(a[i][j])::"memory");
+}
+
+// per-warpgroup register reallocation (all four warps of a warpgroup execute it): warp-specialised kernels give the
+// registers of their lightly loaded producer warps to the consumer warpgroups
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+
 __device__ __forceinline__ void wgmma_ss_n8(float (&d)[4], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
