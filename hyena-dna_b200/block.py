@@ -71,6 +71,10 @@ class Block(nn.Module):
         position depends on that position only, so the block keeps no state of its own."""
         return self._decode(hidden_states, residual, lambda y: self.mixer.step(y, cache))
 
+    def extend(self, hidden_states, residual, cache):
+        """forward of n more positions (B, n, D) from the mixer's DecodeCache (HyenaOperator.extend)."""
+        return self._decode(hidden_states, residual, lambda y: self.mixer.extend(y, cache))
+
     def _decode(self, hidden_states, residual, mix):
         if not hasattr(self.mixer, "step"):
             raise HyenaB200Error(f"Block: the mixer {type(self.mixer).__name__} has no incremental decoding")
@@ -123,6 +127,10 @@ class Backbone(nn.Module):
     def step(self, hidden_states, cache):
         """The output of one more position (B, 1, D)."""
         return self._decode(hidden_states, cache, "step")
+
+    def extend(self, hidden_states, cache):
+        """The outputs of n more positions (B, n, D); on a fresh cache this is prefill."""
+        return self._decode(hidden_states, cache, "extend")
 
     def _decode(self, hidden_states, cache, how):
         if hidden_states.requires_grad:

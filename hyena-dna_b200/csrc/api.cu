@@ -279,7 +279,8 @@ HY_API const char* hyena_b200_kind_name(int kind) {
       "filter_fwd", "filter_bwd", "short_conv_bwd", "twiddle_init", "filter_tc_prep", "filter_tc_fwd", "filter_tc_bwd", "filter_tc_red", "fused_conv_fwd",
       "spectrum_convert", "proj_prep", "proj_gemm", "proj_wgrad",
       "conv_fwd<pipelined>", "conv_bwd<pipelined>", "filter_spectrum<pipelined>", "add_layer_norm", "filter_extra",
-      "proj_gemm<gelu>", "proj_gemm<dgelu>", "proj_wgrad<gelu>", "decode_hist", "decode_step"};
+      "proj_gemm<gelu>", "proj_gemm<dgelu>", "proj_wgrad<gelu>", "decode_hist", "decode_step",
+      "decode_extend_hist", "decode_extend_dot", "decode_extend_combine"};
   return (kind >= 0 && kind < K_COUNT) ? names[kind] : "?";
 }
 
@@ -811,6 +812,59 @@ HY_API int hyena_b200_decode_step(const float* p_t, const float* in_bias, const 
                    ld, p_t, in_bias, sw, sb, tail, s_t, v_in, h, out, B, D, (order + 1) * D, order, t, (order - 1 - o) * D,
                    o == order - 2};
   HY_CUDA(launch_decode_step(dot, st, (cudaStream_t)stream));
+  return 0;
+}
+
+/* extending a decode cache by n positions at once (decode_extend.cuh) */
+static int check_extend_range(int t, int n, int Lcap) {
+  HY_CHECK(n >= 1, "extend of %d positions: n must be >= 1", n);
+  HY_CHECK(t >= 0 && t <= Lcap - n, "positions [%d, %d) outside the decode cache [0, %d)", t, t + n, Lcap);
+  return 0;
+}
+
+HY_API int hyena_b200_decode_extend_groups(int B, int D, int t, int n) {
+  if (B < 1 || D < 1 || t < 0 || n < 1) return 0;
+  return dec::ext_groups(B, D, t, n);
+}
+
+HY_API int hyena_b200_decode_extend_hist(const float* p, const float* in_bias, const float* sw, const float* sb, float* h,
+                                         float* tail, float* s, int B, int cache_B, int D, int order, int t, int n, int Lcap,
+                                         void* stream) {
+  if (check_decode_shape(B, cache_B, D, order, Lcap) || check_extend_range(t, n, Lcap)) return 1;
+  HY_CHECK(p && sw && sb && h && tail && s, "null pointer");
+  dec::ExtHistArgs a{p, in_bias, sw, sb, tail, s, h, B, D, (order + 1) * D, t, n, dec::ld_for(Lcap), (order - 1) * D};
+  HY_CUDA(launch_decode_ext_hist(a, (cudaStream_t)stream));
+  return 0;
+}
+
+HY_API int hyena_b200_decode_extend_dot(const float* h, const float* k, float* part, int groups, int B, int cache_B, int D,
+                                        int order, int o, int t, int n, int Lcap, void* stream) {
+  if (check_decode_shape(B, cache_B, D, order, Lcap) || check_extend_range(t, n, Lcap)) return 1;
+  HY_CHECK(h && k && part, "null pointer");
+  HY_CHECK(o >= 0 && o < order - 1, "recurrence %d outside [0, %d)", o, order - 1);
+  HY_CHECK(groups == dec::ext_groups(B, D, t, n), "partials sized for %d groups; this extend needs %d "
+           "(hyena_b200_decode_extend_groups)", groups, dec::ext_groups(B, D, t, n));
+  HY_CHECK(aligned16(k) && aligned16(h), "k and h must be 16-byte aligned");
+  const int ld = dec::ld_for(Lcap), F = order - 1;
+  const int NT = dec::ext_tile(n);
+  dec::ExtDotArgs a{h, k + (size_t)o * ld, part, B, D, t, n, ld, F * ld, (-t) & 3, (n + NT - 1) / NT,
+                    dec::ext_chunks_per_cta(B, D, t, n), dec::chunks_for(t + n), groups};
+  HY_CUDA(launch_decode_ext_dot(a, (cudaStream_t)stream));
+  return 0;
+}
+
+HY_API int hyena_b200_decode_extend_combine(const float* part, long long row_stride, int j_stride, int groups,
+                                            const float* fbias, const float* h, const float* s, float* out, int B,
+                                            int cache_B, int D, int order, int o, int t, int n, int Lcap, void* stream) {
+  if (check_decode_shape(B, cache_B, D, order, Lcap) || check_extend_range(t, n, Lcap)) return 1;
+  HY_CHECK(part && fbias && h && s && out, "null pointer");
+  HY_CHECK(o >= 0 && o < order - 1, "recurrence %d outside [0, %d)", o, order - 1);
+  HY_CHECK(groups >= 1 && j_stride >= 0 && row_stride >= 0, "bad partial layout: groups %d, strides %lld / %d", groups,
+           row_stride, j_stride);
+  const int ld = dec::ld_for(Lcap), last = o == order - 2;
+  dec::ExtCombineArgs a{part, row_stride, j_stride, groups, fbias + o, order - 1, h, s, last ? nullptr : out,
+                        last ? out : nullptr, B, D, (order + 1) * D, t, n, ld, (order - 2 - o) * D, last};
+  HY_CUDA(launch_decode_ext_combine(a, (cudaStream_t)stream));
   return 0;
 }
 

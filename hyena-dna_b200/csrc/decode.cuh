@@ -15,13 +15,10 @@
 #include <cuda_runtime.h>
 
 #include "decode_args.h"
+#include "decode_common.cuh"
 
 namespace hy {
 namespace dec {
-
-__device__ __forceinline__ float short3(float w0, float w1, float w2, float b, float pm2, float pm1, float p0) {
-  return fmaf(w0, pm2, fmaf(w1, pm1, fmaf(w2, p0, b)));
-}
 
 // g[t] = short(v)[t] * short(x_gate)[t] for t < P into h (row stride ld); tail = P(P-2), P(P-1) of every channel
 __global__ void __launch_bounds__(256) decode_hist_kernel(const HistArgs a) {
@@ -50,8 +47,6 @@ __global__ void __launch_bounds__(256) decode_hist_kernel(const HistArgs a) {
     tl[1] = pc[a.P - 1] + ib;
   }
 }
-
-__device__ __forceinline__ float4 ld4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
 
 // part[b][d][chunk] = sum_{s in chunk, s < t} h[b][d][s] k[t-s]   for the batch rows [z*BG, z*BG + BG)
 template <int BG, int R>

@@ -8,6 +8,8 @@
 //   tail  (B, C, 2)           in_proj outputs (with bias) of the last two positions: the 3-tap short filter's state
 //   s_t   (B, C)              short-filter outputs of the current position (written by recurrence 0, read by the later ones)
 //   part  (B, D, ceil(Lcap/1024)) partial dot products of one step
+// Extending by n positions (Ext* below) uses per-call scratch: the short-filter outputs (B, C, n) and the partials of the
+// direct Toeplitz kernel (B, D, n, ext_groups()).  The cache layout is the same.
 #pragma once
 
 namespace hy {
@@ -56,6 +58,67 @@ struct StepArgs {
   float* out;            // (B, D) recurrence output; times x0 when `last`
   int B, D, C, order, t;
   int gate;              // channel offset of this recurrence's gate: (O-1-o) D
+  int last;
+};
+
+// ---- extending a cache by n positions at once (decode_extend.cuh)
+constexpr int kExtRJ = 8;                 // outputs per thread of the direct Toeplitz kernel (register block)
+constexpr int kExtWarps = 8;              // warps per CTA of the direct Toeplitz kernel
+constexpr int kExtTargetCtas = 4096;      // the direct kernel merges 1024-position chunks per CTA down to about this many CTAs
+
+inline int ext_tile(int n) { return n <= 8 ? 8 : 64; }        // outputs per CTA of the direct kernel (8 or 64)
+inline int ext_bg(int B) { return B <= 1 ? 1 : B <= 2 ? 2 : B <= 4 ? 4 : 8; }
+
+// chunks per CTA of the direct kernel for (B, D, history t, n new positions); the partials have ext_groups() entries per
+// output: ceil(chunks / chunks_per_cta)
+inline int ext_chunks_per_cta(int B, int D, int t, int n) {
+  const int nchunk = chunks_for(t + n);
+  const int njt = (n + ext_tile(n) - 1) / ext_tile(n), bg = ext_bg(B);
+  const long long base = (long long)njt * D * ((B + bg - 1) / bg);
+  long long want = kExtTargetCtas / base;
+  if (want < 1) want = 1;
+  if (want > nchunk) want = nchunk;
+  return (int)((nchunk + want - 1) / want);
+}
+inline int ext_groups(int B, int D, int t, int n) {
+  const int cpb = ext_chunks_per_cta(B, D, t, n);
+  return (chunks_for(t + n) + cpb - 1) / cpb;
+}
+
+struct ExtHistArgs {
+  const float* p;        // (B, C, n) in_proj output of positions [t, t+n) without its bias, channel-major
+  const float* in_bias;  // (C) or null
+  const float* sw;       // (C, 3)
+  const float* sb;       // (C)
+  float* tail;           // (B, C, 2): read as the state before position t, left as the state after position t+n-1
+  float* s;              // (B, C, n) short-filter outputs of the n positions
+  float* h;              // (B, D, ld) history of recurrence 0: g_0 of positions [t, t+n) written
+  int B, D, C, t, n, ld;
+  int gate;              // channel offset of the gate of recurrence 0: (O-1) D
+};
+
+struct ExtDotArgs {
+  const float* h;        // (B, D, ld) history of this recurrence, positions [0, t+n) valid
+  const float* k;        // reversed filter row of channel d of this recurrence: k + d * kstride
+  float* part;           // (B, D, n, groups)
+  int B, D, t, n, ld, kstride;
+  int R;                 // (-t) mod 4: misalignment of every filter window (see decode_ext_dot_kernel)
+  int njt;               // output tiles of the kernel's tile size: ceil(n / NT)
+  int cpb, nchunk, groups;
+};
+
+struct ExtCombineArgs {
+  const float* part;     // sum over g < groups of part[row * prow + j * pj + g] = sum_{s<=t+j} k[t+j-s] g_o[s]
+  long long prow;
+  int pj, groups;
+  const float* fbias;    // effective filter bias of channel d: fbias[d * fstride]
+  int fstride;
+  const float* h;        // (B, D, ld) history of this recurrence (g_o[t+j] for the bias term)
+  const float* s;        // (B, C, n) short-filter outputs (the gates)
+  float* h_next;         // (B, D, ld) history of the next recurrence: g_{o+1} = out * x_{O-2-o}, or null when `last`
+  float* y;              // (B, D, n): out * x_0 when `last`
+  int B, D, C, t, n, ld;
+  int xch;               // channel offset of the gate that multiplies the output: (O-2-o) D
   int last;
 };
 

@@ -20,7 +20,8 @@ enum Kind {
   K_FILTER_EXTRA = 29,      // deltas gradient / channel L1 normalisation (filter_extra.cuh; non-default filter options)
   K_PROJ_GEMM_GELU = 30, K_PROJ_GEMM_DGELU = 31, K_PROJ_WGRAD_GELU = 32,   // block MLP: projection GEMMs with fused GELU
   K_DECODE_HIST = 33, K_DECODE_STEP = 34,   // incremental decoding (decode.cuh): history fill, one-position step
-  K_COUNT = 35
+  K_DECODE_EXT_HIST = 35, K_DECODE_EXT_DOT = 36, K_DECODE_EXT_COMBINE = 37,   // extending by n positions (decode_extend.cuh)
+  K_COUNT = 38
 };
 void prof_begin(int kind, cudaStream_t s);     // api.cu: records an event when profiling is on
 void prof_end(int kind, cudaStream_t s);       // api.cu: records an event when profiling is on; counts the launch
@@ -59,6 +60,10 @@ cudaError_t launch_add_ln_bwd(ln::BwdArgs a, float* dw, float* db, cudaStream_t 
 // k_decode.cu: incremental decoding (decode.cuh)
 cudaError_t launch_decode_hist(const dec::HistArgs& a, cudaStream_t s);
 cudaError_t launch_decode_step(const dec::DotArgs& dot, const dec::StepArgs& st, cudaStream_t s);
+// k_decode_extend.cu: extending a decode cache by n positions (decode_extend.cuh)
+cudaError_t launch_decode_ext_hist(const dec::ExtHistArgs& a, cudaStream_t s);
+cudaError_t launch_decode_ext_dot(const dec::ExtDotArgs& a, cudaStream_t s);
+cudaError_t launch_decode_ext_combine(const dec::ExtCombineArgs& a, cudaStream_t s);
 // k_convert.cu: reference filter-spectrum convention (rfft(k, fft_size), natural order) <-> packed spectrum
 cudaError_t launch_rfft_to_packed(const float2* X, float2* Z, int H, int logM, int logM1, cudaStream_t s);
 cudaError_t launch_packed_to_rfft(const float2* Z, float2* X, int H, int logM, int logM1, float scale, cudaStream_t s);

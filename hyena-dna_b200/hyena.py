@@ -339,8 +339,11 @@ class HyenaOperator(nn.Module):
         if isinstance(cache, DecodeCache):
             # incremental decoding driven by the caller's model (LMBackbone passes inference_params to every mixer,
             # long_conv_lm.py:375-376); any other inference_params object is ignored, as the reference does
+            # a fresh cache takes several positions as a prefill, one position is a step, several positions on a cache
+            # that already holds history extend it
             c = cache.for_module(self)
-            y = self.prefill(u, c) if (c.t == 0 and u.shape[-2] > 1) else self.step(u, c)
+            n = u.shape[-2]
+            y = self.prefill(u, c) if (c.t == 0 and n > 1) else self.step(u, c) if n == 1 else self.extend(u, c)
             return (y, None) if self.return_state else y
         if not u.is_cuda:
             raise HyenaB200Error("HyenaOperator (hyena_b200) runs on CUDA sm_90a only; there is no CPU fallback")
@@ -485,6 +488,32 @@ class HyenaOperator(nn.Module):
             y = torch.nn.functional.linear(y_pre, self.out_proj.weight, self.out_proj.bias)
             c.t += 1
         return y.reshape(B, 1, D).to(in_dtype)
+
+    def extend(self, u, cache):
+        """n >= 1 more positions at once: u (B, n, D) -> y (B, n, D), the outputs at positions [cache.t, cache.t + n);
+        advances the cache by n.  On a fresh cache this is ``prefill`` (bit-identical to ``forward``).  Otherwise in_proj and
+        out_proj of the chunk run on the wgmma projection GEMM and every recurrence on csrc/decode_extend.cuh: the direct
+        Toeplitz kernel over the cached history, or for large n the FFT convolution of the whole history
+        (ops.decode_extend_uses_fft chooses from t and n)."""
+        n = u.shape[1] if u.dim() == 3 else -1
+        if n < 1:
+            raise HyenaB200Error(f"extend input must be (B, n, {self.d_model}) with n >= 1; got {tuple(u.shape)}")
+        c = self._decode_checks(u, cache, n)
+        if c.t == 0:
+            return self.prefill(u, c)
+        return self._extend(u, c, ops.decode_extend)
+
+    def _extend(self, u, c, core):
+        """extend on a non-fresh cache with ``core`` (ops.decode_extend or one of its two routes) for the operator."""
+        with torch.no_grad():
+            in_dtype, n = u.dtype, u.shape[1]
+            p = ops.proj_gemm(u.to(torch.float32).contiguous(), 0, self.in_proj.weight.detach().contiguous(), False, 0)
+            ib, sw, sb = self._decode_params()
+            y_pre = core(p, ib, sw, sb, c)                                              # (B, D, n)
+            b = self.out_proj.bias.detach().contiguous() if self.out_proj.bias is not None else None
+            y = ops.proj_gemm(y_pre, 1, self.out_proj.weight.detach().contiguous(), False, 1, bias=b)
+            c.t += n
+        return y.to(in_dtype)
 
     @property
     def d_output(self):

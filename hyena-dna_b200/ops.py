@@ -734,3 +734,96 @@ def decode_step(p_t, in_bias, sw, sb, cache):
                 _ptr(cache.s_t), 0 if first else _ptr(out[o - 1]), _ptr(out[o]), _ptr(cache.part), B, cache.batch_size, D, O,
                 o, int(cache.t), cache.lcap, _stream()))
     return out[-1]
+
+
+# ------------------------------------------------------------------------------------------ extending by n positions
+# Direct (decode_ext_dot_kernel) against FFT route (fftconv_forward over the whole t + n history).  The direct kernel reads
+# the history and the filter once and does n FMAs per position and channel: memory-bound for small n, then its time grows
+# with n; the FFT route costs O((t+n) log(t+n)) whatever n.  tools/bench_extend.py on an H100 (DESIGN.md section 4.10, B = 1,
+# D = 256): at t = 2^14, 2^17 and 2^20 the direct route is faster (or even, at 2^20) for n <= 256 and the FFT route for
+# n >= 1024, so the threshold sits between them.
+EXTEND_FFT_MIN_N = 512
+
+
+def decode_extend_uses_fft(t, n):
+    """True when extending a history of t positions by n runs on the FFT route, False for the direct Toeplitz kernel."""
+    return int(n) >= EXTEND_FFT_MIN_N
+
+
+def _extend_check(p, cache, what):
+    _need_cuda(p)
+    B, C, n = p.shape if p.dim() == 3 else (0, 0, 0)
+    D, O = cache.d_model, cache.order
+    if p.dim() != 3 or not p.is_contiguous() or C != (O + 1) * D or n < 1:
+        raise _lib.HyenaB200Error(f"{what}: p must be contiguous (B, {(O + 1) * D}, n >= 1); got {tuple(p.shape)}")
+    return B, n
+
+
+def decode_extend_hist(p, in_bias, sw, sb, cache):
+    """Short filter of the n positions [cache.t, cache.t + n) from p (B, (O+1) D, n), the in_proj output without its bias,
+    carried in from cache.tail -> s (B, (O+1) D, n); writes g_0 of the n positions into cache.h[0] and shifts the tail.  Does
+    not advance cache.t."""
+    _need_cuda(in_bias, sw, sb)
+    B, n = _extend_check(p, cache, "decode_extend_hist")
+    s = torch.empty_like(p)
+    with torch.cuda.device(p.device):
+        _lib.check(_lib.lib().hyena_b200_decode_extend_hist(
+            _ptr(p), _ptr(in_bias), _ptr(sw), _ptr(sb), _ptr(cache.h), _ptr(cache.tail), _ptr(s), B, cache.batch_size,
+            cache.d_model, cache.order, int(cache.t), n, cache.lcap, _stream()))
+    return s
+
+
+def _extend_combine(part, row_stride, j_stride, groups, s, out, o, B, n, cache):
+    with torch.cuda.device(s.device):
+        _lib.check(_lib.lib().hyena_b200_decode_extend_combine(
+            _ptr(part), int(row_stride), int(j_stride), int(groups), _ptr(cache.bias), _ptr(cache.h[o]), _ptr(s), _ptr(out),
+            B, cache.batch_size, cache.d_model, cache.order, o, int(cache.t), n, cache.lcap, _stream()))
+
+
+def _decode_extend(p, in_bias, sw, sb, cache, fft):
+    B, n = _extend_check(p, cache, "decode_extend")
+    D, O, t = cache.d_model, cache.order, int(cache.t)
+    L, ld = t + n, cache.h.shape[-1]
+    s = decode_extend_hist(p, in_bias, sw, sb, cache)
+    y = torch.empty(B, D, n, dtype=torch.float32, device=p.device)
+    if fft:
+        krev = cache.k[:(O - 1) * D * ld].view(D, O - 1, ld)
+        zero = torch.zeros(D, dtype=torch.float32, device=p.device)
+    else:
+        groups = int(_lib.lib().hyena_b200_decode_extend_groups(B, D, t, n))
+        part = torch.empty(B, D, n, groups, dtype=torch.float32, device=p.device)
+    for o in range(O - 1):
+        out = y if o == O - 2 else cache.h[o + 1]
+        if fft:
+            # the cache keeps k reversed and h with row stride ld: the convolution wants both forward and compact (O(t)
+            # copies beside the O(t log t) transform); it recomputes all t + n outputs and keeps the last n
+            k = krev[:, o, ld - L:].flip(-1).contiguous()
+            conv = fftconv_forward(cache.h[o, :, :, :L].contiguous(), filter_spectrum(k), zero)
+            _extend_combine(conv[:, :, t:], L, 1, 1, s, out, o, B, n, cache)
+        else:
+            with torch.cuda.device(p.device):
+                _lib.check(_lib.lib().hyena_b200_decode_extend_dot(
+                    _ptr(cache.h[o]), _ptr(cache.k), _ptr(part), groups, B, cache.batch_size, D, O, o, t, n, cache.lcap,
+                    _stream()))
+            _extend_combine(part, n * groups, groups, groups, s, out, o, B, n, cache)
+    return y
+
+
+def decode_extend_direct(p, in_bias, sw, sb, cache):
+    """y_pre (B, D, n) of the positions [cache.t, cache.t + n) from p (B, (O+1) D, n), the in_proj output without its bias,
+    on the direct Toeplitz kernel: per recurrence one decode_ext_dot_kernel over the history and one combine
+    (csrc/decode_extend.cuh).  Writes the n positions into the cache's history and tail; does not advance cache.t."""
+    return _decode_extend(p, in_bias, sw, sb, cache, fft=False)
+
+
+def decode_extend_fft(p, in_bias, sw, sb, cache):
+    """decode_extend_direct on the FFT route: per recurrence, the causal convolution of the whole history [0, t + n) with
+    the first t + n filter taps (filter_spectrum + fftconv_forward), then the same combine kernel."""
+    return _decode_extend(p, in_bias, sw, sb, cache, fft=True)
+
+
+def decode_extend(p, in_bias, sw, sb, cache):
+    """decode_extend_direct or decode_extend_fft, as decode_extend_uses_fft(cache.t, n) selects."""
+    n = p.shape[-1]
+    fn = decode_extend_fft if decode_extend_uses_fft(cache.t, n) else decode_extend_direct
+    return fn(p, in_bias, sw, sb, cache)

@@ -266,6 +266,26 @@ HY_API int hyena_b200_decode_step(const float* p_t, const float* in_bias, const 
                                   const float* fbias, float* h, float* tail, float* s_t, const float* v_in, float* out,
                                   float* part, int B, int cache_B, int D, int order, int o, int t, int Lcap, void* stream);
 
+/* ---- extending a decode cache by n >= 1 positions [t, t+n), t + n <= Lcap (chunked prefill, continuation scoring) ----
+ *   decode_extend_hist:    p (B, C, n) in_proj output of the n positions WITHOUT in_proj.bias -> s (B, C, n) short-filter
+ *                          outputs (carried in from the tail), g_0[t, t+n) -> h (recurrence 0's rows); shifts the tail.
+ *   decode_extend_groups:  the partial count per output of decode_extend_dot for (B, D, t, n) (0 for a bad shape).
+ *   decode_extend_dot:     direct Toeplitz product of recurrence o: part (B, D, n, groups), summed over groups =
+ *                          sum_{s<=t+j} k_o[t+j-s] g_o[s] over h[0, t+n), which must already hold g_o of the n positions.
+ *   decode_extend_combine: out_o[t+j] = sum_g part[row * row_stride + j * j_stride + g] + fbias_o g_o[t+j], times the gate
+ *                          s[(O-2-o) D + d][j]: into the rows of recurrence o+1 (out = its h) or, for the last recurrence,
+ *                          y_pre (B, D, n) (out).  part may also be a full convolution (groups 1: the FFT route).
+ * Deterministic: fixed summation orders, no atomics. */
+HY_API int hyena_b200_decode_extend_groups(int B, int D, int t, int n);
+HY_API int hyena_b200_decode_extend_hist(const float* p, const float* in_bias, const float* sw, const float* sb, float* h,
+                                         float* tail, float* s, int B, int cache_B, int D, int order, int t, int n, int Lcap,
+                                         void* stream);
+HY_API int hyena_b200_decode_extend_dot(const float* h, const float* k, float* part, int groups, int B, int cache_B, int D,
+                                        int order, int o, int t, int n, int Lcap, void* stream);
+HY_API int hyena_b200_decode_extend_combine(const float* part, long long row_stride, int j_stride, int groups,
+                                            const float* fbias, const float* h, const float* s, float* out, int B,
+                                            int cache_B, int D, int order, int o, int t, int n, int Lcap, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
