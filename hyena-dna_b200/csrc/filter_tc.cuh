@@ -521,8 +521,7 @@ filter_tc_bwd_kernel(const FilterParams P, const float* __restrict__ wimg, const
 // ---------------------------------------------------------------------------------------------- backward, stage 2
 // All parameter gradients of the filter are reductions over the sequence.  With the stage-1 arrays stored feature-
 // major every operand is K-major with K = position, so they are three accumulating wgmma GEMM groups whose fp32
-// accumulators stay in registers for the whole kernel (persistent CTAs, split over the sequence, one atomic
-// flush at the end):
+// accumulators stay in registers (persistent CTAs, split over the sequence, an atomic flush every kRedChain K blocks):
 //   G1  dW3[c][j]      = sum_t dh[c][t] a3[j][t]                       M = 128 channels per tile (<= 2 tiles), N = 64
 //   G2  [dp3;dp2] x [a2;a1;1]^T : block(0,0) = dW2, block(1,1) = dW1, column 128 = (db2 ; db1)     M = 128, N = 144
 //   G3  [dp1;X]  x [z;1]^T      : rows 0..63 -> (dW0 | db0), rows 64..127 col 8 -> dfreq             M = 128, N = 16
@@ -545,8 +544,8 @@ constexpr uint32_t kRedOffBz = kRedOffBs + 36864;                  // [z pad 8; 
 constexpr uint32_t kRedOffMisc = kRedOffBz + 4096;
 constexpr size_t kRedSmemBytes = kRedOffMisc + 64;
 
-// D (+)= A * B^T over one K block of 32 positions as 3xTF32, all products into one accumulator (a per-block sum here is
-// tiny next to the accumulated value, and the chain is split into three groups that each see a fraction of the blocks)
+// D (+)= A * B^T over one K block of 32 positions as 3xTF32, all products into one accumulator (restarted every
+// kRedChain blocks, see below)
 template <int R>
 __device__ __forceinline__ void issue_red(float (&d)[R], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo, uint32_t first_acc) {
   uint32_t acc = first_acc;
@@ -620,6 +619,45 @@ __device__ __forceinline__ RedItem red_item(const RedArgs& R, int it, int tid) {
   return m;
 }
 
+// K blocks per accumulator chain.  The tensor core truncates every add into its accumulator, so a chain of n MMAs biases
+// the sum towards zero by ~n 2^-24 of its magnitude: one chain through a CTA's whole slice of a 2^20-position sequence
+// (~250 blocks x 12 MMAs) put same-sign sums 8.5e-5 (relative) off, 100x the error of an fp32 library GEMM.  So every
+// kRedChain blocks the accumulators are flushed into the gradients with round-to-nearest atomic adds and restarted.
+// Shorter chains trade the bias for more atomic adds per gradient element (their own rounding) and time: on an H100
+// (400 W) at L = 2^20, D = 256 the kernel took 5.4 ms with one chain, 5.65 ms with 8 blocks, 6.0 ms with 4, 7.3 ms with 2.
+constexpr int kRedChain = 8;
+
+// accumulators -> gradients (fragment element i: row f.row(i) of the group, column f.col(i, n_half))
+__device__ __forceinline__ void red_flush(const RedArgs& R, const Frag& f, int nmt, const float (&g1)[2][16],
+                                          const float (&g2)[36], const float (&g3)[4]) {
+  for (int mt = 0; mt < nmt; ++mt) {                       // G1: dW3 rows c = 128 mt + row, 64 columns
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const int c = mt * 128 + f.row(i);
+      if (c < R.D) atomicAdd(R.dW3 + (size_t)c * 64 + f.col(i, 32), g1[mt][i]);
+    }
+  }
+  // G2: rows < 64: cols 0..63 -> dW2[row][j]; rows >= 64: cols 64..127 -> dW1[row-64][j]; col 128 -> db2 / db1
+#pragma unroll
+  for (int i = 0; i < 36; ++i) {
+    const int r = f.row(i), n = f.col(i, 72);
+    if (n == 128) atomicAdd(((r < 64) ? R.db2 : R.db1) + (r & 63), g2[i]);
+    else if (r < 64 && n < 64) atomicAdd(R.dW2 + r * 64 + n, g2[i]);
+    else if (r >= 64 && n >= 64 && n < 128) atomicAdd(R.dW1 + (r - 64) * 64 + (n - 64), g2[i]);
+  }
+  // G3: rows < 64: cols 0..E-1 -> dW0[row][e], col 8 -> db0[row]; rows >= 64: col 8 -> dfreq[row-64]
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int r = f.row(i), n = f.col(i, 8);
+    if (r < 64) {
+      if (n < R.E) atomicAdd(R.dW0 + r * R.E + n, g3[i]);
+      else if (n == 8) atomicAdd(R.db0 + r, g3[i]);
+    } else if (n == 8) {
+      atomicAdd(R.dfreq + (r - 64), g3[i]);
+    }
+  }
+}
+
 __global__ void __launch_bounds__(kRedThreads, 1) filter_tc_red_kernel(const RedArgs R, int nblocks) {
   extern __shared__ __align__(1024) unsigned char smem[];
   const int tid = threadIdx.x;
@@ -646,7 +684,8 @@ __global__ void __launch_bounds__(kRedThreads, 1) filter_tc_red_kernel(const Red
   // accumulators of this warpgroup: rows 64 rh .. of every group, column half ch
   float g1[2][16], g2[36], g3[4];
   const uint32_t arow = (uint32_t)f.rh * 8u * kRedSBO;
-  bool first = true;
+  bool first = true;                                       // no MMA issued yet
+  int chain = 0;                                           // K blocks in the accumulators since their last flush
   for (int blk = blockIdx.x; blk < nblocks; blk += gridDim.x) {
     const size_t t = (size_t)blk * kRedKB + 4 * pc;
     if (!first) {                                          // previous MMAs have read the images
@@ -677,7 +716,7 @@ __global__ void __launch_bounds__(kRedThreads, 1) filter_tc_red_kernel(const Red
     }
     fence_async_smem();
     __syncthreads();
-    const uint32_t acc0 = first ? 0u : 1u;
+    const uint32_t acc0 = chain ? 1u : 0u;
     wgmma_fence();
     fence_regs(g1[0]); fence_regs(g1[1]); fence_regs(g2); fence_regs(g3);
 #pragma unroll
@@ -691,38 +730,17 @@ __global__ void __launch_bounds__(kRedThreads, 1) filter_tc_red_kernel(const Red
               sbase + kRedOffBz + 2048 + f.ch * kRedSBO, acc0);
     wgmma_commit();
     first = false;
+    if (++chain == kRedChain) {                            // the images stay untouched until the barrier at the loop top
+      wgmma_wait<0>();
+      fence_regs(g1[0]); fence_regs(g1[1]); fence_regs(g2); fence_regs(g3);
+      red_flush(R, f, nmt, g1, g2, g3);
+      chain = 0;
+    }
   }
-  if (first) return;
+  if (chain == 0) return;
   wgmma_wait<0>();
   fence_regs(g1[0]); fence_regs(g1[1]); fence_regs(g2); fence_regs(g3);
-
-  // ---- flush (fragment element i: row f.row(i) of the group, column f.col(i, n_half))
-  for (int mt = 0; mt < nmt; ++mt) {                       // G1: dW3 rows c = 128 mt + row, 64 columns
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      const int c = mt * 128 + f.row(i);
-      if (c < R.D) atomicAdd(R.dW3 + (size_t)c * 64 + f.col(i, 32), g1[mt][i]);
-    }
-  }
-  // G2: rows < 64: cols 0..63 -> dW2[row][j]; rows >= 64: cols 64..127 -> dW1[row-64][j]; col 128 -> db2 / db1
-#pragma unroll
-  for (int i = 0; i < 36; ++i) {
-    const int r = f.row(i), n = f.col(i, 72);
-    if (n == 128) atomicAdd(((r < 64) ? R.db2 : R.db1) + (r & 63), g2[i]);
-    else if (r < 64 && n < 64) atomicAdd(R.dW2 + r * 64 + n, g2[i]);
-    else if (r >= 64 && n >= 64 && n < 128) atomicAdd(R.dW1 + (r - 64) * 64 + (n - 64), g2[i]);
-  }
-  // G3: rows < 64: cols 0..E-1 -> dW0[row][e], col 8 -> db0[row]; rows >= 64: col 8 -> dfreq[row-64]
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int r = f.row(i), n = f.col(i, 8);
-    if (r < 64) {
-      if (n < R.E) atomicAdd(R.dW0 + r * R.E + n, g3[i]);
-      else if (n == 8) atomicAdd(R.db0 + r, g3[i]);
-    } else if (n == 8) {
-      atomicAdd(R.dfreq + (r - 64), g3[i]);
-    }
-  }
+  red_flush(R, f, nmt, g1, g2, g3);
 }
 
 }  // namespace tc
