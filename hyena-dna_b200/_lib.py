@@ -62,6 +62,7 @@ SIGNATURES = {
                              _i, ctypes.c_longlong, _i, c_fp, _i, _vp, _sz, _vp]),
     "hyena_b200_decode_hist": (_i, [c_fp] * 6 + [_i] * 6 + [_vp]),
     "hyena_b200_decode_step": (_i, [c_fp] * 12 + [_i] * 7 + [_vp]),
+    "hyena_b200_decode_win_step": (_i, [c_fp] * 13 + [_i] * 10 + [_vp]),
     "hyena_b200_decode_extend_groups": (_i, [_i] * 4),
     "hyena_b200_decode_extend_hist": (_i, [c_fp] * 7 + [_i] * 7 + [_vp]),
     "hyena_b200_decode_extend_dot": (_i, [c_fp] * 3 + [_i] * 9 + [_vp]),

@@ -280,7 +280,7 @@ HY_API const char* hyena_b200_kind_name(int kind) {
       "spectrum_convert", "proj_prep", "proj_gemm", "proj_wgrad",
       "conv_fwd<pipelined>", "conv_bwd<pipelined>", "filter_spectrum<pipelined>", "add_layer_norm", "filter_extra",
       "proj_gemm<gelu>", "proj_gemm<dgelu>", "proj_wgrad<gelu>", "decode_hist", "decode_step",
-      "decode_extend_hist", "decode_extend_dot", "decode_extend_combine"};
+      "decode_extend_hist", "decode_extend_dot", "decode_extend_combine", "decode_win_step"};
   return (kind >= 0 && kind < K_COUNT) ? names[kind] : "?";
 }
 
@@ -812,6 +812,31 @@ HY_API int hyena_b200_decode_step(const float* p_t, const float* in_bias, const 
                    ld, p_t, in_bias, sw, sb, tail, s_t, v_in, h, out, B, D, (order + 1) * D, order, t, (order - 1 - o) * D,
                    o == order - 2};
   HY_CUDA(launch_decode_step(dot, st, (cudaStream_t)stream));
+  return 0;
+}
+
+HY_API int hyena_b200_decode_win_step(const float* p_t, const float* in_bias, const float* sw, const float* sb,
+                                      const float* k, const float* fbias, float* h, float* tail, float* s_t,
+                                      const float* v_in, float* out, float* part, const float* win, int B, int cache_B,
+                                      int D, int order, int o, int t, int b, int Wc, int W, int Lcap, void* stream) {
+  if (check_decode_shape(B, cache_B, D, order, Lcap)) return 1;
+  HY_CHECK(k && fbias && h && s_t && out && part && win, "null pointer");
+  HY_CHECK(o >= 0 && o < order - 1, "recurrence %d outside [0, %d)", o, order - 1);
+  HY_CHECK(o == 0 ? (p_t && sw && sb && tail && !v_in) : (v_in != nullptr),
+           o == 0 ? "null pointer: recurrence 0 needs p_t, sw, sb, tail (and no v_in)" : "null pointer: v_in");
+  HY_CHECK(b >= 0 && (b & 3) == 0, "window base %d must be a non-negative multiple of 4", b);
+  HY_CHECK(Wc >= 1 && Wc <= W && b <= Lcap - Wc, "window [%d, %d) of width %d outside the decode cache [0, %d)", b,
+           b + Wc, W, Lcap);
+  HY_CHECK(t - b >= 0 && t - b < Wc, "position %d outside the window [%d, %d)", t, b, b + Wc);
+  const int ld = dec::ld_for(Lcap);
+  HY_CHECK(aligned16(k) && aligned16(h), "k and h must be 16-byte aligned");
+  const int F = order - 1;
+  dec::DotArgs dot{h + b, k + (size_t)o * ld, part, B, D, t - b, ld, F * ld, dec::chunks_for(Lcap)};
+  dec::WinStepArgs w{{part, (t - b + dec::kChunk - 1) / dec::kChunk, dec::chunks_for(Lcap), k + (size_t)o * ld, fbias + o,
+                      F * ld, F, ld, p_t, in_bias, sw, sb, tail, s_t, v_in, h, out, B, D, (order + 1) * D, order, t,
+                      (order - 1 - o) * D, o == order - 2},
+                     win, W, t - b};
+  HY_CUDA(launch_decode_win_step(dot, w, (cudaStream_t)stream));
   return 0;
 }
 

@@ -10,6 +10,8 @@
 //                          template parameter: two aligned float4 loads are funnelled into the four values a lane needs
 //   decode_step_kernel     one warp per (b, channel): fixed-order reduction of the chunk partials, the short filter of
 //                          position t from the tail (recurrence 0), the gates, g[t] into the history, the epilogue
+//   decode_win_step_kernel decode_step_kernel inside an open window [b, b + Wc): the partials cover only [b, t) (the dot
+//                          kernel run on h + b with t - b) and the precomputed F[t-b] = sum_{s<b} k[t-s] g[s] is added
 // fp32 throughout, no atomics: every sum has a fixed order, so a step is bitwise reproducible.
 #pragma once
 #include <cuda_runtime.h>
@@ -101,17 +103,18 @@ __global__ void __launch_bounds__(32 * kDotWarps) decode_dot_kernel(const DotArg
   }
 }
 
-__global__ void __launch_bounds__(32 * kStepWarps) decode_step_kernel(const StepArgs a) {
-  const int lane = threadIdx.x & 31;
-  const int row = blockIdx.x * kStepWarps + (threadIdx.x >> 5);      // b * D + d
-  if (row >= a.B * a.D) return;
-  const int b = row / a.D, d = row - b * a.D;
-  // fixed-order reduction of the chunk partials: lane-strided chains, then a butterfly
+// fixed-order reduction of the chunk partials of one (b, channel) row: lane-strided chains, then a butterfly
+__device__ __forceinline__ float reduce_partials(const StepArgs& a, int row, int lane) {
   float acc = 0.f;
   const float* part = a.part + (size_t)row * a.nchunk_max;
   for (int i = lane; i < a.nchunk; i += 32) acc += part[i];
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  return acc;
+}
+
+// everything of a step at position t once acc = sum_{s<t} k[t-s] g[s] is known (one warp per (b, channel) row)
+__device__ __forceinline__ void step_epilogue(const StepArgs& a, int row, int b, int d, int lane, float acc) {
   float v, gate, x0;
   if (a.v_in == nullptr) {
     // recurrence 0: lane j < O+1 runs the short filter of channel j D + d from the tail and p_t, and shifts the tail
@@ -143,6 +146,26 @@ __global__ void __launch_bounds__(32 * kStepWarps) decode_step_kernel(const Step
     y = fmaf(a.fbias[(size_t)d * a.fstride], g, y);
     a.out[row] = a.last ? y * x0 : y;
   }
+}
+
+__global__ void __launch_bounds__(32 * kStepWarps) decode_step_kernel(const StepArgs a) {
+  const int lane = threadIdx.x & 31;
+  const int row = blockIdx.x * kStepWarps + (threadIdx.x >> 5);      // b * D + d
+  if (row >= a.B * a.D) return;
+  const int b = row / a.D, d = row - b * a.D;
+  const float acc = reduce_partials(a, row, lane);
+  step_epilogue(a, row, b, d, lane, acc);
+}
+
+// a step inside an open window: the partials of the window positions [b, t), then F[t-b] (the history before b), then
+// the same epilogue as decode_step_kernel; the summation order is fixed, so a windowed step is bitwise reproducible
+__global__ void __launch_bounds__(32 * kStepWarps) decode_win_step_kernel(const WinStepArgs w) {
+  const int lane = threadIdx.x & 31;
+  const int row = blockIdx.x * kStepWarps + (threadIdx.x >> 5);      // b * D + d
+  if (row >= w.st.B * w.st.D) return;
+  const int b = row / w.st.D, d = row - b * w.st.D;
+  const float acc = reduce_partials(w.st, row, lane) + w.win[(size_t)row * w.wstride + w.j];
+  step_epilogue(w.st, row, b, d, lane, acc);
 }
 
 }  // namespace dec

@@ -8,6 +8,7 @@
 //   tail  (B, C, 2)           in_proj outputs (with bias) of the last two positions: the 3-tap short filter's state
 //   s_t   (B, C)              short-filter outputs of the current position (written by recurrence 0, read by the later ones)
 //   part  (B, D, ceil(Lcap/1024)) partial dot products of one step
+// A windowed step (WinStepArgs below) also reads the window's history tail F (O-1, B, D, W), kept beside the cache.
 // Extending by n positions (Ext* below) uses per-call scratch: the short-filter outputs (B, C, n) and the partials of the
 // direct Toeplitz kernel (B, D, n, ext_groups()).  The cache layout is the same.
 #pragma once
@@ -59,6 +60,16 @@ struct StepArgs {
   int B, D, C, order, t;
   int gate;              // channel offset of this recurrence's gate: (O-1-o) D
   int last;
+};
+
+// A windowed step at position t in the window [b, b + Wc) (b a multiple of 4): st.part / st.nchunk hold the partials of
+// sum_{b<=s<t} h[s] k[t-s] (decode_dot_kernel on h + b with t - b), and win the precomputed history tail
+// F[j] = sum_{s<b} k[b+j-s] h[s] of the window positions j in [0, Wc)
+struct WinStepArgs {
+  StepArgs st;
+  const float* win;      // (B, D, wstride) F of this recurrence
+  int wstride;           // W >= Wc
+  int j;                 // t - b
 };
 
 // ---- extending a cache by n positions at once (decode_extend.cuh)

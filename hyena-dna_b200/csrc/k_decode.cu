@@ -25,22 +25,42 @@ static cudaError_t dot_bg(const dec::DotArgs& a, int R, dim3 grid, cudaStream_t 
   return cudaGetLastError();
 }
 
+// the split dot product over dot.t positions in nchunk chunks
+static cudaError_t launch_dot(const dec::DotArgs& dot, int nchunk, int kind, cudaStream_t s) {
+  const int BG = dot.B <= 1 ? 1 : dot.B <= 2 ? 2 : dot.B <= 4 ? 4 : 8;
+  const int R = (dot.ld - 1 - dot.t) & 3;
+  dim3 grid(nchunk, (dot.D + dec::kDotWarps - 1) / dec::kDotWarps, (dot.B + BG - 1) / BG);
+  prof_begin(kind, s);
+  cudaError_t e = BG == 1 ? dot_bg<1>(dot, R, grid, s) : BG == 2 ? dot_bg<2>(dot, R, grid, s)
+                : BG == 4 ? dot_bg<4>(dot, R, grid, s) : dot_bg<8>(dot, R, grid, s);
+  prof_end(kind, s);
+  return e;
+}
+
 // one recurrence of one step: the split dot product over the history (skipped at t = 0), then the combine kernel
 cudaError_t launch_decode_step(const dec::DotArgs& dot, const dec::StepArgs& st, cudaStream_t s) {
   if (st.nchunk > 0) {
-    const int BG = dot.B <= 1 ? 1 : dot.B <= 2 ? 2 : dot.B <= 4 ? 4 : 8;
-    const int R = (dot.ld - 1 - dot.t) & 3;
-    dim3 grid(st.nchunk, (dot.D + dec::kDotWarps - 1) / dec::kDotWarps, (dot.B + BG - 1) / BG);
-    prof_begin(K_DECODE_STEP, s);
-    cudaError_t e = BG == 1 ? dot_bg<1>(dot, R, grid, s) : BG == 2 ? dot_bg<2>(dot, R, grid, s)
-                  : BG == 4 ? dot_bg<4>(dot, R, grid, s) : dot_bg<8>(dot, R, grid, s);
-    prof_end(K_DECODE_STEP, s);
+    cudaError_t e = launch_dot(dot, st.nchunk, K_DECODE_STEP, s);
     if (e != cudaSuccess) return e;
   }
   const int rows = st.B * st.D;
   prof_begin(K_DECODE_STEP, s);
   dec::decode_step_kernel<<<(rows + dec::kStepWarps - 1) / dec::kStepWarps, 32 * dec::kStepWarps, 0, s>>>(st);
   prof_end(K_DECODE_STEP, s);
+  return cudaGetLastError();
+}
+
+// one recurrence of a windowed step: the dot product over the window positions [b, t) (skipped at t = b), then the
+// windowed combine kernel
+cudaError_t launch_decode_win_step(const dec::DotArgs& dot, const dec::WinStepArgs& w, cudaStream_t s) {
+  if (w.st.nchunk > 0) {
+    cudaError_t e = launch_dot(dot, w.st.nchunk, K_DECODE_WIN_STEP, s);
+    if (e != cudaSuccess) return e;
+  }
+  const int rows = w.st.B * w.st.D;
+  prof_begin(K_DECODE_WIN_STEP, s);
+  dec::decode_win_step_kernel<<<(rows + dec::kStepWarps - 1) / dec::kStepWarps, 32 * dec::kStepWarps, 0, s>>>(w);
+  prof_end(K_DECODE_WIN_STEP, s);
   return cudaGetLastError();
 }
 

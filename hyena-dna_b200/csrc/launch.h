@@ -21,7 +21,8 @@ enum Kind {
   K_PROJ_GEMM_GELU = 30, K_PROJ_GEMM_DGELU = 31, K_PROJ_WGRAD_GELU = 32,   // block MLP: projection GEMMs with fused GELU
   K_DECODE_HIST = 33, K_DECODE_STEP = 34,   // incremental decoding (decode.cuh): history fill, one-position step
   K_DECODE_EXT_HIST = 35, K_DECODE_EXT_DOT = 36, K_DECODE_EXT_COMBINE = 37,   // extending by n positions (decode_extend.cuh)
-  K_COUNT = 38
+  K_DECODE_WIN_STEP = 38,   // a step inside an open window (decode.cuh): its dot product and combine kernel
+  K_COUNT = 39
 };
 void prof_begin(int kind, cudaStream_t s);     // api.cu: records an event when profiling is on
 void prof_end(int kind, cudaStream_t s);       // api.cu: records an event when profiling is on; counts the launch
@@ -60,6 +61,7 @@ cudaError_t launch_add_ln_bwd(ln::BwdArgs a, float* dw, float* db, cudaStream_t 
 // k_decode.cu: incremental decoding (decode.cuh)
 cudaError_t launch_decode_hist(const dec::HistArgs& a, cudaStream_t s);
 cudaError_t launch_decode_step(const dec::DotArgs& dot, const dec::StepArgs& st, cudaStream_t s);
+cudaError_t launch_decode_win_step(const dec::DotArgs& dot, const dec::WinStepArgs& w, cudaStream_t s);
 // k_decode_extend.cu: extending a decode cache by n positions (decode_extend.cuh)
 cudaError_t launch_decode_ext_hist(const dec::ExtHistArgs& a, cudaStream_t s);
 cudaError_t launch_decode_ext_dot(const dec::ExtDotArgs& a, cudaStream_t s);

@@ -40,7 +40,12 @@ class DecodeCache:
       tail  (B, C, 2)           in_proj outputs (with bias) of the last two positions
       s_t   (B, C)              short-filter outputs of the current position
       part  (B, D, ceil(Lcap / 1024))  partial dot products of one step
-    ``t`` is the number of positions consumed so far."""
+    ``t`` is the number of positions consumed so far.
+
+    Window state of the windowed step (ops.decode_window_plan, DESIGN.md section 4.11): a window [win_b, win_b + win_wc)
+    is valid while win_b <= t < win_b + win_wc; ``win_f`` (O-1, B, D, W) holds F_o[j] = sum_{s < win_b} k_o[win_b+j-s]
+    g_o[s] for j < win_wc.  F depends on h[:, :, :, :win_b] only, so an extend inside the window leaves it valid.  It is
+    allocated at the first refresh (``window_nbytes``).  ``steps`` counts the steps since the last prefill or extend."""
 
     def __init__(self, owner=None, batch_size=0, max_seqlen=0, lcap=0, k=None, bias=None, h=None, tail=None, s_t=None,
                  part=None, layers=None):
@@ -49,6 +54,7 @@ class DecodeCache:
         self.k, self.bias, self.h, self.tail, self.s_t, self.part = k, bias, h, tail, s_t, part
         self.layers = list(layers) if layers is not None else []
         self._t = 0
+        self.win_b, self.win_wc, self.win_f, self.steps = 0, 0, None, 0
         if owner is not None:
             self.d_model, self.order = owner.d_model, owner.order
 
@@ -99,6 +105,17 @@ class DecodeCache:
         if self.layers:
             return sum(c.nbytes for c in self.layers)
         return sum(x.numel() * x.element_size() for x in (self.k, self.bias, self.h, self.tail, self.s_t, self.part))
+
+    @property
+    def window_nbytes(self):
+        """Bytes of the windowed step's history tails (0 until the first window opens); not part of ``nbytes``."""
+        if self.layers:
+            return sum(c.window_nbytes for c in self.layers)
+        return 0 if self.win_f is None else self.win_f.numel() * self.win_f.element_size()
+
+    def reset_window(self):
+        """Close the window and restart the step count (a prefill starts a new sequence)."""
+        self.win_b, self.win_wc, self.steps = 0, 0, 0
 
     @property
     def t(self):

@@ -471,12 +471,15 @@ class HyenaOperator(nn.Module):
             for o in range(1, self.order - 1):
                 c.h[o, :, :, :P].copy_(gs[o])
             c.t = P
+            c.reset_window()
         return y
 
     def step(self, u_t, cache):
         """One position: u_t (B, 1, D) -> y (B, 1, D), the output at position ``cache.t``; advances the cache.  Stepping a
         fresh cache starts the sequence (empty history).  The in_proj / out_proj products of one position are fp32
-        matrix-vector products (F.linear); the operator itself runs in csrc/decode.cuh, two launches per recurrence."""
+        matrix-vector products (F.linear); the operator itself runs in csrc/decode.cuh, two launches per recurrence.  After
+        a run of steps at a long history the step reads only the positions of a window opened by one FFT refresh
+        (ops.decode_window_plan chooses)."""
         c = self._decode_checks(u_t, cache, 1)
         with torch.no_grad():
             in_dtype = u_t.dtype
@@ -484,7 +487,7 @@ class HyenaOperator(nn.Module):
             u = u_t.to(torch.float32).reshape(B, D)
             p_t = torch.nn.functional.linear(u, self.in_proj.weight).contiguous()          # bias added in the kernel
             ib, sw, sb = self._decode_params()
-            y_pre = ops.decode_step(p_t, ib, sw, sb, c)
+            y_pre = ops.decode_step_auto(p_t, ib, sw, sb, c)
             y = torch.nn.functional.linear(y_pre, self.out_proj.weight, self.out_proj.bias)
             c.t += 1
         return y.reshape(B, 1, D).to(in_dtype)
@@ -513,6 +516,7 @@ class HyenaOperator(nn.Module):
             b = self.out_proj.bias.detach().contiguous() if self.out_proj.bias is not None else None
             y = ops.proj_gemm(y_pre, 1, self.out_proj.weight.detach().contiguous(), False, 1, bias=b)
             c.t += n
+            c.steps = 0
         return y.to(in_dtype)
 
     @property

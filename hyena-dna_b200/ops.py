@@ -736,6 +736,100 @@ def decode_step(p_t, in_bias, sw, sb, cache):
     return out[-1]
 
 
+# ------------------------------------------------------------------------------------------ windowed steps
+# A plain step reads the whole history [0, t).  Inside a window [b, b + Wc) a step reads [b, t) and adds
+# F_o[t-b] = sum_{s<b} k_o[t-s] g_o[s], computed for the whole window at once by one FFT convolution of the history
+# (the refresh).  HyenaOperator.step opens a window once the cache is long enough and the last WINDOW_AFTER_STEPS operations
+# on it were steps: the refresh costs about that many plain steps, so a caller that goes on stepping pays at most about twice
+# the cheaper route and one that mixes a few steps with extends pays no refresh.  Derivation from tools/bench_generate.py in
+# DESIGN.md section 4.11.
+WINDOW = 4096                # positions per window (W)
+WINDOW_MIN_T = 1 << 16       # no window below this history: a plain step there is bound by launch latency
+WINDOW_AFTER_STEPS = 16      # consecutive steps before a window opens
+
+
+def decode_window_plan(t, lcap, steps, win_b=0, win_wc=0):
+    """Route of a step at position t of a cache with Lcap = lcap whose last ``steps`` operations were steps and whose
+    window is [win_b, win_b + win_wc) (win_wc = 0: none): "window" (the window holds t), "refresh" (open the window
+    decode_window_bounds(t, lcap) first, then step in it) or "plain"."""
+    if win_wc > 0 and win_b <= t < win_b + win_wc:
+        return "window"
+    if t >= WINDOW_MIN_T and steps >= WINDOW_AFTER_STEPS and t < lcap:
+        return "refresh"
+    return "plain"
+
+
+def decode_window_bounds(t, lcap):
+    """(b, Wc) of the window a refresh at position t opens: b = t rounded down to a multiple of 4 (history rows stay 16-byte
+    aligned), Wc = min(WINDOW, lcap - b)."""
+    b = int(t) - int(t) % 4
+    return b, min(WINDOW, int(lcap) - b)
+
+
+def _history_conv(cache, o, hist, L):
+    """Causal convolution of g_o[0, hist) (zero from hist on) with the first L filter taps of recurrence o -> (B, D, L), on the
+    library's filter_spectrum + fftconv_forward with a zero skip term.  The cache keeps k reversed and h with row stride ld,
+    so the filter rows are un-reversed and the history compacted or zero-padded first (O(L) copies beside the transforms);
+    h is not read at positions >= hist."""
+    D, O, ld = cache.d_model, cache.order, cache.h.shape[-1]
+    k = cache.k[:(O - 1) * D * ld].view(D, O - 1, ld)[:, o, ld - L:].flip(-1).contiguous()
+    if hist == L:
+        u = cache.h[o, :, :, :L].contiguous()
+    else:
+        u = torch.zeros(cache.h.shape[1], D, L, dtype=torch.float32, device=cache.h.device)
+        u[:, :, :hist] = cache.h[o, :, :, :hist]
+    zero = torch.zeros(D, dtype=torch.float32, device=u.device)
+    return fftconv_forward(u, filter_spectrum(k), zero)
+
+
+def decode_window_refresh(cache):
+    """Open the window [b, b + Wc) = decode_window_bounds(cache.t, cache.lcap): per recurrence, F_o = outputs [b, b + Wc) of
+    the causal convolution of g_o[0, b) with the first b + Wc filter taps, into cache.win_f (allocated (O-1, B, D, WINDOW)
+    on first use).  Reads the history below b only."""
+    b, wc = decode_window_bounds(cache.t, cache.lcap)
+    if wc < 1:
+        raise _lib.HyenaB200Error(f"decode_window_refresh: position {cache.t} leaves no room for a window (Lcap {cache.lcap})")
+    O, B, D = cache.order, cache.batch_size, cache.d_model
+    if cache.win_f is None or cache.win_f.shape[-1] < wc:
+        cache.win_f = None
+        cache.win_f = torch.empty(O - 1, B, D, max(WINDOW, wc), dtype=torch.float32, device=cache.h.device)
+    for o in range(O - 1):
+        cache.win_f[o, :, :, :wc] = _history_conv(cache, o, b, b + wc)[:, :, b:]
+    cache.win_b, cache.win_wc = b, wc
+
+
+def decode_win_step(p_t, in_bias, sw, sb, cache):
+    """decode_step at a position cache.t inside the open window: per recurrence the dot product over the window positions
+    [b, t) and decode_win_step_kernel, which adds F_o[t-b] (csrc/decode.cuh); does not advance cache.t."""
+    _need_cuda(p_t, in_bias, sw, sb)
+    B = p_t.shape[0]
+    D, O = cache.d_model, cache.order
+    if not p_t.is_contiguous() or tuple(p_t.shape) != (B, (O + 1) * D):
+        raise _lib.HyenaB200Error(f"decode_win_step: p_t must be contiguous (B, {(O + 1) * D})")
+    W = 0 if cache.win_f is None else cache.win_f.shape[-1]
+    out = [torch.empty(B, D, dtype=torch.float32, device=p_t.device) for _ in range(O - 1)]
+    with torch.cuda.device(p_t.device):
+        for o in range(O - 1):
+            first = o == 0
+            _lib.check(_lib.lib().hyena_b200_decode_win_step(
+                _ptr(p_t) if first else 0, _ptr(in_bias) if first else 0, _ptr(sw) if first else 0,
+                _ptr(sb) if first else 0, _ptr(cache.k), _ptr(cache.bias), _ptr(cache.h[o]), _ptr(cache.tail) if first else 0,
+                _ptr(cache.s_t), 0 if first else _ptr(out[o - 1]), _ptr(out[o]), _ptr(cache.part),
+                0 if cache.win_f is None else _ptr(cache.win_f[o]), B, cache.batch_size, D, O, o, int(cache.t),
+                cache.win_b, cache.win_wc, W, cache.lcap, _stream()))
+    return out[-1]
+
+
+def decode_step_auto(p_t, in_bias, sw, sb, cache):
+    """One step on the route decode_window_plan selects (refreshing the window first when it says so); counts the step."""
+    route = decode_window_plan(cache.t, cache.lcap, cache.steps, cache.win_b, cache.win_wc)
+    if route == "refresh":
+        decode_window_refresh(cache)
+    y = decode_step(p_t, in_bias, sw, sb, cache) if route == "plain" else decode_win_step(p_t, in_bias, sw, sb, cache)
+    cache.steps += 1
+    return y
+
+
 # ------------------------------------------------------------------------------------------ extending by n positions
 # Direct (decode_ext_dot_kernel) against FFT route (fftconv_forward over the whole t + n history).  The direct kernel reads
 # the history and the filter once and does n FMAs per position and channel: memory-bound for small n, then its time grows
@@ -786,19 +880,14 @@ def _decode_extend(p, in_bias, sw, sb, cache, fft):
     L, ld = t + n, cache.h.shape[-1]
     s = decode_extend_hist(p, in_bias, sw, sb, cache)
     y = torch.empty(B, D, n, dtype=torch.float32, device=p.device)
-    if fft:
-        krev = cache.k[:(O - 1) * D * ld].view(D, O - 1, ld)
-        zero = torch.zeros(D, dtype=torch.float32, device=p.device)
-    else:
+    if not fft:
         groups = int(_lib.lib().hyena_b200_decode_extend_groups(B, D, t, n))
         part = torch.empty(B, D, n, groups, dtype=torch.float32, device=p.device)
     for o in range(O - 1):
         out = y if o == O - 2 else cache.h[o + 1]
         if fft:
-            # the cache keeps k reversed and h with row stride ld: the convolution wants both forward and compact (O(t)
-            # copies beside the O(t log t) transform); it recomputes all t + n outputs and keeps the last n
-            k = krev[:, o, ld - L:].flip(-1).contiguous()
-            conv = fftconv_forward(cache.h[o, :, :, :L].contiguous(), filter_spectrum(k), zero)
+            # recomputes all t + n outputs and keeps the last n
+            conv = _history_conv(cache, o, L, L)
             _extend_combine(conv[:, :, t:], L, 1, 1, s, out, o, B, n, cache)
         else:
             with torch.cuda.device(p.device):

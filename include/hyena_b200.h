@@ -265,6 +265,14 @@ HY_API int hyena_b200_decode_hist(const float* p, const float* in_bias, const fl
 HY_API int hyena_b200_decode_step(const float* p_t, const float* in_bias, const float* sw, const float* sb, const float* k,
                                   const float* fbias, float* h, float* tail, float* s_t, const float* v_in, float* out,
                                   float* part, int B, int cache_B, int D, int order, int o, int t, int Lcap, void* stream);
+/*   decode_win_step: decode_step at a position t inside an open window [b, b + Wc) (b a multiple of 4, b + Wc <= Lcap,
+ *                win (B, D, W) with W >= Wc: recurrence o's F[j] = sum_{s<b} k_o[b+j-s] g_o[s] for j < Wc, computed
+ *                beforehand).  Reads the history at [b, t) only: out_o[t] = F[t-b] + sum_{b<=s<t} k_o[t-s] g_o[s]
+ *                + (k_o[0] + bias_o) g_o[t].  Two launches (one at t = b); deterministic.  Same arguments otherwise. */
+HY_API int hyena_b200_decode_win_step(const float* p_t, const float* in_bias, const float* sw, const float* sb,
+                                      const float* k, const float* fbias, float* h, float* tail, float* s_t,
+                                      const float* v_in, float* out, float* part, const float* win, int B, int cache_B,
+                                      int D, int order, int o, int t, int b, int Wc, int W, int Lcap, void* stream);
 
 /* ---- extending a decode cache by n >= 1 positions [t, t+n), t + n <= Lcap (chunked prefill, continuation scoring) ----
  *   decode_extend_hist:    p (B, C, n) in_proj output of the n positions WITHOUT in_proj.bias -> s (B, C, n) short-filter
