@@ -893,4 +893,80 @@ HY_API int hyena_b200_decode_extend_combine(const float* part, long long row_str
   return 0;
 }
 
+/* decoding a branched cache (DecodeCache.fork): each of the R rows holds positions [b, b + Hc) of one branch with row stride
+   H; the filter is the parent cache's (row stride ld = ld_for(Lcap)) and is addressed from k + ld - H (decode_args.h) */
+static int check_branch(int R, int D, int order, int o, int t, int n, int b, int Hc, int H, int Lcap) {
+  if (check_decode_shape(R, R, D, order, Lcap)) return 1;
+  HY_CHECK(o >= 0 && o < order - 1, "recurrence %d outside [0, %d)", o, order - 1);
+  HY_CHECK(b >= 0 && (b & 3) == 0, "branch base %d must be a non-negative multiple of 4", b);
+  HY_CHECK(Hc >= 1 && b <= Lcap - Hc, "branch horizon [%d, %d) outside the decode cache [0, %d)", b, b + Hc, Lcap);
+  HY_CHECK((H & 3) == 0 && H >= Hc && H <= dec::ld_for(Lcap) - b,
+           "branch history width %d must be a multiple of 4 in [Hc, ld - b] = [%d, %d]", H, Hc, dec::ld_for(Lcap) - b);
+  HY_CHECK(n >= 1 && t >= b && t <= b + Hc - n, "positions [%d, %d) outside the branch horizon [%d, %d)", t, t + n, b,
+           b + Hc);
+  return 0;
+}
+
+HY_API int hyena_b200_decode_branch_step(const float* p_t, const float* in_bias, const float* sw, const float* sb,
+                                         const float* k, const float* fbias, float* h, float* tail, float* s_t,
+                                         const float* v_in, float* out, float* part, const float* f, const int* parent,
+                                         int R, int D, int order, int o, int t, int b, int Hc, int H, int Lcap,
+                                         void* stream) {
+  if (check_branch(R, D, order, o, t, 1, b, Hc, H, Lcap)) return 1;
+  HY_CHECK(k && fbias && h && s_t && out && part && f && parent, "null pointer");
+  HY_CHECK(o == 0 ? (p_t && sw && sb && tail && !v_in) : (v_in != nullptr),
+           o == 0 ? "null pointer: recurrence 0 needs p_t, sw, sb, tail (and no v_in)" : "null pointer: v_in");
+  HY_CHECK(aligned16(k) && aligned16(h), "k and h must be 16-byte aligned");
+  const int ld = dec::ld_for(Lcap), F = order - 1;
+  const float* kb = k + (size_t)o * ld + (ld - H);
+  dec::DotArgs dot{h, kb, part, R, D, t - b, H, F * ld, dec::chunks_for(H)};
+  dec::BranchStepArgs w{{part, (t - b + dec::kChunk - 1) / dec::kChunk, dec::chunks_for(H), kb, fbias + o, F * ld, F, H,
+                         p_t, in_bias, sw, sb, tail, s_t, v_in, h, out, R, D, (order + 1) * D, order, t - b,
+                         (order - 1 - o) * D, o == order - 2},
+                        f, parent};
+  HY_CUDA(launch_decode_branch_step(dot, w, (cudaStream_t)stream));
+  return 0;
+}
+
+HY_API int hyena_b200_decode_branch_extend_hist(const float* p, const float* in_bias, const float* sw, const float* sb,
+                                                float* h, float* tail, float* s, int R, int D, int order, int t, int n,
+                                                int b, int Hc, int H, int Lcap, void* stream) {
+  if (check_branch(R, D, order, 0, t, n, b, Hc, H, Lcap)) return 1;
+  HY_CHECK(p && sw && sb && h && tail && s, "null pointer");
+  dec::ExtHistArgs a{p, in_bias, sw, sb, tail, s, h, R, D, (order + 1) * D, t - b, n, H, (order - 1) * D};
+  HY_CUDA(launch_decode_ext_hist(a, (cudaStream_t)stream));
+  return 0;
+}
+
+HY_API int hyena_b200_decode_branch_extend_dot(const float* h, const float* k, float* part, int groups, int R, int D,
+                                               int order, int o, int t, int n, int b, int Hc, int H, int Lcap,
+                                               void* stream) {
+  if (check_branch(R, D, order, o, t, n, b, Hc, H, Lcap)) return 1;
+  HY_CHECK(h && k && part, "null pointer");
+  HY_CHECK(groups == dec::ext_groups(R, D, t - b, n), "partials sized for %d groups; this extend needs %d "
+           "(hyena_b200_decode_extend_groups with t - b)", groups, dec::ext_groups(R, D, t - b, n));
+  HY_CHECK(aligned16(k) && aligned16(h), "k and h must be 16-byte aligned");
+  const int ld = dec::ld_for(Lcap), F = order - 1, NT = dec::ext_tile(n), j = t - b;
+  dec::ExtDotArgs a{h, k + (size_t)o * ld + (ld - H), part, R, D, j, n, H, F * ld, (-j) & 3, (n + NT - 1) / NT,
+                    dec::ext_chunks_per_cta(R, D, j, n), dec::chunks_for(j + n), groups};
+  HY_CUDA(launch_decode_ext_dot(a, (cudaStream_t)stream));
+  return 0;
+}
+
+HY_API int hyena_b200_decode_branch_combine(const float* part, long long row_stride, int j_stride, int groups,
+                                            const float* fbias, const float* h, const float* s, float* out,
+                                            const float* f, const int* parent, int R, int D, int order, int o, int t,
+                                            int n, int b, int Hc, int H, int Lcap, void* stream) {
+  if (check_branch(R, D, order, o, t, n, b, Hc, H, Lcap)) return 1;
+  HY_CHECK(part && fbias && h && s && out && f && parent, "null pointer");
+  HY_CHECK(groups >= 1 && j_stride >= 0 && row_stride >= 0, "bad partial layout: groups %d, strides %lld / %d", groups,
+           row_stride, j_stride);
+  const int last = o == order - 2;
+  dec::BranchCombineArgs a{{part, row_stride, j_stride, groups, fbias + o, order - 1, h, s, last ? nullptr : out,
+                            last ? out : nullptr, R, D, (order + 1) * D, t - b, n, H, (order - 2 - o) * D, last},
+                           f, parent};
+  HY_CUDA(launch_decode_branch_combine(a, (cudaStream_t)stream));
+  return 0;
+}
+
 }  // extern "C"

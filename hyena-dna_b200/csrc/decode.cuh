@@ -12,6 +12,8 @@
 //                          position t from the tail (recurrence 0), the gates, g[t] into the history, the epilogue
 //   decode_win_step_kernel decode_step_kernel inside an open window [b, b + Wc): the partials cover only [b, t) (the dot
 //                          kernel run on h + b with t - b) and the precomputed F[t-b] = sum_{s<b} k[t-s] g[s] is added
+//   decode_branch_step_kernel the same for a branched cache (decode_args.h BranchStepArgs): each batch row is a branch with
+//                          its own history from b on, and F is read from the row of the branch's parent
 // fp32 throughout, no atomics: every sum has a fixed order, so a step is bitwise reproducible.
 #pragma once
 #include <cuda_runtime.h>
@@ -165,6 +167,18 @@ __global__ void __launch_bounds__(32 * kStepWarps) decode_win_step_kernel(const 
   if (row >= w.st.B * w.st.D) return;
   const int b = row / w.st.D, d = row - b * w.st.D;
   const float acc = reduce_partials(w.st, row, lane) + w.win[(size_t)row * w.wstride + w.j];
+  step_epilogue(w.st, row, b, d, lane, acc);
+}
+
+// a step of a branched cache: the partials of the branch's own positions [b, t), then F[parent[row b]][d][t-b] (the shared
+// context before b), then the same epilogue on the branch's history row (stride H); fixed order, bitwise reproducible
+__global__ void __launch_bounds__(32 * kStepWarps) decode_branch_step_kernel(const BranchStepArgs w) {
+  const int lane = threadIdx.x & 31;
+  const int row = blockIdx.x * kStepWarps + (threadIdx.x >> 5);      // b * D + d
+  if (row >= w.st.B * w.st.D) return;
+  const int b = row / w.st.D, d = row - b * w.st.D;
+  const float* f = w.f + ((size_t)__ldg(w.parent + b) * w.st.D + d) * w.st.ld;
+  const float acc = reduce_partials(w.st, row, lane) + f[w.st.t];
   step_epilogue(w.st, row, b, d, lane, acc);
 }
 

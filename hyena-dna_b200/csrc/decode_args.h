@@ -133,5 +133,22 @@ struct ExtCombineArgs {
   int last;
 };
 
+// ---- decoding a branched cache (DecodeCache.fork): branches of one context that share its history tail F
+// A branch row holds g_o of positions [b, b + Hc) only, with row stride H (b and H multiples of 4, Hc <= H).  The kernels run
+// on it with ld = H, t - b in place of t and the filter pointer moved by ld_parent - H: every tap index ld-1-t+s then lands on
+// the same absolute filter element as in the unbranched call.  F (P, D, H) of a recurrence holds, per parent row, the
+// contribution of the context before b to the positions [b, b + Hc); parent[row b] selects the F row of branch b.
+struct BranchStepArgs {
+  StepArgs st;           // st.ld = H, st.t = t - b, st.k shifted; st.part holds the partials over [b, t)
+  const float* f;        // (P, D, H) F of this recurrence
+  const int* parent;     // (B) F row of each branch
+};
+
+struct BranchCombineArgs {
+  ExtCombineArgs c;      // c.ld = H, c.t = t - b
+  const float* f;        // (P, D, H) F of this recurrence
+  const int* parent;     // (B) F row of each branch
+};
+
 }  // namespace dec
 }  // namespace hy

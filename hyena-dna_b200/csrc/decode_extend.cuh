@@ -10,6 +10,8 @@
 //                              memory, so both are read once per launch; each thread keeps an 8-output register block
 //   decode_ext_combine_kernel  fixed-order sum of the partials (or the FFT route's convolution), + bias g, the gates:
 //                              g_{o+1} into the next recurrence's history, or y_pre = out * x_0 after the last recurrence
+//   decode_branch_combine_kernel the combine of a branched cache: + the parent row's F[t-b+j] (decode_args.h); the hist and
+//                              dot kernels run unchanged on a branch's history row with shifted arguments
 // fp32, no atomics: every sum has a fixed order for a given (B, D, t, n), so an extend is bitwise reproducible.
 #pragma once
 #include <cuda_runtime.h>
@@ -178,20 +180,42 @@ __global__ void __launch_bounds__(32 * kExtWarps, 1) decode_ext_dot_kernel(const
   }
 }
 
+// fixed-order sum of the partials of output j of one (b, channel) row
+__device__ __forceinline__ float ext_partial_sum(const ExtCombineArgs& a, int row, int j) {
+  const float* pp = a.part + (size_t)row * a.prow + (size_t)j * a.pj;
+  float acc = 0.f;
+  for (int g = 0; g < a.groups; ++g) acc += pp[g];
+  return acc;
+}
+
+// everything of output j once acc = sum_{s<t+j} k[t+j-s] g[s] is known: + bias g, times the gate, into h_next or y
+__device__ __forceinline__ void ext_combine_epilogue(const ExtCombineArgs& a, int row, int b, int d, int j, float acc) {
+  const float gv = a.h[(size_t)row * a.ld + a.t + j];
+  const float y = fmaf(__ldg(a.fbias + (size_t)d * a.fstride), gv, acc);
+  const float x = a.s[((size_t)b * a.C + a.xch + d) * a.n + j];
+  if (a.last) a.y[(size_t)row * a.n + j] = y * x;
+  else a.h_next[(size_t)row * a.ld + a.t + j] = y * x;
+}
+
 // one thread per (b, d, j)
 __global__ void __launch_bounds__(256) decode_ext_combine_kernel(const ExtCombineArgs a) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (long long)a.B * a.D * a.n) return;
   const int row = (int)(idx / a.n), j = (int)(idx - (long long)row * a.n);
   const int b = row / a.D, d = row - b * a.D;
-  const float* pp = a.part + (size_t)row * a.prow + (size_t)j * a.pj;
-  float acc = 0.f;
-  for (int g = 0; g < a.groups; ++g) acc += pp[g];
-  const float gv = a.h[(size_t)row * a.ld + a.t + j];
-  const float y = fmaf(__ldg(a.fbias + (size_t)d * a.fstride), gv, acc);
-  const float x = a.s[((size_t)b * a.C + a.xch + d) * a.n + j];
-  if (a.last) a.y[(size_t)row * a.n + j] = y * x;
-  else a.h_next[(size_t)row * a.ld + a.t + j] = y * x;
+  ext_combine_epilogue(a, row, b, d, j, ext_partial_sum(a, row, j));
+}
+
+// the combine of a branched cache (decode_args.h BranchCombineArgs): the partials over the branch's positions [b, t+j), then
+// F[parent[row b]][d][t-b+j] (the shared context before b), then the same epilogue; one thread per (b, d, j)
+__global__ void __launch_bounds__(256) decode_branch_combine_kernel(const BranchCombineArgs w) {
+  const ExtCombineArgs& a = w.c;
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)a.B * a.D * a.n) return;
+  const int row = (int)(idx / a.n), j = (int)(idx - (long long)row * a.n);
+  const int b = row / a.D, d = row - b * a.D;
+  const float* f = w.f + ((size_t)__ldg(w.parent + b) * a.D + d) * a.ld;
+  ext_combine_epilogue(a, row, b, d, j, ext_partial_sum(a, row, j) + f[a.t + j]);
 }
 
 }  // namespace dec

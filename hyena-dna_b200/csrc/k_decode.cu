@@ -64,4 +64,18 @@ cudaError_t launch_decode_win_step(const dec::DotArgs& dot, const dec::WinStepAr
   return cudaGetLastError();
 }
 
+// one recurrence of a branch step: the dot product over the branch's positions [b, t) (skipped at t = b), then the branch
+// combine kernel; counted as a windowed step (a window whose F is selected per row)
+cudaError_t launch_decode_branch_step(const dec::DotArgs& dot, const dec::BranchStepArgs& w, cudaStream_t s) {
+  if (w.st.nchunk > 0) {
+    cudaError_t e = launch_dot(dot, w.st.nchunk, K_DECODE_WIN_STEP, s);
+    if (e != cudaSuccess) return e;
+  }
+  const int rows = w.st.B * w.st.D;
+  prof_begin(K_DECODE_WIN_STEP, s);
+  dec::decode_branch_step_kernel<<<(rows + dec::kStepWarps - 1) / dec::kStepWarps, 32 * dec::kStepWarps, 0, s>>>(w);
+  prof_end(K_DECODE_WIN_STEP, s);
+  return cudaGetLastError();
+}
+
 }  // namespace hy

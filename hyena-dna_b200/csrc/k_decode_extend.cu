@@ -45,4 +45,12 @@ cudaError_t launch_decode_ext_combine(const dec::ExtCombineArgs& a, cudaStream_t
   return cudaGetLastError();
 }
 
+cudaError_t launch_decode_branch_combine(const dec::BranchCombineArgs& a, cudaStream_t s) {
+  const long long n = (long long)a.c.B * a.c.D * a.c.n;
+  prof_begin(K_DECODE_EXT_COMBINE, s);
+  dec::decode_branch_combine_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a);
+  prof_end(K_DECODE_EXT_COMBINE, s);
+  return cudaGetLastError();
+}
+
 }  // namespace hy

@@ -62,10 +62,12 @@ cudaError_t launch_add_ln_bwd(ln::BwdArgs a, float* dw, float* db, cudaStream_t 
 cudaError_t launch_decode_hist(const dec::HistArgs& a, cudaStream_t s);
 cudaError_t launch_decode_step(const dec::DotArgs& dot, const dec::StepArgs& st, cudaStream_t s);
 cudaError_t launch_decode_win_step(const dec::DotArgs& dot, const dec::WinStepArgs& w, cudaStream_t s);
+cudaError_t launch_decode_branch_step(const dec::DotArgs& dot, const dec::BranchStepArgs& w, cudaStream_t s);
 // k_decode_extend.cu: extending a decode cache by n positions (decode_extend.cuh)
 cudaError_t launch_decode_ext_hist(const dec::ExtHistArgs& a, cudaStream_t s);
 cudaError_t launch_decode_ext_dot(const dec::ExtDotArgs& a, cudaStream_t s);
 cudaError_t launch_decode_ext_combine(const dec::ExtCombineArgs& a, cudaStream_t s);
+cudaError_t launch_decode_branch_combine(const dec::BranchCombineArgs& a, cudaStream_t s);
 // k_convert.cu: reference filter-spectrum convention (rfft(k, fft_size), natural order) <-> packed spectrum
 cudaError_t launch_rfft_to_packed(const float2* X, float2* Z, int H, int logM, int logM1, cudaStream_t s);
 cudaError_t launch_packed_to_rfft(const float2* Z, float2* X, int H, int logM, int logM1, float scale, cudaStream_t s);

@@ -27,6 +27,26 @@ def _chunks(lcap):
     return (lcap + CHUNK - 1) // CHUNK
 
 
+def _host_index(index, n, what):
+    """index (a sequence or 1-D tensor of integers) -> list of ints in [0, n), checked on the host before any device work."""
+    if torch.is_tensor(index):
+        if index.dim() != 1 or index.dtype.is_floating_point or index.dtype.is_complex or index.dtype == torch.bool:
+            raise HyenaB200Error(f"{what} must be a 1-D integer index; got {index.dtype} of shape {tuple(index.shape)}")
+        index = index.tolist()
+    try:
+        out = [int(i) for i in index]
+        if any(isinstance(i, bool) or int(i) != i for i in index):
+            raise ValueError
+    except (TypeError, ValueError):
+        raise HyenaB200Error(f"{what} must be a 1-D sequence of integers") from None
+    if not out:
+        raise HyenaB200Error(f"{what} is empty")
+    bad = [i for i in out if not 0 <= i < n]
+    if bad:
+        raise HyenaB200Error(f"{what} {bad[0]} outside [0, {n})")
+    return out
+
+
 class DecodeCache:
     """Decoding state of one HyenaOperator (``HyenaOperator.allocate_decode_cache``), or of every mixer of a stack
     (``Backbone.allocate_decode_cache``: ``layers`` holds one per layer, looked up by module identity).
@@ -45,7 +65,18 @@ class DecodeCache:
     Window state of the windowed step (ops.decode_window_plan, DESIGN.md section 4.11): a window [win_b, win_b + win_wc)
     is valid while win_b <= t < win_b + win_wc; ``win_f`` (O-1, B, D, W) holds F_o[j] = sum_{s < win_b} k_o[win_b+j-s]
     g_o[s] for j < win_wc.  F depends on h[:, :, :, :win_b] only, so an extend inside the window leaves it valid.  It is
-    allocated at the first refresh (``window_nbytes``).  ``steps`` counts the steps since the last prefill or extend."""
+    allocated at the first refresh (``window_nbytes``).  ``steps`` counts the steps since the last prefill or extend.
+
+    A *branched* cache (``fork``, ``select``; DESIGN.md section 4.12) holds R branches that continue rows of a parent cache
+    from its position t0.  With base b = t0 - t0 mod 4, Hc = min(horizon rounded up to a multiple of 4, Lcap - b) and
+    H = Hc rounded up to a multiple of 4, per operator:
+      k, bias                the parent's (shared: never written after allocation)
+      h     (O-1, R, D, H)   g_o of each branch at positions [b, b + Hc)
+      f     (O-1, P, D, H)   F_o[p][j] = sum_{s<b} k_o[b+j-s] g_o[s] of the P distinct forked parent rows, j < Hc
+      parent (R,) int32      the row of f each branch reads
+      tail, s_t, part        as above with R rows and ceil(H / 1024) partials
+    so out_o[t] = F_o[parent][t-b] + sum_{b<=s<t} k_o[t-s] g_o[s] + (k_o[0] + bias_o) g_o[t] for b <= t < b + Hc, and no
+    operation on a branch reads the context before b."""
 
     def __init__(self, owner=None, batch_size=0, max_seqlen=0, lcap=0, k=None, bias=None, h=None, tail=None, s_t=None,
                  part=None, layers=None):
@@ -55,6 +86,7 @@ class DecodeCache:
         self.layers = list(layers) if layers is not None else []
         self._t = 0
         self.win_b, self.win_wc, self.win_f, self.steps = 0, 0, None, 0
+        self._branched, self.base, self.hc, self.f, self.parent = False, 0, 0, None, None
         if owner is not None:
             self.d_model, self.order = owner.d_model, owner.order
 
@@ -102,9 +134,49 @@ class DecodeCache:
 
     @property
     def nbytes(self):
+        """Bytes the cache owns: the layout above, or for a branched cache its branch state (h, f, tail, s_t, part, parent;
+        the filter is the parent's)."""
         if self.layers:
             return sum(c.nbytes for c in self.layers)
-        return sum(x.numel() * x.element_size() for x in (self.k, self.bias, self.h, self.tail, self.s_t, self.part))
+        own = (self.h, self.f, self.tail, self.s_t, self.part, self.parent) if self.branched else \
+              (self.k, self.bias, self.h, self.tail, self.s_t, self.part)
+        return sum(x.numel() * x.element_size() for x in own)
+
+    @property
+    def branched(self):
+        return self.layers[0].branched if self.layers else self._branched
+
+    def fork(self, rows, horizon=4096):
+        """A branched cache of len(rows) rows: row i continues row ``rows[i]`` of this cache from its current position t0
+        (repeat a row for several branches of one context) and can be stepped and extended up to horizon positions past
+        its base t0 - t0 mod 4, or to Lcap.  A snapshot: this cache can go on decoding without changing the branches.  A
+        stack's cache forks every layer."""
+        if self.branched:
+            raise HyenaB200Error("fork: this cache is branched already; use select() to reorder, repeat or drop branches")
+        rows = _host_index(rows, self.batch_size, "fork: rows")
+        horizon = int(horizon)
+        if horizon < 1:
+            raise HyenaB200Error(f"fork: horizon {horizon} must be >= 1")
+        for c in (self.layers or [self]):
+            if c.owner.filter_fn.bidirectional:
+                raise HyenaB200Error("decoding needs a causal filter; this HyenaFilter is bidirectional")
+            if c.t < 1 or c.t >= c.lcap:
+                raise HyenaB200Error(f"fork: the cache is at position {c.t}; forking needs 1 <= t0 < Lcap = {c.lcap}")
+        from . import ops
+        if self.layers:
+            return DecodeCache.stack(ops.decode_fork(c, rows, horizon) for c in self.layers)
+        return ops.decode_fork(self, rows, horizon)
+
+    def select(self, index):
+        """A branched cache of the branches ``index`` of this one (repeats allowed): each row copies that branch's history,
+        tail and parent row; F is shared.  Reorders, prunes or re-forks beams in one call."""
+        if not self.branched:
+            raise HyenaB200Error("select: this cache is not branched (fork() first)")
+        index = _host_index(index, self.batch_size, "select: index")
+        from . import ops
+        if self.layers:
+            return DecodeCache.stack(ops.decode_select(c, index) for c in self.layers)
+        return ops.decode_select(self, index)
 
     @property
     def window_nbytes(self):

@@ -428,8 +428,13 @@ class HyenaOperator(nn.Module):
             raise HyenaB200Error(f"decoding input must be (B, {n}, {self.d_model}); got {tuple(u.shape)}")
         if u.shape[0] != c.batch_size:
             raise HyenaB200Error(f"batch size {u.shape[0]} differs from the decode cache's {c.batch_size}")
+        if fresh and c.branched:
+            raise HyenaB200Error("prefill needs a fresh cache; this one is branched (DecodeCache.fork)")
         if fresh and c.t != 0:
             raise HyenaB200Error(f"prefill needs a fresh cache; this one is at position {c.t}")
+        if c.branched and c.t + n > c.base + c.hc:
+            raise HyenaB200Error(f"decoding past the branch horizon: positions [{c.t}, {c.t + n}) exceed base + Hc = "
+                                 f"{c.base} + {c.hc} = {c.base + c.hc} (fork with a larger horizon, up to Lcap = {c.lcap})")
         if c.t + n > c.lcap:
             raise HyenaB200Error(f"decoding past the cache: positions [{c.t}, {c.t + n}) exceed Lcap = min(max_seqlen, "
                                  f"l_max) = {c.lcap} (l_max = {self.l_max}: the filter has no taps beyond it)")
@@ -479,7 +484,8 @@ class HyenaOperator(nn.Module):
         fresh cache starts the sequence (empty history).  The in_proj / out_proj products of one position are fp32
         matrix-vector products (F.linear); the operator itself runs in csrc/decode.cuh, two launches per recurrence.  After
         a run of steps at a long history the step reads only the positions of a window opened by one FFT refresh
-        (ops.decode_window_plan chooses)."""
+        (ops.decode_window_plan chooses).  On a branched cache (DecodeCache.fork) the step reads each branch's positions since
+        the fork base only (ops.decode_branch_step)."""
         c = self._decode_checks(u_t, cache, 1)
         with torch.no_grad():
             in_dtype = u_t.dtype
@@ -487,7 +493,7 @@ class HyenaOperator(nn.Module):
             u = u_t.to(torch.float32).reshape(B, D)
             p_t = torch.nn.functional.linear(u, self.in_proj.weight).contiguous()          # bias added in the kernel
             ib, sw, sb = self._decode_params()
-            y_pre = ops.decode_step_auto(p_t, ib, sw, sb, c)
+            y_pre = (ops.decode_branch_step if c.branched else ops.decode_step_auto)(p_t, ib, sw, sb, c)
             y = torch.nn.functional.linear(y_pre, self.out_proj.weight, self.out_proj.bias)
             c.t += 1
         return y.reshape(B, 1, D).to(in_dtype)
@@ -497,11 +503,14 @@ class HyenaOperator(nn.Module):
         advances the cache by n.  On a fresh cache this is ``prefill`` (bit-identical to ``forward``).  Otherwise in_proj and
         out_proj of the chunk run on the wgmma projection GEMM and every recurrence on csrc/decode_extend.cuh: the direct
         Toeplitz kernel over the cached history, or for large n the FFT convolution of the whole history
-        (ops.decode_extend_uses_fft chooses from t and n)."""
+        (ops.decode_extend_uses_fft chooses from t and n).  On a branched cache the same routes run over each branch's
+        positions since the fork base only (ops.decode_branch_extend)."""
         n = u.shape[1] if u.dim() == 3 else -1
         if n < 1:
             raise HyenaB200Error(f"extend input must be (B, n, {self.d_model}) with n >= 1; got {tuple(u.shape)}")
         c = self._decode_checks(u, cache, n)
+        if c.branched:
+            return self._extend(u, c, ops.decode_branch_extend)
         if c.t == 0:
             return self.prefill(u, c)
         return self._extend(u, c, ops.decode_extend)

@@ -766,18 +766,18 @@ def decode_window_bounds(t, lcap):
     return b, min(WINDOW, int(lcap) - b)
 
 
-def _history_conv(cache, o, hist, L):
-    """Causal convolution of g_o[0, hist) (zero from hist on) with the first L filter taps of recurrence o -> (B, D, L), on the
-    library's filter_spectrum + fftconv_forward with a zero skip term.  The cache keeps k reversed and h with row stride ld,
-    so the filter rows are un-reversed and the history compacted or zero-padded first (O(L) copies beside the transforms);
-    h is not read at positions >= hist."""
-    D, O, ld = cache.d_model, cache.order, cache.h.shape[-1]
+def _history_conv(cache, ld, h, o, hist, L):
+    """Causal convolution of h[:, :, 0:hist) (zero from hist on) with the first L filter taps of recurrence o -> (B, D, L), on
+    the library's filter_spectrum + fftconv_forward with a zero skip term.  h (B, D, >= hist) is g_o by position; ld is the
+    row stride of the cache's filter, which is kept reversed, so the filter rows are un-reversed and the history compacted or
+    zero-padded first (O(L) copies beside the transforms); h is not read at positions >= hist."""
+    D, O = cache.d_model, cache.order
     k = cache.k[:(O - 1) * D * ld].view(D, O - 1, ld)[:, o, ld - L:].flip(-1).contiguous()
     if hist == L:
-        u = cache.h[o, :, :, :L].contiguous()
+        u = h[:, :, :L].contiguous()
     else:
-        u = torch.zeros(cache.h.shape[1], D, L, dtype=torch.float32, device=cache.h.device)
-        u[:, :, :hist] = cache.h[o, :, :, :hist]
+        u = torch.zeros(h.shape[0], D, L, dtype=torch.float32, device=h.device)
+        u[:, :, :hist] = h[:, :, :hist]
     zero = torch.zeros(D, dtype=torch.float32, device=u.device)
     return fftconv_forward(u, filter_spectrum(k), zero)
 
@@ -794,7 +794,7 @@ def decode_window_refresh(cache):
         cache.win_f = None
         cache.win_f = torch.empty(O - 1, B, D, max(WINDOW, wc), dtype=torch.float32, device=cache.h.device)
     for o in range(O - 1):
-        cache.win_f[o, :, :, :wc] = _history_conv(cache, o, b, b + wc)[:, :, b:]
+        cache.win_f[o, :, :, :wc] = _history_conv(cache, cache.h.shape[-1], cache.h[o], o, b, b + wc)[:, :, b:]
     cache.win_b, cache.win_wc = b, wc
 
 
@@ -887,7 +887,7 @@ def _decode_extend(p, in_bias, sw, sb, cache, fft):
         out = y if o == O - 2 else cache.h[o + 1]
         if fft:
             # recomputes all t + n outputs and keeps the last n
-            conv = _history_conv(cache, o, L, L)
+            conv = _history_conv(cache, ld, cache.h[o], o, L, L)
             _extend_combine(conv[:, :, t:], L, 1, 1, s, out, o, B, n, cache)
         else:
             with torch.cuda.device(p.device):
@@ -916,3 +916,122 @@ def decode_extend(p, in_bias, sw, sb, cache):
     n = p.shape[-1]
     fn = decode_extend_fft if decode_extend_uses_fft(cache.t, n) else decode_extend_direct
     return fn(p, in_bias, sw, sb, cache)
+
+
+# ------------------------------------------------------------------------------------------ branched caches (fork)
+# Branches of one context share its history tail: with base b <= t0 (a multiple of 4), out_o[t] = F_o[t-b] + the sum over
+# the branch's own positions [b, t) + (k_o[0] + bias_o) g_o[t], where F_o[j] = sum_{s<b} k_o[b+j-s] g_o[s] depends on the
+# parent row's context only -- the windowed step's identity (section 4.11) with the horizon as the window and a history row per
+# branch.  F is computed once per distinct parent row at the fork; no later operation reads the context.  DESIGN.md 4.12.
+def decode_branch_bounds(t0, lcap, horizon):
+    """(b, Hc, H) of a fork at position t0: b = t0 rounded down to a multiple of 4, Hc = min(horizon rounded up to a multiple
+    of 4, lcap - b) positions a branch can hold, H = Hc rounded up to a multiple of 4 (the row stride of its history)."""
+    b = int(t0) - int(t0) % 4
+    hc = min((int(horizon) + 3) // 4 * 4, int(lcap) - b)
+    return b, hc, (hc + 3) // 4 * 4
+
+
+def _branch_cache(cache, h, tail, f, parent, base, hc):
+    """A branched DecodeCache of h.shape[1] rows at cache.t sharing cache's filter; fresh step scratch."""
+    R, D, C = h.shape[1], cache.d_model, (cache.order + 1) * cache.d_model
+    dev = h.device
+    s_t = torch.zeros(R, C, dtype=torch.float32, device=dev)
+    part = torch.zeros(R, D, (h.shape[-1] + 1023) // 1024, dtype=torch.float32, device=dev)
+    new = type(cache)(cache.owner, R, cache.max_seqlen, cache.lcap, cache.k, cache.bias, h, tail, s_t, part)
+    new.t = cache.t
+    new._branched, new.base, new.hc, new.f, new.parent = True, base, hc, f, parent
+    return new
+
+
+def decode_fork(cache, rows, horizon):
+    """Branches of the unbranched operator cache ``cache`` (host-validated ``rows``, see DecodeCache.fork): F of every
+    distinct parent row by one FFT convolution of its history [0, b) per recurrence (_history_conv, as decode_window_refresh
+    computes it; none when b = 0), the positions [b, t0) and the tails copied, the device parent index built."""
+    t0, O, D = cache.t, cache.order, cache.d_model
+    b, hc, H = decode_branch_bounds(t0, cache.lcap, horizon)
+    dev = cache.h.device
+    uniq = sorted(set(rows))
+    slot = {r: i for i, r in enumerate(uniq)}
+    f = torch.zeros(O - 1, len(uniq), D, H, dtype=torch.float32, device=dev)
+    if b > 0:
+        ld = cache.h.shape[-1]
+        for o in range(O - 1):
+            hist = cache.h[o] if uniq == list(range(cache.batch_size)) else cache.h[o, uniq, :, :b]
+            f[o, :, :, :hc] = _history_conv(cache, ld, hist, o, b, b + hc)[:, :, b:]
+    ridx = torch.tensor(rows, dtype=torch.long, device=dev)
+    h = torch.zeros(O - 1, len(rows), D, H, dtype=torch.float32, device=dev)
+    if t0 > b:
+        h[:, :, :, :t0 - b] = cache.h[:, ridx, :, b:t0]
+    parent = torch.tensor([slot[r] for r in rows], dtype=torch.int32, device=dev)
+    return _branch_cache(cache, h, cache.tail.index_select(0, ridx), f, parent, b, hc)
+
+
+def decode_select(cache, index):
+    """The branches ``index`` (host-validated, see DecodeCache.select) of the branched operator cache ``cache``: history,
+    tail and parent row copied per row, F shared."""
+    idx = torch.tensor(index, dtype=torch.long, device=cache.h.device)
+    return _branch_cache(cache, cache.h.index_select(1, idx), cache.tail.index_select(0, idx), cache.f,
+                         cache.parent.index_select(0, idx), cache.base, cache.hc)
+
+
+def _branch_args(cache, B, what):
+    if B != cache.batch_size:
+        raise _lib.HyenaB200Error(f"{what}: batch size {B} differs from the branched cache's {cache.batch_size}")
+    return int(cache.t), cache.base, cache.hc, cache.h.shape[-1]
+
+
+def decode_branch_step(p_t, in_bias, sw, sb, cache):
+    """decode_step on a branched cache: per recurrence the dot product over each branch's positions [b, t) and
+    decode_branch_step_kernel, which adds the parent row's F[t-b] (csrc/decode.cuh); does not advance cache.t."""
+    _need_cuda(p_t, in_bias, sw, sb)
+    B = p_t.shape[0]
+    D, O = cache.d_model, cache.order
+    if not p_t.is_contiguous() or tuple(p_t.shape) != (B, (O + 1) * D):
+        raise _lib.HyenaB200Error(f"decode_branch_step: p_t must be contiguous (B, {(O + 1) * D})")
+    t, b, hc, H = _branch_args(cache, B, "decode_branch_step")
+    out = [torch.empty(B, D, dtype=torch.float32, device=p_t.device) for _ in range(O - 1)]
+    with torch.cuda.device(p_t.device):
+        for o in range(O - 1):
+            first = o == 0
+            _lib.check(_lib.lib().hyena_b200_decode_branch_step(
+                _ptr(p_t) if first else 0, _ptr(in_bias) if first else 0, _ptr(sw) if first else 0,
+                _ptr(sb) if first else 0, _ptr(cache.k), _ptr(cache.bias), _ptr(cache.h[o]), _ptr(cache.tail) if first else 0,
+                _ptr(cache.s_t), 0 if first else _ptr(out[o - 1]), _ptr(out[o]), _ptr(cache.part), _ptr(cache.f[o]),
+                _ptr(cache.parent), B, D, O, o, t, b, hc, H, cache.lcap, _stream()))
+    return out[-1]
+
+
+def decode_branch_extend(p, in_bias, sw, sb, cache, fft=None):
+    """decode_extend on a branched cache: y_pre (B, D, n) of the positions [t, t + n), t = cache.t, per recurrence over each
+    branch's positions [b, t + n) only -- decode_ext_dot_kernel on the branch rows (or, with ``fft``, the FFT convolution of
+    them), then decode_branch_combine_kernel, which adds the parent row's F.  ``fft`` None: decode_extend_uses_fft(t - b, n)
+    chooses.  Writes the n positions into the branch rows and tails; does not advance cache.t."""
+    _need_cuda(in_bias, sw, sb)
+    B, n = _extend_check(p, cache, "decode_branch_extend")
+    t, b, hc, H = _branch_args(cache, B, "decode_branch_extend")
+    D, O, lcap, j = cache.d_model, cache.order, cache.lcap, t - b
+    if fft is None:
+        fft = decode_extend_uses_fft(j, n)
+    lib = _lib.lib()
+    s = torch.empty_like(p)
+    y = torch.empty(B, D, n, dtype=torch.float32, device=p.device)
+    with torch.cuda.device(p.device):
+        _lib.check(lib.hyena_b200_decode_branch_extend_hist(
+            _ptr(p), _ptr(in_bias), _ptr(sw), _ptr(sb), _ptr(cache.h), _ptr(cache.tail), _ptr(s), B, D, O, t, n, b, hc, H,
+            lcap, _stream()))
+        if not fft:
+            groups = int(lib.hyena_b200_decode_extend_groups(B, D, j, n))
+            part = torch.empty(B, D, n, groups, dtype=torch.float32, device=p.device)
+        for o in range(O - 1):
+            out = y if o == O - 2 else cache.h[o + 1]
+            if fft:
+                conv = _history_conv(cache, (lcap + 3) // 4 * 4, cache.h[o], o, j + n, j + n)
+                src, row_stride, j_stride, g = conv[:, :, j:], j + n, 1, 1
+            else:
+                _lib.check(lib.hyena_b200_decode_branch_extend_dot(
+                    _ptr(cache.h[o]), _ptr(cache.k), _ptr(part), groups, B, D, O, o, t, n, b, hc, H, lcap, _stream()))
+                src, row_stride, j_stride, g = part, n * groups, groups, groups
+            _lib.check(lib.hyena_b200_decode_branch_combine(
+                _ptr(src), int(row_stride), int(j_stride), int(g), _ptr(cache.bias), _ptr(cache.h[o]), _ptr(s), _ptr(out),
+                _ptr(cache.f[o]), _ptr(cache.parent), B, D, O, o, t, n, b, hc, H, lcap, _stream()))
+    return y

@@ -294,6 +294,36 @@ HY_API int hyena_b200_decode_extend_combine(const float* part, long long row_str
                                             const float* fbias, const float* h, const float* s, float* out, int B,
                                             int cache_B, int D, int order, int o, int t, int n, int Lcap, void* stream);
 
+/* ---- decoding a branched cache (R branches forked from one context at base b, a multiple of 4) ----
+ * Each of the R rows of h (recurrence o's rows, 16-byte aligned) holds g_o of positions [b, b + Hc) of one branch with row
+ * stride H (a multiple of 4, Hc <= H <= ld - b, b + Hc <= Lcap); tail, s_t, s, part and out have R rows.  k and fbias are the
+ * parent cache's (ld = Lcap rounded up to a multiple of 4).  f (P, D, H) holds recurrence o's F[p][d][j] =
+ * sum_{s<b} k_o[b+j-s] g_o[s] of parent row p for j < Hc; parent (R) int32 on the device gives the F row of each branch
+ * (not checked here: every entry must be in [0, P)).  Positions t are absolute; t and t + n must stay in [b, b + Hc).
+ *   decode_branch_step:        decode_step of position t on the branches: out_o[t] = F[parent][t-b]
+ *                              + sum_{b<=s<t} k_o[t-s] g_o[s] + (k_o[0] + bias_o) g_o[t].  Two launches (one at t = b).
+ *   decode_branch_extend_hist: decode_extend_hist of the n positions [t, t+n) on the branch rows.
+ *   decode_branch_extend_dot:  decode_extend_dot over the branch positions [b, t+n): part (R, D, n, groups) with groups =
+ *                              decode_extend_groups(R, D, t - b, n).
+ *   decode_branch_combine:     decode_extend_combine + F[parent][t-b+j]; part may also be the FFT route's convolution of the
+ *                              branch rows (positions from b on).
+ * Deterministic: fixed summation orders, no atomics. */
+HY_API int hyena_b200_decode_branch_step(const float* p_t, const float* in_bias, const float* sw, const float* sb,
+                                         const float* k, const float* fbias, float* h, float* tail, float* s_t,
+                                         const float* v_in, float* out, float* part, const float* f, const int* parent,
+                                         int R, int D, int order, int o, int t, int b, int Hc, int H, int Lcap,
+                                         void* stream);
+HY_API int hyena_b200_decode_branch_extend_hist(const float* p, const float* in_bias, const float* sw, const float* sb,
+                                                float* h, float* tail, float* s, int R, int D, int order, int t, int n,
+                                                int b, int Hc, int H, int Lcap, void* stream);
+HY_API int hyena_b200_decode_branch_extend_dot(const float* h, const float* k, float* part, int groups, int R, int D,
+                                               int order, int o, int t, int n, int b, int Hc, int H, int Lcap,
+                                               void* stream);
+HY_API int hyena_b200_decode_branch_combine(const float* part, long long row_stride, int j_stride, int groups,
+                                            const float* fbias, const float* h, const float* s, float* out,
+                                            const float* f, const int* parent, int R, int D, int order, int o, int t,
+                                            int n, int b, int Hc, int H, int Lcap, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
