@@ -9,11 +9,11 @@ from .hyena import (ExponentialModulation, HyenaFilter, HyenaOperator, OptimModu
 from .fftconv import FFTConvFunc, fftconv_bwd, fftconv_func, fftconv_fwd, fftconv_ref  # noqa: F401
 from . import block, decode, distributed, mlp, ops, registry, stack  # noqa: F401
 from .block import Backbone, Block  # noqa: F401
-from .decode import DecodeCache  # noqa: F401
+from .decode import DecodeCache, StepGraph  # noqa: F401
 from .mlp import Mlp  # noqa: F401
 from .stack import CheckpointedHyenaStack, enable_filter_cache, memory_plan  # noqa: F401
 from .host import HostStep  # noqa: F401
 
 __all__ = ["HyenaOperator", "HyenaFilter", "PositionalEmbedding", "ExponentialModulation", "Sin", "OptimModule",
            "fftconv_func", "fftconv_ref", "FFTConvFunc", "fftconv_fwd", "fftconv_bwd", "registry", "distributed", "ops",
-           "HostStep", "Block", "Backbone", "block", "Mlp", "mlp", "DecodeCache", "decode", "CheckpointedHyenaStack", "enable_filter_cache", "memory_plan", "stack", "build", "launch_count", "HyenaB200Error", "LIB_PATH"]
+           "HostStep", "Block", "Backbone", "block", "Mlp", "mlp", "DecodeCache", "StepGraph", "decode", "CheckpointedHyenaStack", "enable_filter_cache", "memory_plan", "stack", "build", "launch_count", "HyenaB200Error", "LIB_PATH"]

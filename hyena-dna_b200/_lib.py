@@ -71,6 +71,10 @@ SIGNATURES = {
     "hyena_b200_decode_branch_extend_hist": (_i, [c_fp] * 7 + [_i] * 9 + [_vp]),
     "hyena_b200_decode_branch_extend_dot": (_i, [c_fp] * 3 + [_i] * 11 + [_vp]),
     "hyena_b200_decode_branch_combine": (_i, [c_fp, ctypes.c_longlong, _i, _i] + [c_fp] * 6 + [_i] * 10 + [_vp]),
+    "hyena_b200_decode_step_dev": (_i, [c_fp] * 13 + [_i] * 7 + [_vp]),
+    "hyena_b200_decode_win_step_dev": (_i, [c_fp] * 14 + [_i] * 7 + [_vp]),
+    "hyena_b200_decode_branch_step_dev": (_i, [c_fp] * 15 + [_i] * 6 + [_vp]),
+    "hyena_b200_decode_pos_advance": (_i, [c_fp, _vp]),
 }
 
 

@@ -15,7 +15,7 @@ import torch.nn as nn
 
 from . import ops
 from ._lib import HyenaB200Error
-from .decode import DecodeCache
+from .decode import DecodeCache, StepGraph
 
 
 class Block(nn.Module):
@@ -75,6 +75,11 @@ class Block(nn.Module):
         """forward of n more positions (B, n, D) from the mixer's DecodeCache (HyenaOperator.extend)."""
         return self._decode(hidden_states, residual, lambda y: self.mixer.extend(y, cache))
 
+    def capture_step(self, cache, batch_size=None, dtype=torch.float32, residual=False):
+        """A decode.StepGraph of ``step`` on the mixer's cache; ``residual`` says whether steps pass a residual (False for
+        a first block)."""
+        return StepGraph(self, cache, batch_size, dtype, residual=residual)
+
     def _decode(self, hidden_states, residual, mix):
         if not hasattr(self.mixer, "step"):
             raise HyenaB200Error(f"Block: the mixer {type(self.mixer).__name__} has no incremental decoding")
@@ -131,6 +136,10 @@ class Backbone(nn.Module):
     def extend(self, hidden_states, cache):
         """The outputs of n more positions (B, n, D); on a fresh cache this is prefill."""
         return self._decode(hidden_states, cache, "extend")
+
+    def capture_step(self, cache, batch_size=None, dtype=torch.float32):
+        """A decode.StepGraph of ``step`` on ``cache``: every layer and ln_f in one CUDA graph per route."""
+        return StepGraph(self, cache, batch_size, dtype)
 
     def _decode(self, hidden_states, cache, how):
         if hidden_states.requires_grad:

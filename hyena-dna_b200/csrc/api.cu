@@ -33,9 +33,15 @@ static cudaEvent_t get_event() {
   cudaEventCreate(&e);
   return e;
 }
+// a stream being captured into a CUDA graph gets no timing events: they would become graph nodes, and the pooled events
+// would be recycled while the graph still records them
+static bool capturing(cudaStream_t s) {
+  cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+  return cudaStreamIsCapturing(s, &st) != cudaSuccess || st != cudaStreamCaptureStatusNone;
+}
 void prof_begin(int kind, cudaStream_t s) {
   (void)kind;
-  if (!g_prof_on || g_prof_suppress) return;
+  if (!g_prof_on || g_prof_suppress || capturing(s)) return;
   std::lock_guard<std::mutex> lk(g_prof_mu);
   g_cur_e0 = get_event();
   cudaEventRecord(g_cur_e0, s);
@@ -49,6 +55,8 @@ void prof_end(int kind, cudaStream_t s) {
   g_prof.push_back({kind, g_cur_e0, e1});
   g_cur_e0 = nullptr;
 }
+
+void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 
 int api_fail(const char* fmt, ...) {
   va_list ap;
@@ -966,6 +974,74 @@ HY_API int hyena_b200_decode_branch_combine(const float* part, long long row_str
                             last ? out : nullptr, R, D, (order + 1) * D, t - b, n, H, (order - 2 - o) * D, last},
                            f, parent};
   HY_CUDA(launch_decode_branch_combine(a, (cudaStream_t)stream));
+  return 0;
+}
+
+/* device-position steps (a step captured once in a CUDA graph): the kernels read pos = [t, win_b, base] */
+static int check_dev_step(int o, int order, const float* p_t, const float* sw, const float* sb, const float* tail,
+                          const float* v_in, const float* k, const float* h, const int* pos) {
+  HY_CHECK(o >= 0 && o < order - 1, "recurrence %d outside [0, %d)", o, order - 1);
+  HY_CHECK(o == 0 ? (p_t && sw && sb && tail && !v_in) : (v_in != nullptr),
+           o == 0 ? "null pointer: recurrence 0 needs p_t, sw, sb, tail (and no v_in)" : "null pointer: v_in");
+  HY_CHECK(pos && (reinterpret_cast<uintptr_t>(pos) & 3u) == 0, "null or misaligned device position");
+  HY_CHECK(aligned16(k) && aligned16(h), "k and h must be 16-byte aligned");
+  return 0;
+}
+
+HY_API int hyena_b200_decode_step_dev(const float* p_t, const float* in_bias, const float* sw, const float* sb,
+                                      const float* k, const float* fbias, float* h, float* tail, float* s_t,
+                                      const float* v_in, float* out, float* part, const int* pos, int B, int cache_B, int D,
+                                      int order, int o, int t_max, int Lcap, void* stream) {
+  if (check_decode_shape(B, cache_B, D, order, Lcap)) return 1;
+  HY_CHECK(k && fbias && h && s_t && out && part, "null pointer");
+  if (check_dev_step(o, order, p_t, sw, sb, tail, v_in, k, h, pos)) return 1;
+  HY_CHECK(t_max >= 1 && t_max <= Lcap, "position bound %d outside [1, %d]", t_max, Lcap);
+  const int ld = dec::ld_for(Lcap), F = order - 1;
+  dec::DotArgs dot{h, k + (size_t)o * ld, part, B, D, 0, ld, F * ld, dec::chunks_for(Lcap)};
+  dec::StepArgs st{part, 0, dec::chunks_for(Lcap), k + (size_t)o * ld, fbias + o, F * ld, F, ld, p_t, in_bias, sw, sb, tail,
+                   s_t, v_in, h, out, B, D, (order + 1) * D, order, 0, (order - 1 - o) * D, o == order - 2};
+  HY_CUDA(launch_decode_step_dev(dot, st, pos, dec::chunks_for(t_max), (cudaStream_t)stream));
+  return 0;
+}
+
+HY_API int hyena_b200_decode_win_step_dev(const float* p_t, const float* in_bias, const float* sw, const float* sb,
+                                          const float* k, const float* fbias, float* h, float* tail, float* s_t,
+                                          const float* v_in, float* out, float* part, const float* win, const int* pos, int B,
+                                          int cache_B, int D, int order, int o, int W, int Lcap, void* stream) {
+  if (check_decode_shape(B, cache_B, D, order, Lcap)) return 1;
+  HY_CHECK(k && fbias && h && s_t && out && part && win, "null pointer");
+  if (check_dev_step(o, order, p_t, sw, sb, tail, v_in, k, h, pos)) return 1;
+  HY_CHECK(W >= 1 && W <= Lcap, "window width %d outside [1, %d]", W, Lcap);
+  const int ld = dec::ld_for(Lcap), F = order - 1;
+  dec::DotArgs dot{h, k + (size_t)o * ld, part, B, D, 0, ld, F * ld, dec::chunks_for(Lcap)};
+  dec::WinStepArgs w{{part, 0, dec::chunks_for(Lcap), k + (size_t)o * ld, fbias + o, F * ld, F, ld, p_t, in_bias, sw, sb,
+                      tail, s_t, v_in, h, out, B, D, (order + 1) * D, order, 0, (order - 1 - o) * D, o == order - 2},
+                     win, W, 0};
+  HY_CUDA(launch_decode_win_step_dev(dot, w, pos, dec::chunks_for(W), (cudaStream_t)stream));
+  return 0;
+}
+
+HY_API int hyena_b200_decode_branch_step_dev(const float* p_t, const float* in_bias, const float* sw, const float* sb,
+                                             const float* k, const float* fbias, float* h, float* tail, float* s_t,
+                                             const float* v_in, float* out, float* part, const float* f, const int* parent,
+                                             const int* pos, int R, int D, int order, int o, int H, int Lcap, void* stream) {
+  if (check_decode_shape(R, R, D, order, Lcap)) return 1;
+  HY_CHECK(k && fbias && h && s_t && out && part && f && parent, "null pointer");
+  if (check_dev_step(o, order, p_t, sw, sb, tail, v_in, k, h, pos)) return 1;
+  const int ld = dec::ld_for(Lcap), F = order - 1;
+  HY_CHECK((H & 3) == 0 && H >= 4 && H <= ld, "branch history width %d must be a multiple of 4 in [4, %d]", H, ld);
+  const float* kb = k + (size_t)o * ld + (ld - H);
+  dec::DotArgs dot{h, kb, part, R, D, 0, H, F * ld, dec::chunks_for(H)};
+  dec::BranchStepArgs w{{part, 0, dec::chunks_for(H), kb, fbias + o, F * ld, F, H, p_t, in_bias, sw, sb, tail, s_t, v_in, h,
+                         out, R, D, (order + 1) * D, order, 0, (order - 1 - o) * D, o == order - 2},
+                        f, parent};
+  HY_CUDA(launch_decode_branch_step_dev(dot, w, pos, dec::chunks_for(H), (cudaStream_t)stream));
+  return 0;
+}
+
+HY_API int hyena_b200_decode_pos_advance(int* pos, void* stream) {
+  HY_CHECK(pos && (reinterpret_cast<uintptr_t>(pos) & 3u) == 0, "null or misaligned device position");
+  HY_CUDA(launch_decode_pos_advance(pos, (cudaStream_t)stream));
   return 0;
 }
 

@@ -14,6 +14,8 @@
 //                          kernel run on h + b with t - b) and the precomputed F[t-b] = sum_{s<b} k[t-s] g[s] is added
 //   decode_branch_step_kernel the same for a branched cache (decode_args.h BranchStepArgs): each batch row is a branch with
 //                          its own history from b on, and F is read from the row of the branch's parent
+//   *_dev_kernel           the same steps with the position read on the device (decode_args.h DevPos), for a step captured
+//                          once in a CUDA graph and replayed at every position; decode_pos_advance_kernel moves it
 // fp32 throughout, no atomics: every sum has a fixed order, so a step is bitwise reproducible.
 #pragma once
 #include <cuda_runtime.h>
@@ -54,7 +56,7 @@ __global__ void __launch_bounds__(256) decode_hist_kernel(const HistArgs a) {
 
 // part[b][d][chunk] = sum_{s in chunk, s < t} h[b][d][s] k[t-s]   for the batch rows [z*BG, z*BG + BG)
 template <int BG, int R>
-__global__ void __launch_bounds__(32 * kDotWarps) decode_dot_kernel(const DotArgs a) {
+__device__ __forceinline__ void dot_body(const DotArgs a) {
   const int lane = threadIdx.x & 31;
   const int d = blockIdx.y * kDotWarps + (threadIdx.x >> 5);
   if (d >= a.D) return;
@@ -102,6 +104,26 @@ __global__ void __launch_bounds__(32 * kDotWarps) decode_dot_kernel(const DotArg
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
     const int b = b0 + i;
     if (lane == 0 && b < a.B) a.part[((size_t)b * a.D + d) * a.nchunk_max + chunk] = s;
+  }
+}
+
+template <int BG, int R>
+__global__ void __launch_bounds__(32 * kDotWarps) decode_dot_kernel(const DotArgs a) { dot_body<BG, R>(a); }
+
+// decode_dot_kernel with t (and the history offset) read from the device position: the grid covers a fixed chunk bound and
+// the CTAs of chunks at or past t leave at once (the combine reads only the ceil(t / kChunk) partials below them)
+template <int BG>
+__global__ void __launch_bounds__(32 * kDotWarps) decode_dot_dev_kernel(DotArgs a, const DevPos p) {
+  const int t0 = p.pos[0];
+  const int off = p.mode == kPosWindow ? p.pos[1] : p.mode == kPosBranch ? p.pos[2] : 0;
+  a.t = t0 - off;
+  if ((int)blockIdx.x * kChunk >= a.t) return;
+  if (p.mode == kPosWindow) a.h += off;
+  switch ((a.ld - 1 - a.t) & 3) {
+    case 0: dot_body<BG, 0>(a); break;
+    case 1: dot_body<BG, 1>(a); break;
+    case 2: dot_body<BG, 2>(a); break;
+    default: dot_body<BG, 3>(a); break;
   }
 }
 
@@ -181,6 +203,49 @@ __global__ void __launch_bounds__(32 * kStepWarps) decode_branch_step_kernel(con
   const float acc = reduce_partials(w.st, row, lane) + f[w.st.t];
   step_epilogue(w.st, row, b, d, lane, acc);
 }
+
+// the combine kernels of a device-position step: t (and win_b, base) from pos, then the same bodies as above
+__device__ __forceinline__ void dev_position(StepArgs& st, int t) {
+  st.t = t;
+  st.nchunk = (t + kChunk - 1) / kChunk;
+}
+
+__global__ void __launch_bounds__(32 * kStepWarps) decode_step_dev_kernel(StepArgs a, const int* pos) {
+  const int lane = threadIdx.x & 31;
+  const int row = blockIdx.x * kStepWarps + (threadIdx.x >> 5);      // b * D + d
+  if (row >= a.B * a.D) return;
+  dev_position(a, pos[0]);
+  const int b = row / a.D, d = row - b * a.D;
+  const float acc = reduce_partials(a, row, lane);
+  step_epilogue(a, row, b, d, lane, acc);
+}
+
+// the partials cover [win_b, t); st.t stays absolute (g_t is written at h[t]) while the partial count follows t - win_b
+__global__ void __launch_bounds__(32 * kStepWarps) decode_win_step_dev_kernel(WinStepArgs w, const int* pos) {
+  const int lane = threadIdx.x & 31;
+  const int row = blockIdx.x * kStepWarps + (threadIdx.x >> 5);      // b * D + d
+  if (row >= w.st.B * w.st.D) return;
+  const int t = pos[0], j = t - pos[1];
+  dev_position(w.st, j);
+  w.st.t = t;
+  const int b = row / w.st.D, d = row - b * w.st.D;
+  const float acc = reduce_partials(w.st, row, lane) + w.win[(size_t)row * w.wstride + j];
+  step_epilogue(w.st, row, b, d, lane, acc);
+}
+
+__global__ void __launch_bounds__(32 * kStepWarps) decode_branch_step_dev_kernel(BranchStepArgs w, const int* pos) {
+  const int lane = threadIdx.x & 31;
+  const int row = blockIdx.x * kStepWarps + (threadIdx.x >> 5);      // b * D + d
+  if (row >= w.st.B * w.st.D) return;
+  dev_position(w.st, pos[0] - pos[2]);
+  const int b = row / w.st.D, d = row - b * w.st.D;
+  const float* f = w.f + ((size_t)__ldg(w.parent + b) * w.st.D + d) * w.st.ld;
+  const float acc = reduce_partials(w.st, row, lane) + f[w.st.t];
+  step_epilogue(w.st, row, b, d, lane, acc);
+}
+
+// the end of a device-position step: one thread, launched after every kernel of the step has read pos
+__global__ void decode_pos_advance_kernel(int* pos) { pos[0] += 1; }
 
 }  // namespace dec
 }  // namespace hy

@@ -72,6 +72,16 @@ struct WinStepArgs {
   int j;                 // t - b
 };
 
+// A step whose position is read on the device (a captured CUDA graph replays it at every position): pos = [t, win_b, base]
+// (int32).  The dot kernel runs on a grid of a fixed chunk bound; it takes its t and history offset from pos by `mode`:
+constexpr int kPosPlain = 0;              // t = pos[0] over h
+constexpr int kPosWindow = 1;             // t = pos[0] - pos[1] over h + pos[1]
+constexpr int kPosBranch = 2;             // t = pos[0] - pos[2] over the branch rows h
+struct DevPos {
+  const int* pos;        // [t, win_b, base]
+  int mode;              // kPos*
+};
+
 // ---- extending a cache by n positions at once (decode_extend.cuh)
 constexpr int kExtRJ = 8;                 // outputs per thread of the direct Toeplitz kernel (register block)
 constexpr int kExtWarps = 8;              // warps per CTA of the direct Toeplitz kernel

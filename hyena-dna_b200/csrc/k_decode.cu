@@ -78,4 +78,59 @@ cudaError_t launch_decode_branch_step(const dec::DotArgs& dot, const dec::Branch
   return cudaGetLastError();
 }
 
+// ---- device-position steps: fixed grids, the position read by the kernels (decode.cuh *_dev_kernel)
+static cudaError_t launch_dot_dev(const dec::DotArgs& dot, const dec::DevPos& p, int nchunk, int kind, cudaStream_t s) {
+  const int BG = dot.B <= 1 ? 1 : dot.B <= 2 ? 2 : dot.B <= 4 ? 4 : 8;
+  const int threads = 32 * dec::kDotWarps;
+  dim3 grid(nchunk, (dot.D + dec::kDotWarps - 1) / dec::kDotWarps, (dot.B + BG - 1) / BG);
+  prof_begin(kind, s);
+  switch (BG) {
+    case 1: dec::decode_dot_dev_kernel<1><<<grid, threads, 0, s>>>(dot, p); break;
+    case 2: dec::decode_dot_dev_kernel<2><<<grid, threads, 0, s>>>(dot, p); break;
+    case 4: dec::decode_dot_dev_kernel<4><<<grid, threads, 0, s>>>(dot, p); break;
+    default: dec::decode_dot_dev_kernel<8><<<grid, threads, 0, s>>>(dot, p); break;
+  }
+  prof_end(kind, s);
+  return cudaGetLastError();
+}
+
+static dim3 step_grid(int B, int D) { return dim3((B * D + dec::kStepWarps - 1) / dec::kStepWarps); }
+
+cudaError_t launch_decode_step_dev(const dec::DotArgs& dot, const dec::StepArgs& st, const int* pos, int nchunk,
+                                   cudaStream_t s) {
+  cudaError_t e = launch_dot_dev(dot, dec::DevPos{pos, dec::kPosPlain}, nchunk, K_DECODE_STEP, s);
+  if (e != cudaSuccess) return e;
+  prof_begin(K_DECODE_STEP, s);
+  dec::decode_step_dev_kernel<<<step_grid(st.B, st.D), 32 * dec::kStepWarps, 0, s>>>(st, pos);
+  prof_end(K_DECODE_STEP, s);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_decode_win_step_dev(const dec::DotArgs& dot, const dec::WinStepArgs& w, const int* pos, int nchunk,
+                                       cudaStream_t s) {
+  cudaError_t e = launch_dot_dev(dot, dec::DevPos{pos, dec::kPosWindow}, nchunk, K_DECODE_WIN_STEP, s);
+  if (e != cudaSuccess) return e;
+  prof_begin(K_DECODE_WIN_STEP, s);
+  dec::decode_win_step_dev_kernel<<<step_grid(w.st.B, w.st.D), 32 * dec::kStepWarps, 0, s>>>(w, pos);
+  prof_end(K_DECODE_WIN_STEP, s);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_decode_branch_step_dev(const dec::DotArgs& dot, const dec::BranchStepArgs& w, const int* pos, int nchunk,
+                                          cudaStream_t s) {
+  cudaError_t e = launch_dot_dev(dot, dec::DevPos{pos, dec::kPosBranch}, nchunk, K_DECODE_WIN_STEP, s);
+  if (e != cudaSuccess) return e;
+  prof_begin(K_DECODE_WIN_STEP, s);
+  dec::decode_branch_step_dev_kernel<<<step_grid(w.st.B, w.st.D), 32 * dec::kStepWarps, 0, s>>>(w, pos);
+  prof_end(K_DECODE_WIN_STEP, s);
+  return cudaGetLastError();
+}
+
+// counted by launch_count but under no kind: it is not a step kernel
+cudaError_t launch_decode_pos_advance(int* pos, cudaStream_t s) {
+  dec::decode_pos_advance_kernel<<<1, 1, 0, s>>>(pos);
+  count_launch();
+  return cudaGetLastError();
+}
+
 }  // namespace hy

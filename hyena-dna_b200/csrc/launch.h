@@ -26,6 +26,7 @@ enum Kind {
 };
 void prof_begin(int kind, cudaStream_t s);     // api.cu: records an event when profiling is on
 void prof_end(int kind, cudaStream_t s);       // api.cu: records an event when profiling is on; counts the launch
+void count_launch();                           // api.cu: counts a launch that belongs to no kernel class
 cudaError_t launch_col_fwd(int mode, const PassArgs& a, int rows, cudaStream_t s);
 cudaError_t launch_col_inv(int mode, const PassArgs& a, int rows, cudaStream_t s);
 cudaError_t launch_row_pass(int mode, const PassArgs& a, int rows, cudaStream_t s);
@@ -63,6 +64,14 @@ cudaError_t launch_decode_hist(const dec::HistArgs& a, cudaStream_t s);
 cudaError_t launch_decode_step(const dec::DotArgs& dot, const dec::StepArgs& st, cudaStream_t s);
 cudaError_t launch_decode_win_step(const dec::DotArgs& dot, const dec::WinStepArgs& w, cudaStream_t s);
 cudaError_t launch_decode_branch_step(const dec::DotArgs& dot, const dec::BranchStepArgs& w, cudaStream_t s);
+// the same steps with the position read on the device from pos = [t, win_b, base]; the dot kernel's grid is nchunk chunks
+cudaError_t launch_decode_step_dev(const dec::DotArgs& dot, const dec::StepArgs& st, const int* pos, int nchunk,
+                                   cudaStream_t s);
+cudaError_t launch_decode_win_step_dev(const dec::DotArgs& dot, const dec::WinStepArgs& w, const int* pos, int nchunk,
+                                       cudaStream_t s);
+cudaError_t launch_decode_branch_step_dev(const dec::DotArgs& dot, const dec::BranchStepArgs& w, const int* pos, int nchunk,
+                                          cudaStream_t s);
+cudaError_t launch_decode_pos_advance(int* pos, cudaStream_t s);
 // k_decode_extend.cu: extending a decode cache by n positions (decode_extend.cuh)
 cudaError_t launch_decode_ext_hist(const dec::ExtHistArgs& a, cudaStream_t s);
 cudaError_t launch_decode_ext_dot(const dec::ExtDotArgs& a, cudaStream_t s);

@@ -47,6 +47,13 @@ def _host_index(index, n, what):
     return out
 
 
+class _PositionState:
+    """The values last written to a device position (None: unknown), shared by every cache that holds the tensor."""
+
+    def __init__(self):
+        self.value = None
+
+
 class DecodeCache:
     """Decoding state of one HyenaOperator (``HyenaOperator.allocate_decode_cache``), or of every mixer of a stack
     (``Backbone.allocate_decode_cache``: ``layers`` holds one per layer, looked up by module identity).
@@ -76,7 +83,11 @@ class DecodeCache:
       parent (R,) int32      the row of f each branch reads
       tail, s_t, part        as above with R rows and ceil(H / 1024) partials
     so out_o[t] = F_o[parent][t-b] + sum_{b<=s<t} k_o[t-s] g_o[s] + (k_o[0] + bias_o) g_o[t] for b <= t < b + Hc, and no
-    operation on a branch reads the context before b."""
+    operation on a branch reads the context before b.
+
+    Device position (``sync_position``, StepGraph): ``pos`` (3,) int32 on the device holds [t, win_b, base] for the step
+    kernels that read the position on the device.  One tensor serves every layer of a stack.  It is allocated on first
+    use and written only by ``sync_position`` and by a replayed StepGraph; ``t`` on the host stays authoritative."""
 
     def __init__(self, owner=None, batch_size=0, max_seqlen=0, lcap=0, k=None, bias=None, h=None, tail=None, s_t=None,
                  part=None, layers=None):
@@ -87,6 +98,7 @@ class DecodeCache:
         self._t = 0
         self.win_b, self.win_wc, self.win_f, self.steps = 0, 0, None, 0
         self._branched, self.base, self.hc, self.f, self.parent = False, 0, 0, None, None
+        self.pos, self._pos_state = None, None
         if owner is not None:
             self.d_model, self.order = owner.d_model, owner.order
 
@@ -199,6 +211,23 @@ class DecodeCache:
             raise HyenaB200Error("the position of a stack's cache is advanced by its layers")
         self._t = int(value)
 
+    def sync_position(self):
+        """The device position ``pos`` = [t, win_b, base] (allocated on first use, one tensor for a stack and all its layers),
+        written from the host fields when they differ from the values it was last given."""
+        cs = self.layers or [self]
+        want = {(c.t, c.win_b, c.base) for c in cs}
+        if len(want) != 1:
+            raise HyenaB200Error(f"the layers of this stack's cache disagree on (t, win_b, base): {sorted(want)}")
+        want = want.pop()
+        if self.pos is None or self._pos_state is None:
+            pos, state = torch.zeros(3, dtype=torch.int32, device=cs[0].h.device), _PositionState()
+            for c in [self] + self.layers:
+                c.pos, c._pos_state = pos, state
+        if self._pos_state.value != want:
+            self.pos.copy_(torch.tensor(want, dtype=torch.int32))
+            self._pos_state.value = want
+        return self.pos
+
     def for_module(self, module):
         """The state of ``module`` (this cache itself, or the layer cache allocated for it)."""
         if self.owner is module:
@@ -207,3 +236,201 @@ class DecodeCache:
             if c.owner is module:
                 return c
         raise HyenaB200Error("this DecodeCache was not allocated for this HyenaOperator")
+
+
+class StepGraph:
+    """``step`` of a HyenaOperator, Block or Backbone on one cache, captured in CUDA graphs and replayed per position.
+
+    An eager step costs about 0.1 ms of host and launch time per operator (DESIGN.md section 4.13).  Here the whole step --
+    the projections, the step kernels, the add + LayerNorm kernels, the block MLP and ln_f -- is one graph launch.  Its
+    kernels read the position from the cache's device position (``DecodeCache.sync_position``), and the last kernel of the
+    graph advances it, so every replay steps the next position.  The outputs are the bits eager ``step`` gives on the same
+    route.  The routes differ in one case: at t >= WINDOW_MIN_T less than WINDOW_AFTER_STEPS steps after a prefill or an
+    extend, eager ``step`` stays on the plain route while a graph step opens a window, whose sums run in another order.
+
+    Routes: the plain step (below ops.WINDOW_MIN_T), the windowed step and the branch step (a branched cache) are separate
+    graphs, each captured on first use: warm-up steps on a side stream (their writes to the cache undone), then the capture.
+    Before each replay the host runs the route rule on its copy of the position.  When the next position needs a window
+    and none holds it, the window is refreshed eagerly, outside the graph, on the current stream: the first step at
+    t >= WINDOW_MIN_T opens one, with no run of plain steps before it.  After each replay the host advances ``t`` of every
+    layer cache (and the step count of an unbranched one), so eager ``step``, ``extend``, ``fork`` and ``select`` go on
+    from there; steps taken eagerly in between are picked up at the next replay.
+
+    ``step`` returns static output tensors that the next ``step`` of this object overwrites: copy what you keep.  It
+    raises before any device work on an input of another shape, dtype or device than the captured one, at Lcap or a
+    branch horizon, and when a buffer the graphs read was replaced since their capture."""
+
+    WARMUP = 2
+
+    def __init__(self, module, cache, batch_size=None, dtype=torch.float32, residual=False):
+        from .block import Backbone, Block
+        from .hyena import HyenaOperator
+        if isinstance(module, HyenaOperator):
+            mixers = [module]
+        elif isinstance(module, Block):
+            mixers = [module.mixer]
+        elif isinstance(module, Backbone):
+            mixers = [layer.mixer for layer in module.layers]
+        else:
+            raise HyenaB200Error(f"StepGraph: expected a HyenaOperator, Block or Backbone; got {type(module).__name__}")
+        if not all(isinstance(m, HyenaOperator) for m in mixers):
+            raise HyenaB200Error("StepGraph: every mixer must be a HyenaOperator (incremental decoding)")
+        if not isinstance(cache, DecodeCache):
+            raise HyenaB200Error(f"StepGraph needs a DecodeCache, got {type(cache).__name__}")
+        if residual and not isinstance(module, Block):
+            raise HyenaB200Error("StepGraph: a residual input exists for a Block only")
+        self.module, self.mixers = module, mixers
+        self.caches = [cache.for_module(m) for m in mixers]
+        # the position the graphs advance: the stack's (one for all its layers) or the operator's own
+        self.cache = cache if isinstance(module, Backbone) or len(self.caches) > 1 else self.caches[0]
+        B = cache.batch_size if batch_size is None else int(batch_size)
+        if B != self.caches[0].batch_size:
+            raise HyenaB200Error(f"StepGraph: batch size {B} differs from the decode cache's {self.caches[0].batch_size}")
+        if any(m.filter_fn.bidirectional for m in mixers):
+            raise HyenaB200Error("decoding needs a causal filter; this HyenaFilter is bidirectional")
+        self.device = self.caches[0].h.device
+        self.shape, self.dtype = (B, 1, mixers[0].d_model), dtype
+        self.residual = residual
+        self.res_dtype = (torch.float32 if module.residual_in_fp32 else dtype) if residual else None
+        self._graphs, self._keys, self._side, self._scratch = {}, {}, None, []
+        self._check_room()
+        self._in = torch.zeros(self.shape, dtype=dtype, device=self.device)
+        self._res = torch.zeros(self.shape, dtype=self.res_dtype, device=self.device) if residual else None
+        self._graph(self.plan()[0])
+
+    # ---------------------------------------------------------------------------------------- host planning
+    def plan(self):
+        """(route, refresh) of the next step: route "plain", "window" or "branch"; refresh when the window must be opened
+        (decode_window_plan with the step count satisfied: a graph step never waits WINDOW_AFTER_STEPS steps)."""
+        from . import ops
+        c = self.caches[0]
+        if c.branched:
+            return "branch", False
+        route = ops.decode_window_plan(c.t, c.lcap, ops.WINDOW_AFTER_STEPS, c.win_b, c.win_wc)
+        return ("window", True) if route == "refresh" else (route, False)
+
+    def _check_room(self):
+        c = self.caches[0]
+        if c.branched and c.t >= c.base + c.hc:
+            raise HyenaB200Error(f"StepGraph: decoding past the branch horizon: position {c.t} is base + Hc = {c.base} + "
+                                 f"{c.hc} (fork with a larger horizon, up to Lcap = {c.lcap})")
+        if c.t >= c.lcap:
+            raise HyenaB200Error(f"StepGraph: decoding past the cache: position {c.t} is Lcap = {c.lcap}")
+
+    _READS = {"plain": ("k", "bias", "h", "tail", "s_t", "part", "pos"),
+              "window": ("k", "bias", "h", "tail", "s_t", "part", "pos", "win_f"),
+              "branch": ("k", "bias", "h", "tail", "s_t", "part", "pos", "f", "parent")}
+
+    def _key(self, route):
+        return tuple((id(x), x.data_ptr()) if x is not None else None
+                     for c in self.caches for x in (getattr(c, n) for n in self._READS[route]))
+
+    def _check_input(self, u_t, residual):
+        for name, x, dt in (("input", u_t, self.dtype), ("residual", residual, self.res_dtype)):
+            if x is None and dt is None:
+                continue
+            if x is None or dt is None:
+                raise HyenaB200Error(f"StepGraph.step: this graph was captured {'with' if dt is not None else 'without'} "
+                                     "a residual input")
+            if tuple(x.shape) != self.shape or x.dtype != dt or x.device != self.device:
+                raise HyenaB200Error(f"StepGraph.step: {name} {tuple(x.shape)} {x.dtype} on {x.device} differs from the "
+                                     f"captured {self.shape} {dt} on {self.device}")
+
+    # ---------------------------------------------------------------------------------------- stepping
+    def step(self, u_t, residual=None):
+        """One position: u_t (B, 1, D) -> the module's step output (a Block's is (hidden_states, residual)), in static
+        tensors that the next step overwrites."""
+        from . import ops
+        self._check_input(u_t, residual)
+        self._check_room()
+        route, refresh = self.plan()
+        if route in self._keys and self._key(route) != self._keys[route]:
+            raise HyenaB200Error("StepGraph.step: a buffer of the decode cache was replaced since the capture (reallocated, "
+                                 "re-forked or re-synced elsewhere); capture a new StepGraph")
+        if refresh:
+            for c in self.caches:
+                ops.decode_window_refresh(c)
+        graph, out = self._graph(route)
+        c0 = self.caches[0]
+        t = c0.t
+        self.cache.sync_position()
+        self._in.copy_(u_t)
+        if residual is not None:
+            self._res.copy_(residual)
+        graph.replay()
+        for c in self.caches:
+            c.t += 1
+            if not c.branched:
+                c.steps += 1
+        self.cache._pos_state.value = (t + 1, c0.win_b, c0.base)
+        return out
+
+    def _graph(self, route):
+        """(graph, static output) of ``route``, captured on first use."""
+        if route not in self._graphs:
+            self._graphs[route] = self._capture(route)
+            self._keys[route] = self._key(route)
+        return self._graphs[route]
+
+    def _run(self, route):
+        """The step on the static inputs with the device-position kernels of ``route``, then the position advance."""
+        from . import ops
+        from .block import Backbone, Block
+        if route == "plain":
+            def core(p_t, ib, sw, sb, c):
+                return ops.decode_step_dev(p_t, ib, sw, sb, c, min(c.lcap, ops.WINDOW_MIN_T))
+        else:
+            core = ops.decode_win_step_dev if route == "window" else ops.decode_branch_step_dev
+
+        def mix(op, c):
+            return lambda y: op._step_with(y, c, core)
+        m = self.module
+        with torch.no_grad():
+            if isinstance(m, Backbone):
+                hidden, res = self._in, None
+                for layer, c in zip(m.layers, self.caches):
+                    hidden, res = layer._run(hidden, res, mix(layer.mixer, c))
+                y, _ = Block._add_norm(hidden, res, m.ln_f)
+                out = y.to(hidden.dtype)
+            elif isinstance(m, Block):
+                out = m._run(self._in, self._res, mix(m.mixer, self.caches[0]))
+            else:
+                out = m._step_with(self._in, self.caches[0], core)
+            ops.decode_pos_advance(self.cache.pos)
+        return out
+
+    def _capture(self, route):
+        from . import ops
+        caches, c0 = self.caches, self.caches[0]
+        if route == "window":
+            for c in caches:
+                if c.win_f is None:           # the refresh writes it in place from now on (decode_window_refresh)
+                    c.win_f = torch.zeros(c.order - 1, c.batch_size, c.d_model, ops.WINDOW, dtype=torch.float32,
+                                          device=c.h.device)
+        pos = self.cache.sync_position()
+        # warm-up at the current position: the library's lazy set-up for the capturing stream (cuBLAS workspace, weight
+        # images, module loading) happens here, not inside the capture.  A step writes g_t into h and shifts the tail:
+        # both are restored.  The warm-up position keeps every route in bounds (window base t - t mod 4).
+        j = c0.t - c0.base if c0.branched else c0.t
+        saved = [(c.tail.clone(), c.h[..., j].clone()) for c in caches]
+        warm = torch.tensor([c0.t, c0.t - c0.t % 4, c0.base], dtype=torch.int32)
+        if self._side is None:
+            self._side = torch.cuda.Stream(device=self.device)
+        side = self._side
+        side.wait_stream(torch.cuda.current_stream(self.device))
+        # torch's streams are pooled, so the library's per-stream weight-image scratch of the capturing stream could be
+        # replaced and freed by other work on it later: the graph gets scratch of its own, held here as long as it lives
+        with ops.private_weight_images(self.device, side, self._scratch):
+            with torch.cuda.stream(side):
+                for _ in range(self.WARMUP):
+                    pos.copy_(warm)
+                    self._run(route)
+                for c, (tail, col) in zip(caches, saved):
+                    c.tail.copy_(tail)
+                    c.h[..., j].copy_(col)
+            torch.cuda.current_stream(self.device).wait_stream(side)
+            self.cache._pos_state.value = None
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph, stream=side):
+                out = self._run(route)
+        return graph, out

@@ -13,7 +13,7 @@ import torch.nn as nn
 
 from . import ops
 from ._lib import HyenaB200Error
-from .decode import DecodeCache
+from .decode import DecodeCache, StepGraph
 
 
 class OptimModule(nn.Module):
@@ -487,16 +487,26 @@ class HyenaOperator(nn.Module):
         (ops.decode_window_plan chooses).  On a branched cache (DecodeCache.fork) the step reads each branch's positions since
         the fork base only (ops.decode_branch_step)."""
         c = self._decode_checks(u_t, cache, 1)
+        y = self._step_with(u_t, c, ops.decode_branch_step if c.branched else ops.decode_step_auto)
+        c.t += 1
+        return y
+
+    def _step_with(self, u_t, c, core):
+        """The work of step on the operator's cache ``c`` with ``core`` (one of the ops.decode_*step functions) for the
+        operator itself; no checks and no position advance (StepGraph captures this with the device-position steps)."""
         with torch.no_grad():
             in_dtype = u_t.dtype
             B, D = u_t.shape[0], self.d_model
             u = u_t.to(torch.float32).reshape(B, D)
             p_t = torch.nn.functional.linear(u, self.in_proj.weight).contiguous()          # bias added in the kernel
             ib, sw, sb = self._decode_params()
-            y_pre = (ops.decode_branch_step if c.branched else ops.decode_step_auto)(p_t, ib, sw, sb, c)
+            y_pre = core(p_t, ib, sw, sb, c)
             y = torch.nn.functional.linear(y_pre, self.out_proj.weight, self.out_proj.bias)
-            c.t += 1
         return y.reshape(B, 1, D).to(in_dtype)
+
+    def capture_step(self, cache, batch_size=None, dtype=torch.float32):
+        """A decode.StepGraph: ``step`` on ``cache`` captured in CUDA graphs and replayed one position at a time."""
+        return StepGraph(self, cache, batch_size, dtype)
 
     def extend(self, u, cache):
         """n >= 1 more positions at once: u (B, n, D) -> y (B, n, D), the outputs at positions [cache.t, cache.t + n);

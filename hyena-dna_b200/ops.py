@@ -3,6 +3,8 @@
 PyTorch provides device memory, streams and autograd plumbing; all arithmetic of the custom-kernel
 span runs in libhyena_b200.so.  Inputs must be CUDA fp32 tensors -- anything else raises.
 """
+import contextlib
+
 import torch
 
 from . import _lib
@@ -480,6 +482,24 @@ def _gelu_code(approximate):
     if approximate not in _GELU_CODES:
         raise _lib.HyenaB200Error(f"GELU approximate must be 'tanh' or 'none', got {approximate!r}")
     return _GELU_CODES[approximate]
+
+
+@contextlib.contextmanager
+def private_weight_images(device, stream, keep):
+    """proj_gemm calls on ``stream`` inside the block use weight-image scratch of their own instead of the shared
+    per-stream entry of _wimg_cache, and that scratch is appended to ``keep``.  For CUDA-graph capture: a graph bakes the
+    scratch address in, while the shared entry can be replaced (and its memory freed) by any later, larger call on a stream
+    with the same handle (torch hands out pooled streams).  The shared entry is restored afterwards."""
+    key = (device.index if device.index is not None else torch.cuda.current_device(), stream.cuda_stream)
+    shared = _wimg_cache.pop(key, None)
+    try:
+        yield
+    finally:
+        own = _wimg_cache.pop(key, None)
+        if own is not None:
+            keep.append(own)
+        if shared is not None:
+            _wimg_cache[key] = shared
 
 
 def proj_gemm(act, act_layout, W, w_transposed, out_layout, bias=None, fir=None, out=None, l_range=None, gelu=None,
@@ -999,6 +1019,76 @@ def decode_branch_step(p_t, in_bias, sw, sb, cache):
                 _ptr(cache.s_t), 0 if first else _ptr(out[o - 1]), _ptr(out[o]), _ptr(cache.part), _ptr(cache.f[o]),
                 _ptr(cache.parent), B, D, O, o, t, b, hc, H, cache.lcap, _stream()))
     return out[-1]
+
+
+# ------------------------------------------------------------------------------------------ device-position steps
+# The steps above take the position from the host (cache.t), so a captured CUDA graph would replay one position forever.
+# These variants read t, the window base and the branch base from cache.pos ([t, win_b, base], int32 on the device) inside
+# the kernels, with a grid fixed at capture time to a chunk bound of the route; decode_pos_advance moves t on the device.
+# They launch nothing else and allocate nothing but their outputs, so a step built from them can be captured
+# (decode.StepGraph).  They sum the same partials in the same order as the host-position kernels: the same bits.
+def _dev_step_check(p_t, in_bias, sw, sb, cache, what):
+    _need_cuda(p_t, in_bias, sw, sb)
+    B = p_t.shape[0]
+    D, O = cache.d_model, cache.order
+    if not p_t.is_contiguous() or tuple(p_t.shape) != (B, (O + 1) * D):
+        raise _lib.HyenaB200Error(f"{what}: p_t must be contiguous (B, {(O + 1) * D})")
+    if cache.pos is None:
+        raise _lib.HyenaB200Error(f"{what}: the cache has no device position (DecodeCache.sync_position)")
+    return B, D, O, [torch.empty(B, D, dtype=torch.float32, device=p_t.device) for _ in range(O - 1)]
+
+
+def decode_step_dev(p_t, in_bias, sw, sb, cache, t_max):
+    """decode_step at the position cache.pos[0] on the device, for positions below t_max (the dot kernel's grid covers
+    chunks_for(min(t_max, Lcap)) chunks); does not advance the position."""
+    B, D, O, out = _dev_step_check(p_t, in_bias, sw, sb, cache, "decode_step_dev")
+    with torch.cuda.device(p_t.device):
+        for o in range(O - 1):
+            first = o == 0
+            _lib.check(_lib.lib().hyena_b200_decode_step_dev(
+                _ptr(p_t) if first else 0, _ptr(in_bias) if first else 0, _ptr(sw) if first else 0,
+                _ptr(sb) if first else 0, _ptr(cache.k), _ptr(cache.bias), _ptr(cache.h[o]), _ptr(cache.tail) if first else 0,
+                _ptr(cache.s_t), 0 if first else _ptr(out[o - 1]), _ptr(out[o]), _ptr(cache.part), _ptr(cache.pos), B,
+                cache.batch_size, D, O, o, int(t_max), cache.lcap, _stream()))
+    return out[-1]
+
+
+def decode_win_step_dev(p_t, in_bias, sw, sb, cache):
+    """decode_win_step at the position cache.pos[0] inside the window based at cache.pos[1] on the device (the window
+    buffer cache.win_f must be allocated; the host keeps pos[1] and win_f current, see decode_window_refresh)."""
+    B, D, O, out = _dev_step_check(p_t, in_bias, sw, sb, cache, "decode_win_step_dev")
+    if cache.win_f is None:
+        raise _lib.HyenaB200Error("decode_win_step_dev: the cache has no window buffer")
+    with torch.cuda.device(p_t.device):
+        for o in range(O - 1):
+            first = o == 0
+            _lib.check(_lib.lib().hyena_b200_decode_win_step_dev(
+                _ptr(p_t) if first else 0, _ptr(in_bias) if first else 0, _ptr(sw) if first else 0,
+                _ptr(sb) if first else 0, _ptr(cache.k), _ptr(cache.bias), _ptr(cache.h[o]), _ptr(cache.tail) if first else 0,
+                _ptr(cache.s_t), 0 if first else _ptr(out[o - 1]), _ptr(out[o]), _ptr(cache.part), _ptr(cache.win_f[o]),
+                _ptr(cache.pos), B, cache.batch_size, D, O, o, cache.win_f.shape[-1], cache.lcap, _stream()))
+    return out[-1]
+
+
+def decode_branch_step_dev(p_t, in_bias, sw, sb, cache):
+    """decode_branch_step at the position cache.pos[0] of a branched cache whose base cache.pos[2] is on the device."""
+    B, D, O, out = _dev_step_check(p_t, in_bias, sw, sb, cache, "decode_branch_step_dev")
+    _branch_args(cache, B, "decode_branch_step_dev")
+    with torch.cuda.device(p_t.device):
+        for o in range(O - 1):
+            first = o == 0
+            _lib.check(_lib.lib().hyena_b200_decode_branch_step_dev(
+                _ptr(p_t) if first else 0, _ptr(in_bias) if first else 0, _ptr(sw) if first else 0,
+                _ptr(sb) if first else 0, _ptr(cache.k), _ptr(cache.bias), _ptr(cache.h[o]), _ptr(cache.tail) if first else 0,
+                _ptr(cache.s_t), 0 if first else _ptr(out[o - 1]), _ptr(out[o]), _ptr(cache.part), _ptr(cache.f[o]),
+                _ptr(cache.parent), _ptr(cache.pos), B, D, O, o, cache.h.shape[-1], cache.lcap, _stream()))
+    return out[-1]
+
+
+def decode_pos_advance(pos):
+    """pos[0] += 1 on the device: the end of a device-position step (once per token for all layers of a stack)."""
+    with torch.cuda.device(pos.device):
+        _lib.check(_lib.lib().hyena_b200_decode_pos_advance(_ptr(pos), _stream()))
 
 
 def decode_branch_extend(p, in_bias, sw, sb, cache, fft=None):

@@ -324,6 +324,34 @@ HY_API int hyena_b200_decode_branch_combine(const float* part, long long row_str
                                             const float* f, const int* parent, int R, int D, int order, int o, int t,
                                             int n, int b, int Hc, int H, int Lcap, void* stream);
 
+/* ---- device-position steps: one step captured in a CUDA graph and replayed at every position ----
+ * pos (3 int32 on the device) = [t, win_b, base]: the position, the base of the open window and the base of a branched
+ * cache.  These calls read no position on the host: their kernels read pos when they run, on grids fixed by the arguments
+ * (the dot kernel's CTAs past the position leave at once).  The caller keeps pos within the bounds below; a replay
+ * cannot check them.  The outputs are bit-identical to the host-position calls at the same state.  They allocate nothing
+ * and never synchronise, so they can be captured once the library has been used on the capturing stream.
+ *   decode_step_dev:        decode_step at t = pos[0], which must stay below t_max <= Lcap (grid: ceil(t_max / 1024)
+ *                           chunks).
+ *   decode_win_step_dev:    decode_win_step at t = pos[0] in the window based at pos[1]: 0 <= t - pos[1] < the window's
+ *                           width, which is at most W (win (B, D, W); grid: ceil(W / 1024) chunks).
+ *   decode_branch_step_dev: decode_branch_step at t = pos[0] of branches based at pos[2]: t - pos[2] < Hc <= H.
+ *   decode_pos_advance:     pos[0] += 1, one thread.  Enqueue it after every call of the step that reads pos.
+ * Launches count under the kinds of the host-position calls; decode_pos_advance's under none (launch_count only).  While
+ * a stream is being captured, the per-launch event timing (profile_begin / profile_end) skips it. */
+HY_API int hyena_b200_decode_step_dev(const float* p_t, const float* in_bias, const float* sw, const float* sb,
+                                      const float* k, const float* fbias, float* h, float* tail, float* s_t,
+                                      const float* v_in, float* out, float* part, const int* pos, int B, int cache_B, int D,
+                                      int order, int o, int t_max, int Lcap, void* stream);
+HY_API int hyena_b200_decode_win_step_dev(const float* p_t, const float* in_bias, const float* sw, const float* sb,
+                                          const float* k, const float* fbias, float* h, float* tail, float* s_t,
+                                          const float* v_in, float* out, float* part, const float* win, const int* pos, int B,
+                                          int cache_B, int D, int order, int o, int W, int Lcap, void* stream);
+HY_API int hyena_b200_decode_branch_step_dev(const float* p_t, const float* in_bias, const float* sw, const float* sb,
+                                             const float* k, const float* fbias, float* h, float* tail, float* s_t,
+                                             const float* v_in, float* out, float* part, const float* f, const int* parent,
+                                             const int* pos, int R, int D, int order, int o, int H, int Lcap, void* stream);
+HY_API int hyena_b200_decode_pos_advance(int* pos, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
