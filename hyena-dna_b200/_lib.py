@@ -41,6 +41,7 @@ SIGNATURES = {
     "hyena_b200_filter_bwd_stage2": (_i, [c_fp] * 11 + [_i, _i, _i, _vp]),
     "hyena_b200_filter_spectrum": (_i, [c_fp, c_fp, _i, _i, _vp, _sz, _vp]),
     "hyena_b200_core_fwd": (_i, [c_fp] * 9 + [_i, _i, _i, _vp, _sz, _vp]),
+    "hyena_b200_core_fwd_rows": (_i, [c_fp] * 10 + [_i, _i, _i, _vp, _sz, _vp]),
     "hyena_b200_core_bwd": (_i, [c_fp] * 16 + [_i, _i, _i, _vp, _sz, _vp]),
     "hyena_b200_fftconv_fwd": (_i, [c_fp] * 4 + [_i, _i, _i, _vp, _sz, _vp]),
     "hyena_b200_fftconv_bwd": (_i, [c_fp] * 7 + [_i, _i, _i, _vp, _sz, _vp]),
@@ -61,6 +62,7 @@ SIGNATURES = {
     "hyena_b200_gemm": (_i, [_i, _i, _i, _i, _i, _f, c_fp, _i, ctypes.c_longlong, c_fp, _i, ctypes.c_longlong, _f, c_fp,
                              _i, ctypes.c_longlong, _i, c_fp, _i, _vp, _sz, _vp]),
     "hyena_b200_decode_hist": (_i, [c_fp] * 6 + [_i] * 6 + [_vp]),
+    "hyena_b200_decode_hist_rows": (_i, [c_fp] * 7 + [_i] * 6 + [_vp]),
     "hyena_b200_decode_step": (_i, [c_fp] * 12 + [_i] * 7 + [_vp]),
     "hyena_b200_decode_win_step": (_i, [c_fp] * 13 + [_i] * 10 + [_vp]),
     "hyena_b200_decode_extend_groups": (_i, [_i] * 4),

@@ -56,14 +56,28 @@ class Block(nn.Module):
         return ops.add_layer_norm(x, r, norm.weight.to(torch.float32), norm.bias.to(torch.float32) if norm.bias is not None
                                   else None, norm.eps)
 
-    def forward(self, hidden_states, residual=None, mixer_subset=None, mixer_kwargs=None):
-        """(hidden_states, residual) -> (mlp(LN2(.)) or mixer output, new residual); block.py:111-180, prenorm branch."""
+    def forward(self, hidden_states, residual=None, mixer_subset=None, mixer_kwargs=None, lengths=None):
+        """(hidden_states, residual) -> (mlp(LN2(.)) or mixer output, new residual); block.py:111-180, prenorm branch.
+        ``lengths``: left-padded rows, passed to the mixer (HyenaOperator.forward); LayerNorm and the MLP act per position."""
         if mixer_subset is not None:
             raise HyenaB200Error("Block: mixer_subset is not supported")
+        if lengths is not None:
+            self._check_lengths(hidden_states, lengths, None, "forward")
+            kw = dict(mixer_kwargs or {}, lengths=lengths)
+            return self._run(hidden_states, residual, lambda y: self.mixer(y, **kw))
         return self._run(hidden_states, residual, lambda y: self.mixer(y, **(mixer_kwargs or {})))
 
-    def prefill(self, hidden_states, residual, cache):
-        """forward over the first positions, filling the mixer's DecodeCache (HyenaOperator.prefill)."""
+    def _check_lengths(self, hidden_states, lengths, cache, how):
+        if not hasattr(self.mixer, "check_lengths"):
+            raise HyenaB200Error(f"Block: the mixer {type(self.mixer).__name__} takes no lengths")
+        self.mixer.check_lengths(hidden_states, lengths, cache, how)
+
+    def prefill(self, hidden_states, residual, cache, lengths=None):
+        """forward over the first positions, filling the mixer's DecodeCache (HyenaOperator.prefill); ``lengths``:
+        left-padded prompts of different lengths."""
+        if lengths is not None:
+            self._check_lengths(hidden_states, lengths, cache, "prefill")
+            return self._decode(hidden_states, residual, lambda y: self.mixer.prefill(y, cache, lengths))
         return self._decode(hidden_states, residual, lambda y: self.mixer.prefill(y, cache))
 
     def step(self, hidden_states, residual, cache):
@@ -71,8 +85,12 @@ class Block(nn.Module):
         position depends on that position only, so the block keeps no state of its own."""
         return self._decode(hidden_states, residual, lambda y: self.mixer.step(y, cache))
 
-    def extend(self, hidden_states, residual, cache):
-        """forward of n more positions (B, n, D) from the mixer's DecodeCache (HyenaOperator.extend)."""
+    def extend(self, hidden_states, residual, cache, lengths=None):
+        """forward of n more positions (B, n, D) from the mixer's DecodeCache (HyenaOperator.extend); ``lengths`` on a fresh
+        cache only (prefill)."""
+        if lengths is not None:
+            self._check_lengths(hidden_states, lengths, cache, "extend")
+            return self._decode(hidden_states, residual, lambda y: self.mixer.extend(y, cache, lengths))
         return self._decode(hidden_states, residual, lambda y: self.mixer.extend(y, cache))
 
     def capture_step(self, cache, batch_size=None, dtype=torch.float32, residual=False):
@@ -114,10 +132,14 @@ class Backbone(nn.Module):
                   prenorm=True, residual_in_fp32=residual_in_fp32) for _ in range(n_layer)])
         self.ln_f = nn.LayerNorm(d_model, eps=layer_norm_epsilon)
 
-    def forward(self, hidden_states):
+    def forward(self, hidden_states, lengths=None):
+        """``lengths``: left-padded rows (HyenaOperator.forward), inference only."""
+        if lengths is not None:
+            self.layers[0]._check_lengths(hidden_states, lengths, None, "forward")
         residual = None
         for layer in self.layers:
-            hidden_states, residual = layer(hidden_states, residual)
+            hidden_states, residual = layer(hidden_states, residual) if lengths is None else \
+                layer(hidden_states, residual, lengths=lengths)
         y, _ = Block._add_norm(hidden_states, residual, self.ln_f)
         return y.to(hidden_states.dtype)
 
@@ -125,28 +147,32 @@ class Backbone(nn.Module):
         """One DecodeCache holding the state of every layer's mixer (decode.py)."""
         return DecodeCache.stack(layer.mixer.allocate_decode_cache(batch_size, max_seqlen) for layer in self.layers)
 
-    def prefill(self, hidden_states, cache):
-        """forward over the first P positions (B, P, D), filling ``cache`` for step()."""
-        return self._decode(hidden_states, cache, "prefill")
+    def prefill(self, hidden_states, cache, lengths=None):
+        """forward over the first P positions (B, P, D), filling ``cache`` for step(); ``lengths``: left-padded prompts of
+        different lengths (HyenaOperator.prefill)."""
+        return self._decode(hidden_states, cache, "prefill", lengths)
 
     def step(self, hidden_states, cache):
         """The output of one more position (B, 1, D)."""
         return self._decode(hidden_states, cache, "step")
 
-    def extend(self, hidden_states, cache):
-        """The outputs of n more positions (B, n, D); on a fresh cache this is prefill."""
-        return self._decode(hidden_states, cache, "extend")
+    def extend(self, hidden_states, cache, lengths=None):
+        """The outputs of n more positions (B, n, D); on a fresh cache this is prefill (``lengths`` there only)."""
+        return self._decode(hidden_states, cache, "extend", lengths)
 
     def capture_step(self, cache, batch_size=None, dtype=torch.float32):
         """A decode.StepGraph of ``step`` on ``cache``: every layer and ln_f in one CUDA graph per route."""
         return StepGraph(self, cache, batch_size, dtype)
 
-    def _decode(self, hidden_states, cache, how):
+    def _decode(self, hidden_states, cache, how, lengths=None):
         if hidden_states.requires_grad:
             raise HyenaB200Error("decoding is inference only: the input requires grad (run under torch.no_grad())")
+        if lengths is not None:
+            self.layers[0]._check_lengths(hidden_states, lengths, cache, how)
         with torch.no_grad():
             residual = None
             for layer in self.layers:
-                hidden_states, residual = getattr(layer, how)(hidden_states, residual, cache)
+                hidden_states, residual = getattr(layer, how)(hidden_states, residual, cache) if lengths is None else \
+                    getattr(layer, how)(hidden_states, residual, cache, lengths)
             y, _ = Block._add_norm(hidden_states, residual, self.ln_f)
             return y.to(hidden_states.dtype)

@@ -138,6 +138,7 @@ static int channels_per_group(size_t bytes_for_A, int B, int D, int L) {
   return (int)n;
 }
 
+static bool aligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3u) == 0; }
 static bool aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7u) == 0; }
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
@@ -490,11 +491,10 @@ HY_API int hyena_b200_spectrum_to_rfft(const float* dk, int fft_size, float* dfi
   return 0;
 }
 
-HY_API int hyena_b200_core_fwd(const float* p, const float* in_bias, const float* sw, const float* sb, const float* kspec,
-                        const float* fbias, float* y_pre, float* c_save, float* gspec_save, int B, int D, int L,
-                        void* workspace, size_t workspace_bytes, void* stream) {
-  if (check_shape(B, D, L)) return 1;
-  HY_CHECK(p && sw && sb && kspec && fbias && y_pre, "null pointer");
+// the three forward passes of core_fwd; row_start non-null: the left-padded modes (core_fwd_rows), the same launch sequence
+static int core_fwd_run(const float* p, const float* in_bias, const float* sw, const float* sb, const float* kspec,
+                        const float* fbias, float* y_pre, float* c_save, float* gspec_save, const int* row_start, int B,
+                        int D, int L, void* workspace, size_t workspace_bytes, void* stream) {
   cudaStream_t s = (cudaStream_t)stream;
   Twiddles T;
   if (get_twiddles(s, &T)) return 1;
@@ -504,8 +504,10 @@ HY_API int hyena_b200_core_fwd(const float* p, const float* in_bias, const float
   a.A = c.A; a.kspec = reinterpret_cast<const float2*>(kspec);
   a.p = p; a.in_bias = in_bias; a.sw = sw; a.sb = sb; a.fbias = fbias; a.out = y_pre; a.out2 = c_save;
   a.gspec = reinterpret_cast<float2*>(gspec_save);
+  a.row_start = row_start;
   a.vec = ((L & 1) == 0) && aligned8(p) && aligned8(y_pre) && (!c_save || aligned8(c_save));
   a.stage = ((L & 3) == 0) && aligned16(p) && !getenv("HYENA_B200_NO_STAGE");
+  const int col_mode = row_start ? COL_GATE_ROWS : COL_GATE, inv_mode = row_start ? INV_CONV_FWD_ROWS : INV_CONV_FWD;
   const PipeCfg pc = pipe_cfg();
   const int G = pc.G < D ? pc.G : D;
   if (pc.S > 0 && c.nch >= G * pc.S && D > G) {
@@ -517,20 +519,44 @@ HY_API int hyena_b200_core_fwd(const float* p, const float* in_bias, const float
       const int n = (D - c0 < G) ? D - c0 : G;
       cudaStream_t st = run.stream(g);
       a.c0 = c0; a.A = c.A + slot * (size_t)(g % pc.S);
-      HY_CUDA(launch_col_fwd(COL_GATE, a, n * B, st));
+      HY_CUDA(launch_col_fwd(col_mode, a, n * B, st));
       HY_CUDA(launch_row_pass(ROW_CONV_FWD, a, n * B, st));
-      HY_CUDA(launch_col_inv(INV_CONV_FWD, a, n * B, st));
+      HY_CUDA(launch_col_inv(inv_mode, a, n * B, st));
     }
     return run.join();
   }
   for (int c0 = 0; c0 < D; c0 += c.nch) {
     const int n = (D - c0 < c.nch) ? D - c0 : c.nch;
     a.c0 = c0;
-    HY_CUDA(launch_col_fwd(COL_GATE, a, n * B, s));
+    HY_CUDA(launch_col_fwd(col_mode, a, n * B, s));
     HY_CUDA(launch_row_pass(ROW_CONV_FWD, a, n * B, s));
-    HY_CUDA(launch_col_inv(INV_CONV_FWD, a, n * B, s));
+    HY_CUDA(launch_col_inv(inv_mode, a, n * B, s));
   }
   return 0;
+}
+
+HY_API int hyena_b200_core_fwd(const float* p, const float* in_bias, const float* sw, const float* sb, const float* kspec,
+                        const float* fbias, float* y_pre, float* c_save, float* gspec_save, int B, int D, int L,
+                        void* workspace, size_t workspace_bytes, void* stream) {
+  if (check_shape(B, D, L)) return 1;
+  HY_CHECK(p && sw && sb && kspec && fbias && y_pre, "null pointer");
+  return core_fwd_run(p, in_bias, sw, sb, kspec, fbias, y_pre, c_save, gspec_save, nullptr, B, D, L, workspace,
+                      workspace_bytes, stream);
+}
+
+HY_API int hyena_b200_core_fwd_rows(const float* p, const float* in_bias, const float* sw, const float* sb,
+                                    const float* kspec, const float* fbias, float* y_pre, float* c_save, float* gspec_save,
+                                    const int* row_start, int B, int D, int L, void* workspace, size_t workspace_bytes,
+                                    void* stream) {
+  if (check_shape(B, D, L)) return 1;
+  HY_CHECK(p && sw && sb && kspec && fbias && y_pre && row_start, "null pointer");
+  HY_CHECK(aligned4(p) && aligned4(sw) && aligned4(sb) && aligned4(fbias) && aligned4(y_pre) && aligned4(row_start) &&
+               (!in_bias || aligned4(in_bias)) && (!c_save || aligned4(c_save)),
+           "misaligned pointer: p, in_bias, sw, sb, fbias, y_pre, c_save and row_start must be 4-byte aligned");
+  HY_CHECK(aligned8(kspec) && (!gspec_save || aligned8(gspec_save)), "misaligned pointer: kspec and gspec_save must be "
+           "8-byte aligned");
+  return core_fwd_run(p, in_bias, sw, sb, kspec, fbias, y_pre, c_save, gspec_save, row_start, B, D, L, workspace,
+                      workspace_bytes, stream);
 }
 
 HY_API int hyena_b200_core_bwd(const float* dy_pre, const float* p, const float* in_bias, const float* sw, const float* sb,
@@ -798,7 +824,21 @@ HY_API int hyena_b200_decode_hist(const float* p, const float* in_bias, const fl
   if (check_decode_shape(B, cache_B, D, order, Lcap)) return 1;
   HY_CHECK(p && sw && sb && h && tail, "null pointer");
   HY_CHECK(P >= 1 && P <= Lcap, "prefill of %d positions outside [1, %d]", P, Lcap);
-  dec::HistArgs a{p, in_bias, sw, sb, h, tail, B, D, (order + 1) * D, P, dec::ld_for(Lcap), (order - 1) * D};
+  dec::HistArgs a{p, in_bias, sw, sb, h, tail, B, D, (order + 1) * D, P, dec::ld_for(Lcap), (order - 1) * D, nullptr};
+  HY_CUDA(launch_decode_hist(a, (cudaStream_t)stream));
+  return 0;
+}
+
+HY_API int hyena_b200_decode_hist_rows(const float* p, const float* in_bias, const float* sw, const float* sb, float* h,
+                                       float* tail, const int* row_start, int B, int cache_B, int D, int order, int P,
+                                       int Lcap, void* stream) {
+  if (check_decode_shape(B, cache_B, D, order, Lcap)) return 1;
+  HY_CHECK(p && sw && sb && h && tail && row_start, "null pointer");
+  HY_CHECK(P >= 1 && P <= Lcap, "prefill of %d positions outside [1, %d]", P, Lcap);
+  HY_CHECK(aligned4(p) && aligned4(sw) && aligned4(sb) && aligned4(h) && aligned4(tail) && aligned4(row_start) &&
+               (!in_bias || aligned4(in_bias)),
+           "misaligned pointer: p, in_bias, sw, sb, h, tail and row_start must be 4-byte aligned");
+  dec::HistArgs a{p, in_bias, sw, sb, h, tail, B, D, (order + 1) * D, P, dec::ld_for(Lcap), (order - 1) * D, row_start};
   HY_CUDA(launch_decode_hist(a, (cudaStream_t)stream));
   return 0;
 }

@@ -26,10 +26,14 @@
 namespace hy {
 namespace dec {
 
-// g[t] = short(v)[t] * short(x_gate)[t] for t < P into h (row stride ld); tail = P(P-2), P(P-1) of every channel
-__global__ void __launch_bounds__(256) decode_hist_kernel(const HistArgs a) {
+// g[t] = short(v)[t] * short(x_gate)[t] for t < P into h (row stride ld); tail = P(P-2), P(P-1) of every channel.
+// ROWS: row b is left-padded, its positions t < s = row_start[b] read as the short filter's padding before t = 0 (0, no
+// in_proj bias): g is 0 there, and a pad position in the tail is 0.
+template <bool ROWS>
+__device__ __forceinline__ void hist_body(const HistArgs& a) {
   const int row = blockIdx.y;                    // b * D + d
   const int b = row / a.D, d = row - b * a.D;
+  const int s = ROWS ? __ldg(a.row_start + b) : 0;
   const int cv = a.C - a.D + d, cg = a.gate + d;
   const float* pv = a.p + ((size_t)b * a.C + cv) * a.P;
   const float* pg = a.p + ((size_t)b * a.C + cg) * a.P;
@@ -38,9 +42,16 @@ __global__ void __launch_bounds__(256) decode_hist_kernel(const HistArgs a) {
   const float g0 = __ldg(a.sw + 3 * cg), g1 = __ldg(a.sw + 3 * cg + 1), g2 = __ldg(a.sw + 3 * cg + 2), gb = __ldg(a.sb + cg);
   float* h = a.h + (size_t)row * a.ld;
   for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < a.P; t += gridDim.x * blockDim.x) {
-    const float vm2 = t >= 2 ? pv[t - 2] + ibv : 0.f, vm1 = t >= 1 ? pv[t - 1] + ibv : 0.f, vp = pv[t] + ibv;
-    const float gm2 = t >= 2 ? pg[t - 2] + ibg : 0.f, gm1 = t >= 1 ? pg[t - 1] + ibg : 0.f, gp = pg[t] + ibg;
-    h[t] = short3(v0, v1, v2, vb, vm2, vm1, vp) * short3(g0, g1, g2, gb, gm2, gm1, gp);
+    if (ROWS) {
+      if (t < s) { h[t] = 0.f; continue; }
+      const float vm2 = t - 2 >= s ? pv[t - 2] + ibv : 0.f, vm1 = t - 1 >= s ? pv[t - 1] + ibv : 0.f, vp = pv[t] + ibv;
+      const float gm2 = t - 2 >= s ? pg[t - 2] + ibg : 0.f, gm1 = t - 1 >= s ? pg[t - 1] + ibg : 0.f, gp = pg[t] + ibg;
+      h[t] = short3(v0, v1, v2, vb, vm2, vm1, vp) * short3(g0, g1, g2, gb, gm2, gm1, gp);
+    } else {
+      const float vm2 = t >= 2 ? pv[t - 2] + ibv : 0.f, vm1 = t >= 1 ? pv[t - 1] + ibv : 0.f, vp = pv[t] + ibv;
+      const float gm2 = t >= 2 ? pg[t - 2] + ibg : 0.f, gm1 = t >= 1 ? pg[t - 1] + ibg : 0.f, gp = pg[t] + ibg;
+      h[t] = short3(v0, v1, v2, vb, vm2, vm1, vp) * short3(g0, g1, g2, gb, gm2, gm1, gp);
+    }
   }
   // tail of channels d, D + d, ..., O D + d (one thread each, first CTA of the row)
   const int nj = a.C / a.D;
@@ -49,10 +60,13 @@ __global__ void __launch_bounds__(256) decode_hist_kernel(const HistArgs a) {
     const float* pc = a.p + ((size_t)b * a.C + c) * a.P;
     const float ib = a.in_bias ? __ldg(a.in_bias + c) : 0.f;
     float* tl = a.tail + ((size_t)b * a.C + c) * 2;
-    tl[0] = a.P >= 2 ? pc[a.P - 2] + ib : 0.f;
+    tl[0] = (ROWS ? a.P - 2 >= s : a.P >= 2) ? pc[a.P - 2] + ib : 0.f;
     tl[1] = pc[a.P - 1] + ib;
   }
 }
+
+__global__ void __launch_bounds__(256) decode_hist_kernel(const HistArgs a) { hist_body<false>(a); }
+__global__ void __launch_bounds__(256) decode_hist_rows_kernel(const HistArgs a) { hist_body<true>(a); }
 
 // part[b][d][chunk] = sum_{s in chunk, s < t} h[b][d][s] k[t-s]   for the batch rows [z*BG, z*BG + BG)
 template <int BG, int R>

@@ -33,6 +33,7 @@ struct HistArgs {
   float* tail;           // (B, C, 2)
   int B, D, C, P, ld;
   int gate;              // channel offset of the gate of recurrence 0: (O-1) D
+  const int* row_start;  // (B) first real position of each left-padded row (decode_hist_rows_kernel), or null
 };
 
 struct DotArgs {

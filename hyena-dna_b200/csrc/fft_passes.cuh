@@ -126,11 +126,26 @@ __device__ __forceinline__ float2 staged_pair(const float* st, int rr, int col) 
   return *reinterpret_cast<const float2*>(st + rr * (2 * C) + 2 * col);
 }
 
+// Left-padded rows (COL_GATE_ROWS / INV_CONV_FWD_ROWS): positions t < rs of the row are padding and read as the short
+// filter's padding before t = 0 (value 0, no in_proj bias).  Applied per element after the window is loaded or staged, so
+// a window straddling rs is masked however it was fetched.
+__device__ __forceinline__ void mask_window(float (&P)[4], int t0, int rs) {
+#pragma unroll
+  for (int j = 0; j < 4; ++j) P[j] = (t0 - 2 + j >= rs) ? P[j] : 0.f;
+}
+__device__ __forceinline__ float2 mask_pair(float2 v, int t0, int rs) {
+  return make_float2(t0 >= rs ? v.x : 0.f, t0 + 1 >= rs ? v.y : 0.f);
+}
+
 // ------------------------------------------------------------------------------------------------
 // argument blocks
 // ------------------------------------------------------------------------------------------------
-enum ColMode { COL_FILTER = 0, COL_GATE = 1, COL_DC = 2, COL_PLAIN = 3 };
-enum InvMode { INV_CONV_FWD = 0, INV_BWD_DG = 1, INV_DK = 2, INV_PLAIN_FWD = 3, INV_PLAIN_BWD = 4 };
+// *_ROWS: the forward modes on left-padded rows; row b's samples t < row_start[b] are padding (g, y_pre and c_save are 0
+// there, and the short filters see zeros).  Their launches count under the kind of the plain mode (col_kind / inv_kind).
+enum ColMode { COL_FILTER = 0, COL_GATE = 1, COL_DC = 2, COL_PLAIN = 3, COL_GATE_ROWS = 4 };
+enum InvMode { INV_CONV_FWD = 0, INV_BWD_DG = 1, INV_DK = 2, INV_PLAIN_FWD = 3, INV_PLAIN_BWD = 4, INV_CONV_FWD_ROWS = 5 };
+__host__ __device__ constexpr int col_kind(int mode) { return mode == COL_GATE_ROWS ? COL_GATE : mode; }
+__host__ __device__ constexpr int inv_kind(int mode) { return mode == INV_CONV_FWD_ROWS ? INV_CONV_FWD : mode; }
 enum RowMode { ROW_FILTER = 0, ROW_CONV_FWD = 1, ROW_CONV_BWD = 2, ROW_CONV_BWD1 = 3 };
 
 // Rows of one launch are numbered r = ci*B + b (all batches of a channel adjacent), channel c = c0 + ci.
@@ -164,6 +179,7 @@ struct PassArgs {
   float* red;            // INV_BWD_DG: dfbias (D); INV_PLAIN_BWD: dD (H)   (atomicAdd)
   float* dsw;            // INV_BWD_DG: d short_filter.weight (3D,3) (atomicAdd)
   float* dsb;            // INV_BWD_DG: d short_filter.bias (3D)     (atomicAdd)
+  const int* row_start;  // COL_GATE_ROWS / INV_CONV_FWD_ROWS: (B) first real position of each batch row
 };
 
 __device__ __forceinline__ size_t row_off(int b, int ch, int nch, int L) { return ((size_t)b * nch + ch) * (size_t)L; }
@@ -204,7 +220,8 @@ struct ColGeo {
   }
   template <int MODE>
   static constexpr size_t smem_inv() {
-    return (MODE == INV_BWD_DG || MODE == INV_CONV_FWD) && stage_inv<MODE>() > EXCH ? stage_inv<MODE>() : EXCH;
+    return (MODE == INV_BWD_DG || MODE == INV_CONV_FWD || MODE == INV_CONV_FWD_ROWS) && stage_inv<MODE>() > EXCH
+               ? stage_inv<MODE>() : EXCH;
   }
   static constexpr size_t SMEM_FWD = EXCH > STAGE_FWD ? EXCH : STAGE_FWD;
   static constexpr size_t SMEM = EXCH;
@@ -217,8 +234,17 @@ struct WarpSync { __device__ __forceinline__ void operator()() const { __syncwar
 // input sample pair (x[t0], x[t0+1]) of row (b, c) for the forward column pass
 template <int MODE>
 __device__ __forceinline__ float2 col_input(const PassArgs& a, int b, int c, int t0, bool vec,
-                                            const Taps& ka, const Taps& kb) {
-  if constexpr (MODE == COL_FILTER) {
+                                            const Taps& ka, const Taps& kb, int rs = 0) {
+  if constexpr (MODE == COL_GATE_ROWS) {         // COL_GATE on a left-padded row starting at rs
+    float P[4];
+    load_window(a.p + row_off(b, a.D + c, 3 * a.D, a.L), t0, a.L, vec, ka.ib, P);
+    mask_window(P, t0, rs);
+    const float2 x1 = conv_window(P, t0, a.L, ka);
+    load_window(a.p + row_off(b, 2 * a.D + c, 3 * a.D, a.L), t0, a.L, vec, kb.ib, P);
+    mask_window(P, t0, rs);
+    const float2 v = conv_window(P, t0, a.L, kb);
+    return mask_pair(make_float2(x1.x * v.x, x1.y * v.y), t0, rs);
+  } else if constexpr (MODE == COL_FILTER) {
     return load_pair(a.src + (size_t)c * a.L, t0, a.L, vec);
   } else if constexpr (MODE == COL_PLAIN) {
     return load_pair(a.src + row_off(b, c, a.D, a.L), t0, a.L, vec);
@@ -256,9 +282,11 @@ __device__ __forceinline__ void col_fwd_body(const PassArgs& a, const int bx, co
   float2* Arow = a.A + (size_t)r * ((size_t)M1 * kM2);
 
   Taps ka{}, kb{};
-  if constexpr (MODE == COL_GATE) {
+  [[maybe_unused]] int rs = 0;
+  if constexpr (MODE == COL_GATE || MODE == COL_GATE_ROWS) {
     ka = load_taps(a.sw, a.sb, a.in_bias, a.D + c);
     kb = load_taps(a.sw, a.sb, a.in_bias, 2 * a.D + c);
+    if constexpr (MODE == COL_GATE_ROWS) rs = __ldg(a.row_start + b);
   } else if constexpr (MODE == COL_DC) {
     ka = load_taps(a.sw, a.sb, a.in_bias, c);
   }
@@ -268,10 +296,10 @@ __device__ __forceinline__ void col_fwd_body(const PassArgs& a, const int bx, co
     const int col = threadIdx.x % CG::C, q = threadIdx.x / CG::C;
     const int m2 = colbase + col;
     // slots n1 >= 16 (m1 >= M1/2) are the zero padding: never loaded
-    if ((MODE == COL_GATE || MODE == COL_DC) && a.stage) {
+    if ((MODE == COL_GATE || MODE == COL_DC || MODE == COL_GATE_ROWS) && a.stage) {
       float* st0 = reinterpret_cast<float*>(smem_raw);
       float* st1 = st0 + CG::DATA_ROWS * CG::WP;
-      if constexpr (MODE == COL_GATE) {
+      if constexpr (MODE == COL_GATE || MODE == COL_GATE_ROWS) {
         stage_windows<CG::C, kM2>(st0, a.p + row_off(b, a.D + c, 3 * a.D, L), 0, CG::DATA_ROWS, colbase, L);
         stage_windows<CG::C, kM2>(st1, a.p + row_off(b, 2 * a.D + c, 3 * a.D, L), 0, CG::DATA_ROWS, colbase, L);
       } else {
@@ -288,11 +316,14 @@ __device__ __forceinline__ void col_fwd_body(const PassArgs& a, const int bx, co
         if (t0 < L) {
           float P[4];
           staged_window<CG::C>(st0, m1, col, t0, ka.ib, P);
+          if constexpr (MODE == COL_GATE_ROWS) mask_window(P, t0, rs);
           const float2 x = conv_window(P, t0, L, ka);
-          if constexpr (MODE == COL_GATE) {
+          if constexpr (MODE == COL_GATE || MODE == COL_GATE_ROWS) {
             staged_window<CG::C>(st1, m1, col, t0, kb.ib, P);
+            if constexpr (MODE == COL_GATE_ROWS) mask_window(P, t0, rs);
             const float2 y = conv_window(P, t0, L, kb);
             g = make_float2(x.x * y.x, x.y * y.y);
+            if constexpr (MODE == COL_GATE_ROWS) g = mask_pair(g, t0, rs);
           } else {
             const float2 dy = staged_pair<CG::C>(st1, m1, col);
             g = make_float2(x.x * dy.x, x.y * dy.y);
@@ -306,7 +337,7 @@ __device__ __forceinline__ void col_fwd_body(const PassArgs& a, const int bx, co
         constexpr int n1 = decltype(n_)::value;
         const int m1 = CG::R2 * n1 + q;
         const int t0 = 2 * (m1 * kM2 + m2);
-        v[n1] = (t0 < L) ? col_input<MODE>(a, b, c, t0, vec, ka, kb) : make_float2(0.f, 0.f);
+        v[n1] = (t0 < L) ? col_input<MODE>(a, b, c, t0, vec, ka, kb, rs) : make_float2(0.f, 0.f);
       });
     }
     static_for<16, 32>([&](auto n_) { v[decltype(n_)::value] = make_float2(0.f, 0.f); });
@@ -333,7 +364,7 @@ __device__ __forceinline__ void col_fwd_body(const PassArgs& a, const int bx, co
       static_for<0, M1>([&](auto m_) {
         constexpr int m1 = decltype(m_)::value;
         const int t0 = 2 * (m1 * kM2 + m2);
-        v[gi * M1 + m1] = (t0 < L) ? col_input<MODE>(a, b, c, t0, vec, ka, kb) : make_float2(0.f, 0.f);
+        v[gi * M1 + m1] = (t0 < L) ? col_input<MODE>(a, b, c, t0, vec, ka, kb, rs) : make_float2(0.f, 0.f);
       });
       dif<M1, gi * M1, false, 32>(v);
       static_for<0, M1>([&](auto k_) {
@@ -364,6 +395,7 @@ struct InvCtx {
   float red;           // per-thread partial of the reduction this mode produces
   float rw[3][3];      // INV_BWD_DG: partials of d short_filter.weight for the x0 / x1 / v channels
   float rb[3];         //             and of d short_filter.bias
+  int rs;              // INV_CONV_FWD_ROWS: first real position of the row
 };
 
 // dw_j += ds[t0] P(t0-2+j) + ds[t0+1] P(t0-1+j);  db += ds[t0] + ds[t0+1]     (P = window of the filter input)
@@ -389,7 +421,7 @@ __device__ __forceinline__ void inv_load(const PassArgs& a, const InvCtx& cx, in
   } else if constexpr (MODE == INV_PLAIN_BWD) {
     in.a = load_pair(a.src2 + row_off(b, c, D, L), t0, L, vec);
     in.b = load_pair(a.src + row_off(b, c, D, L), t0, L, vec);
-  } else if constexpr (MODE == INV_CONV_FWD) {
+  } else if constexpr (MODE == INV_CONV_FWD || MODE == INV_CONV_FWD_ROWS) {
     load_window(a.p + row_off(b, c, 3 * D, L), t0, L, vec, cx.k0.ib, in.P0);     // x0 only: c = y already holds bias * g
   } else if constexpr (MODE == INV_BWD_DG) {
     load_window(a.p + row_off(b, c, 3 * D, L), t0, L, vec, cx.k0.ib, in.P0);
@@ -416,6 +448,13 @@ __device__ __forceinline__ void inv_finish(const PassArgs& a, InvCtx& cx, int b,
     const float2 x0 = conv_window(in.P0, t0, L, cx.k0);
     if (a.out2) store_pair(a.out2 + row_off(b, c, D, L), t0, L, vec, y);
     store_pair(a.out + row_off(b, c, D, L), t0, L, vec, pmul(y, x0));
+  } else if constexpr (MODE == INV_CONV_FWD_ROWS) {   // the same on a left-padded row: c and y_pre are 0 at t < rs
+    float P0[4] = {in.P0[0], in.P0[1], in.P0[2], in.P0[3]};
+    mask_window(P0, t0, cx.rs);
+    const float2 x0 = conv_window(P0, t0, L, cx.k0);
+    const float2 cm = mask_pair(y, t0, cx.rs);
+    if (a.out2) store_pair(a.out2 + row_off(b, c, D, L), t0, L, vec, cm);
+    store_pair(a.out + row_off(b, c, D, L), t0, L, vec, mask_pair(pmul(y, x0), t0, cx.rs));
   } else {                                            // INV_BWD_DG
     const float2 x0 = conv_window(in.P0, t0, L, cx.k0), x1 = conv_window(in.P1, t0, L, cx.k1),
                  vv = conv_window(in.P2, t0, L, cx.k2);
@@ -460,6 +499,10 @@ __device__ __forceinline__ void col_inv_body(const PassArgs& a, const int bx, co
   InvCtx cx{};
   cx.red = 0.f;
   if constexpr (MODE == INV_CONV_FWD || MODE == INV_BWD_DG) cx.k0 = load_taps(a.sw, a.sb, a.in_bias, c);
+  if constexpr (MODE == INV_CONV_FWD_ROWS) {
+    cx.k0 = load_taps(a.sw, a.sb, a.in_bias, c);
+    cx.rs = __ldg(a.row_start + b);
+  }
   if constexpr (MODE == INV_BWD_DG) {
     cx.k1 = load_taps(a.sw, a.sb, a.in_bias, a.D + c);
     cx.k2 = load_taps(a.sw, a.sb, a.in_bias, 2 * a.D + c);
@@ -475,7 +518,7 @@ __device__ __forceinline__ void col_inv_body(const PassArgs& a, const int bx, co
     });
     block_fft<CG::TWO ? LOGM1 : 5, true, false>(v, smem + col * CG::PITCH, q, a.T.tw1024, CtaSync{});
     // only m1 < M1/2 (slots s < 16) can hold samples t < L
-    if ((MODE == INV_CONV_FWD || MODE == INV_BWD_DG) && a.stage) {
+    if ((MODE == INV_CONV_FWD || MODE == INV_BWD_DG || MODE == INV_CONV_FWD_ROWS) && a.stage) {
       // epilogue operands staged through shared memory, SB slots (SB*R2 consecutive rows) per batch; forward:
       // double buffered, the cp.async group of batch k+1 is in flight while batch k is consumed
       constexpr bool DBL = true;

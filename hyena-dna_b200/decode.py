@@ -47,6 +47,27 @@ def _host_index(index, n, what):
     return out
 
 
+def host_lengths(lengths, batch, positions):
+    """lengths (a sequence or 1-D tensor of B integers, each in [1, positions]) -> list of ints, checked on the host before
+    any device work.  Row b of a left-padded batch holds its real tokens at positions [positions - lengths[b], positions)."""
+    if torch.is_tensor(lengths):
+        if lengths.dim() != 1 or lengths.dtype.is_floating_point or lengths.dtype.is_complex or lengths.dtype == torch.bool:
+            raise HyenaB200Error(f"lengths must be a 1-D integer tensor; got {lengths.dtype} of shape {tuple(lengths.shape)}")
+        lengths = lengths.tolist()
+    try:
+        out = [int(n) for n in lengths]
+        if any(isinstance(n, bool) or int(n) != n for n in lengths):
+            raise ValueError
+    except (TypeError, ValueError):
+        raise HyenaB200Error("lengths must be a 1-D sequence of integers") from None
+    if len(out) != batch:
+        raise HyenaB200Error(f"lengths has {len(out)} entries; the batch has {batch} rows")
+    bad = [n for n in out if not 1 <= n <= positions]
+    if bad:
+        raise HyenaB200Error(f"lengths {bad[0]} outside [1, {positions}] (the padded input has {positions} positions)")
+    return out
+
+
 class _PositionState:
     """The values last written to a device position (None: unknown), shared by every cache that holds the tensor."""
 
@@ -85,6 +106,12 @@ class DecodeCache:
     so out_o[t] = F_o[parent][t-b] + sum_{b<=s<t} k_o[t-s] g_o[s] + (k_o[0] + bias_o) g_o[t] for b <= t < b + Hc, and no
     operation on a branch reads the context before b.
 
+    Left-padded prefill (``HyenaOperator.prefill(u, cache, lengths)``, DESIGN.md section 4.14): ``start`` is the tuple of the
+    rows' first real positions s_b = P - lengths[b] (``start_dev`` the same as a (B,) int32 tensor on the device), None for
+    a cache prefilled without lengths.  The history before s_b is zero, exactly the history the unpadded row would have, so
+    every later operation runs unchanged; ``lengths`` = t - start is the number of real positions each row holds.  Row b
+    can hold at most Lcap - s_b real positions.  ``fork`` gives each branch its parent row's start, ``select`` permutes them.
+
     Device position (``sync_position``, StepGraph): ``pos`` (3,) int32 on the device holds [t, win_b, base] for the step
     kernels that read the position on the device.  One tensor serves every layer of a stack.  It is allocated on first
     use and written only by ``sync_position`` and by a replayed StepGraph; ``t`` on the host stays authoritative."""
@@ -99,6 +126,7 @@ class DecodeCache:
         self.win_b, self.win_wc, self.win_f, self.steps = 0, 0, None, 0
         self._branched, self.base, self.hc, self.f, self.parent = False, 0, 0, None, None
         self.pos, self._pos_state = None, None
+        self._start, self.start_dev = None, None
         if owner is not None:
             self.d_model, self.order = owner.d_model, owner.order
 
@@ -152,6 +180,7 @@ class DecodeCache:
             return sum(c.nbytes for c in self.layers)
         own = (self.h, self.f, self.tail, self.s_t, self.part, self.parent) if self.branched else \
               (self.k, self.bias, self.h, self.tail, self.s_t, self.part)
+        own += (self.start_dev,) if self.start_dev is not None else ()
         return sum(x.numel() * x.element_size() for x in own)
 
     @property
@@ -200,6 +229,24 @@ class DecodeCache:
     def reset_window(self):
         """Close the window and restart the step count (a prefill starts a new sequence)."""
         self.win_b, self.win_wc, self.steps = 0, 0, 0
+
+    @property
+    def start(self):
+        """First real position of every row after a left-padded prefill (a tuple), or None; one for all layers of a stack."""
+        return self.layers[0].start if self.layers else self._start
+
+    def set_start(self, start):
+        """Record the rows' first real positions (None: every row starts at 0), on the host and as (B,) int32 on the device."""
+        if self.layers:
+            raise HyenaB200Error("the row starts of a stack's cache are set by its layers")
+        self._start = None if start is None else tuple(int(s) for s in start)
+        self.start_dev = None if start is None else torch.tensor(self._start, dtype=torch.int32, device=self.h.device)
+
+    @property
+    def lengths(self):
+        """Real positions each row holds: t - start (t for every row of a cache prefilled without lengths)."""
+        start = self.start
+        return tuple(self.t - s for s in start) if start is not None else (self.t,) * self.batch_size
 
     @property
     def t(self):

@@ -13,7 +13,7 @@ import torch.nn as nn
 
 from . import ops
 from ._lib import HyenaB200Error
-from .decode import DecodeCache, StepGraph
+from .decode import DecodeCache, StepGraph, host_lengths
 
 
 class OptimModule(nn.Module):
@@ -334,7 +334,11 @@ class HyenaOperator(nn.Module):
         self.filter_fn = HyenaFilter(self.head_dim * inner_factor * (order - 1), order=filter_order, seq_len=l_max,
                                      channels=1, dropout=filter_dropout, **filter_args)
 
-    def forward(self, u, *args, **kwargs):
+    def forward(self, u, *args, lengths=None, **kwargs):
+        """``lengths`` (B integers in [1, L]): u is left-padded, row b's real tokens are its last lengths[b] positions.  Its
+        outputs there do not depend on the padding: they are the outputs of the unpadded row (DESIGN.md section 4.14); at a
+        pad position the output is out_proj(0) = out_proj.bias.  Inference only: with grad required it raises (train on
+        right-padded batches, where a causal operator is exact as it stands)."""
         cache = kwargs.get("inference_params")
         if isinstance(cache, DecodeCache):
             # incremental decoding driven by the caller's model (LMBackbone passes inference_params to every mixer,
@@ -343,7 +347,14 @@ class HyenaOperator(nn.Module):
             # that already holds history extend it
             c = cache.for_module(self)
             n = u.shape[-2]
-            y = self.prefill(u, c) if (c.t == 0 and n > 1) else self.step(u, c) if n == 1 else self.extend(u, c)
+            if lengths is not None:
+                y = self.prefill(u, c, lengths) if c.t == 0 and not c.branched else \
+                    self.step(u, c, lengths) if n == 1 else self.extend(u, c, lengths)
+            else:
+                y = self.prefill(u, c) if (c.t == 0 and n > 1) else self.step(u, c) if n == 1 else self.extend(u, c)
+            return (y, None) if self.return_state else y
+        if lengths is not None:
+            y = self._forward_left_padded(u, lengths)
             return (y, None) if self.return_state else y
         if not u.is_cuda:
             raise HyenaB200Error("HyenaOperator (hyena_b200) runs on CUDA sm_90a only; there is no CPU fallback")
@@ -380,12 +391,77 @@ class HyenaOperator(nn.Module):
             return y, None
         return y
 
-    def _forward_chained(self, u, k, fb, l_filter, capture=None):
+    def _ragged_checks(self, u, lengths):
+        """Host validation of a left-padded input before any device work -> the rows' first real positions."""
+        if self.filter_fn.bidirectional:
+            raise HyenaB200Error("lengths needs a causal filter; this HyenaFilter is bidirectional")
+        if u.dim() != 3 or u.shape[-1] != self.d_model:
+            raise HyenaB200Error(f"left-padded input must be (B, L, {self.d_model}); got {tuple(u.shape)}")
+        B, P = u.shape[0], u.shape[1]
+        if P > self.l_max:
+            raise HyenaB200Error(f"left-padded input of {P} positions exceeds l_max = {self.l_max}")
+        return [P - n for n in host_lengths(lengths, B, P)]
+
+    def check_lengths(self, u, lengths, cache=None, how="forward"):
+        """Every host check of ``how``(u, [cache,] lengths=lengths) -- "forward", "prefill", "extend" or "step" -- without
+        device work (Block and Backbone run it before their first kernel) -> the rows' first real positions."""
+        if how == "step":
+            self._no_ragged(lengths, "step")
+        if how == "forward":
+            if torch.is_grad_enabled() and (u.requires_grad or any(p.requires_grad for p in self.parameters())):
+                raise HyenaB200Error("forward(u, lengths=...) is inference only (run under torch.no_grad()); to train on "
+                                     "sequences of different lengths pad them on the right: the causal operator is exact "
+                                     "there")
+            starts = self._ragged_checks(u, lengths)
+            if not u.is_cuda:
+                raise HyenaB200Error("HyenaOperator (hyena_b200) runs on CUDA sm_90a only; there is no CPU fallback")
+            return starts
+        c = cache.for_module(self) if isinstance(cache, DecodeCache) else cache
+        if how == "extend" and isinstance(c, DecodeCache) and (c.branched or c.t != 0):
+            self._no_ragged(lengths, "extend on a cache that holds history or is branched")
+        starts = self._ragged_checks(u, lengths)
+        self._decode_checks(u, cache, u.shape[1], fresh=True)
+        return starts
+
+    def _forward_left_padded(self, u, lengths):
+        starts = self.check_lengths(u, lengths)
+        with torch.no_grad():
+            row_start = torch.tensor(starts, dtype=torch.int32, device=u.device)
+            y, _, _ = self._run_left_padded(u, row_start)
+        return y
+
+    def _run_left_padded(self, u, row_start):
+        """Masked forward of a left-padded u (B, P, D) with row_start (B,) int32 on the device, under no_grad ->
+        (y, p, g_o of the recurrences o >= 1 (order >= 3)).  Order 2: in_proj GEMM, the masked fused core
+        (hyena_b200_core_fwd_rows), out_proj.  Order >= 3: the chained route with the pads zeroed in torch."""
+        in_dtype, P = u.dtype, u.shape[1]
+        u32 = u.to(torch.float32)
+        k = self.filter_fn.filter_channel_major(P)
+        fb = self.filter_fn.bias if self.filter_fn.use_bias else 0 * self.filter_fn.bias
+        if self.order == 2:
+            p = _InProj.apply(u32, self.in_proj.weight).contiguous()
+            C = self.short_filter.weight.shape[0]
+            ib = self.in_proj.bias.contiguous() if self.in_proj.bias is not None else None
+            y_pre, _, _ = ops.core_forward(p, ib, self.short_filter.weight.reshape(C, -1).contiguous(),
+                                           self.short_filter.bias.contiguous(), ops.filter_spectrum(k),
+                                           fb.reshape(-1).to(torch.float32).contiguous(), False, row_start)
+            gs = []
+        else:
+            keep = torch.arange(P, device=u.device)[None, None, :] >= row_start.to(torch.long)[:, None, None]
+            cap = {}
+            y_pre = self._forward_chained(u32, k, fb, P, capture=cap, keep=keep)
+            p, gs = cap["p"], cap["g"]
+        y = _OutProj.apply(y_pre, self.out_proj.weight, self.out_proj.bias).to(in_dtype)
+        return y, p, gs
+
+    def _forward_chained(self, u, k, fb, l_filter, capture=None, keep=None):
         """order >= 3 (the shipped HyenaDNA layer default is 3, configs/model/layer/hyena_dna.yaml:3): the recurrence of
         hyena.py:414-423 as a chain of this library's long convolutions.  Projections and every FFT convolution
         (forward and backward) run on the sm_90a kernels; the gates and the 3-tap short filter between them are
         plain elementwise / depthwise torch ops here -- the fully fused pass exists for order 2 only.
-        ``capture`` (a dict) receives the in_proj output "p" and the gated input "g" of every recurrence (prefill)."""
+        ``capture`` (a dict) receives the in_proj output "p" and the gated input "g" of every recurrence (prefill).
+        ``keep`` ((B, 1, L) bool): left-padded rows; the short filter's input, every g and the output are zeroed where it is
+        False (the masking of hyena_b200_core_fwd_rows)."""
         D, O1 = self.d_model, self.order - 1
         from .fftconv import fftconv_func
         p = _InProj.apply(u, self.in_proj.weight)                                   # (B, (order+1) D, l)
@@ -394,6 +470,8 @@ class HyenaOperator(nn.Module):
         if l_filter < p.shape[-1]:
             p = p[..., :l_filter]
         p = p + self.in_proj.bias[None, :, None]
+        if keep is not None:
+            p = torch.where(keep, p, 0.0)
         uc = torch.nn.functional.conv1d(p, self.short_filter.weight, self.short_filter.bias,
                                         padding=self.short_filter_order - 1, groups=p.shape[1])[..., :l_filter]
         *x, v = uc.split(D, dim=1)
@@ -402,6 +480,8 @@ class HyenaOperator(nn.Module):
         bidir = self.filter_fn.bidirectional
         for o, x_i in enumerate(reversed(x[1:])):
             g = (v * x_i).contiguous()
+            if keep is not None:
+                g = torch.where(keep, g, 0.0).contiguous()
             if capture is not None:
                 capture["g"].append(g)
             if bidir:
@@ -409,6 +489,8 @@ class HyenaOperator(nn.Module):
                 v = fftconv_ref(g, kk[:, o].contiguous(), bb[:, o].contiguous(), None, gelu=False, bidirectional=True)
             else:
                 v = fftconv_func(g, kk[:, o].contiguous(), bb[:, o].contiguous(), gelu=False)
+        if keep is not None:
+            return torch.where(keep, v * x[0], 0.0).contiguous()
         return (v * x[0]).contiguous()
 
     # ------------------------------------------------------------------------------ incremental decoding
@@ -447,9 +529,17 @@ class HyenaOperator(nn.Module):
         return (self.in_proj.bias.detach().contiguous() if self.in_proj.bias is not None else None,
                 self.short_filter.weight.detach().reshape(C, -1).contiguous(), self.short_filter.bias.detach().contiguous())
 
-    def prefill(self, u, cache):
+    def prefill(self, u, cache, lengths=None):
         """Run the first P positions, u (B, P, D), and fill ``cache`` (which must be fresh) for stepping.  The output is
-        the one ``forward(u)`` gives, bit for bit: the same kernels run in the same order."""
+        the one ``forward(u)`` gives, bit for bit: the same kernels run in the same order.
+
+        ``lengths`` (B integers in [1, P]): prompts of different lengths, left-padded to P; row b's real tokens are its
+        positions [P - lengths[b], P).  Pad positions enter neither the outputs nor the cache: the output at a real position
+        and everything decoded after the prefill are those of the unpadded row; the output at a pad position is
+        out_proj(0) = out_proj.bias.  Every row ends at position P, so the rows step together; row b can hold at most
+        Lcap - (P - lengths[b]) real positions.  ``forward(u, lengths=...)`` gives the same outputs, bit for bit."""
+        if lengths is not None:
+            return self._prefill_left_padded(u, cache, lengths)
         c = self._decode_checks(u, cache, u.shape[1] if u.dim() == 3 else -1, fresh=True)
         with torch.no_grad():
             in_dtype = u.dtype
@@ -479,13 +569,35 @@ class HyenaOperator(nn.Module):
             c.reset_window()
         return y
 
-    def step(self, u_t, cache):
+    def _prefill_left_padded(self, u, cache, lengths):
+        starts = self.check_lengths(u, lengths, cache, "prefill")
+        c = cache.for_module(self)
+        with torch.no_grad():
+            c.set_start(starts)
+            y, p, gs = self._run_left_padded(u, c.start_dev)
+            ib, sw, sb = self._decode_params()
+            ops.decode_hist(p.contiguous(), ib, sw, sb, c, row_start=c.start_dev)
+            P = u.shape[1]
+            for o in range(1, self.order - 1):
+                c.h[o, :, :, :P].copy_(gs[o])
+            c.t = P
+            c.reset_window()
+        return y
+
+    @staticmethod
+    def _no_ragged(lengths, what):
+        if lengths is not None:
+            raise HyenaB200Error(f"{what} takes no lengths: left-padded prompts are prefilled together on a fresh cache, and "
+                                 "rows then advance together (ragged appends would need per-row positions)")
+
+    def step(self, u_t, cache, lengths=None):
         """One position: u_t (B, 1, D) -> y (B, 1, D), the output at position ``cache.t``; advances the cache.  Stepping a
         fresh cache starts the sequence (empty history).  The in_proj / out_proj products of one position are fp32
         matrix-vector products (F.linear); the operator itself runs in csrc/decode.cuh, two launches per recurrence.  After
         a run of steps at a long history the step reads only the positions of a window opened by one FFT refresh
         (ops.decode_window_plan chooses).  On a branched cache (DecodeCache.fork) the step reads each branch's positions since
         the fork base only (ops.decode_branch_step)."""
+        self._no_ragged(lengths, "step")
         c = self._decode_checks(u_t, cache, 1)
         y = self._step_with(u_t, c, ops.decode_branch_step if c.branched else ops.decode_step_auto)
         c.t += 1
@@ -508,16 +620,20 @@ class HyenaOperator(nn.Module):
         """A decode.StepGraph: ``step`` on ``cache`` captured in CUDA graphs and replayed one position at a time."""
         return StepGraph(self, cache, batch_size, dtype)
 
-    def extend(self, u, cache):
+    def extend(self, u, cache, lengths=None):
         """n >= 1 more positions at once: u (B, n, D) -> y (B, n, D), the outputs at positions [cache.t, cache.t + n);
         advances the cache by n.  On a fresh cache this is ``prefill`` (bit-identical to ``forward``).  Otherwise in_proj and
         out_proj of the chunk run on the wgmma projection GEMM and every recurrence on csrc/decode_extend.cuh: the direct
         Toeplitz kernel over the cached history, or for large n the FFT convolution of the whole history
         (ops.decode_extend_uses_fft chooses from t and n).  On a branched cache the same routes run over each branch's
-        positions since the fork base only (ops.decode_branch_extend)."""
+        positions since the fork base only (ops.decode_branch_extend).  ``lengths`` is accepted on a fresh cache only,
+        where this is ``prefill(u, cache, lengths)``."""
         n = u.shape[1] if u.dim() == 3 else -1
         if n < 1:
             raise HyenaB200Error(f"extend input must be (B, n, {self.d_model}) with n >= 1; got {tuple(u.shape)}")
+        if lengths is not None:
+            self.check_lengths(u, lengths, cache, "extend")
+            return self.prefill(u, cache, lengths)
         c = self._decode_checks(u, cache, n)
         if c.branched:
             return self._extend(u, c, ops.decode_branch_extend)

@@ -268,7 +268,9 @@ def _save_spectrum():
     return os.environ.get("HYENA_B200_SAVE_SPECTRUM", "1") != "0"
 
 
-def core_forward(p, in_bias, sw, sb, kspec, fbias, save_c):
+def core_forward(p, in_bias, sw, sb, kspec, fbias, save_c, row_start=None):
+    """y_pre (B, D, L) of the fused order-2 core, and c / the g spectrum when save_c.  row_start ((B,) int32 on p's device):
+    row b is left-padded, its positions t < row_start[b] are padding (hyena_b200_core_fwd_rows)."""
     _need_cuda(p, in_bias, sw, sb, fbias)
     B, C3, L = p.shape
     D = C3 // 3
@@ -282,11 +284,19 @@ def core_forward(p, in_bias, sw, sb, kspec, fbias, save_c):
     # spectrum of the gated input, rows ordered (c, b): saves a column pass + a row FFT per row in backward
     gs = (torch.empty(D * B, kspec.shape[-1], dtype=torch.complex64, device=p.device)
           if (save_c and _save_spectrum()) else None)
+    if row_start is not None and (row_start.dtype != torch.int32 or row_start.device != p.device
+                                  or tuple(row_start.shape) != (B,) or not row_start.is_contiguous()):
+        raise _lib.HyenaB200Error(f"core_forward: row_start must be a contiguous ({B},) int32 tensor on {p.device}")
     ws = workspace(B, D, L, False, p.device)
     with torch.cuda.device(p.device):
-        _lib.check(_lib.lib().hyena_b200_core_fwd(
-            _ptr(p), _ptr(in_bias), _ptr(sw), _ptr(sb), _ptr(kspec), _ptr(fbias), _ptr(y), _ptr(c), _ptr(gs),
-            B, D, L, _ptr(ws), ws.numel(), _stream()))
+        if row_start is None:
+            _lib.check(_lib.lib().hyena_b200_core_fwd(
+                _ptr(p), _ptr(in_bias), _ptr(sw), _ptr(sb), _ptr(kspec), _ptr(fbias), _ptr(y), _ptr(c), _ptr(gs),
+                B, D, L, _ptr(ws), ws.numel(), _stream()))
+        else:
+            _lib.check(_lib.lib().hyena_b200_core_fwd_rows(
+                _ptr(p), _ptr(in_bias), _ptr(sw), _ptr(sb), _ptr(kspec), _ptr(fbias), _ptr(y), _ptr(c), _ptr(gs),
+                _ptr(row_start), B, D, L, _ptr(ws), ws.numel(), _stream()))
     return y, c, gs
 
 
@@ -723,17 +733,26 @@ def add_layer_norm(x, res, weight, bias, eps):
 
 
 # ------------------------------------------------------------------------------------------ incremental decoding
-def decode_hist(p, in_bias, sw, sb, cache):
+def decode_hist(p, in_bias, sw, sb, cache, row_start=None):
     """After a prefill of P positions: g_0 = short(v) * short(x_{O-1}) of positions [0, P) into cache.h[0] and the last two
-    in_proj outputs (with bias) into cache.tail (csrc/decode.cuh).  p (B, (O+1) D, P) without in_proj.bias."""
+    in_proj outputs (with bias) into cache.tail (csrc/decode.cuh).  p (B, (O+1) D, P) without in_proj.bias.  row_start
+    ((B,) int32 on the device): left-padded rows, positions t < row_start[b] are padding (hyena_b200_decode_hist_rows)."""
     _need_cuda(p, in_bias, sw, sb)
     B, C, P = p.shape
     if not p.is_contiguous() or C != (cache.order + 1) * cache.d_model:
         raise _lib.HyenaB200Error(f"decode_hist: p must be contiguous (B, {(cache.order + 1) * cache.d_model}, P)")
+    if row_start is not None and (row_start.dtype != torch.int32 or row_start.device != p.device
+                                  or tuple(row_start.shape) != (B,) or not row_start.is_contiguous()):
+        raise _lib.HyenaB200Error(f"decode_hist: row_start must be a contiguous ({B},) int32 tensor on {p.device}")
     with torch.cuda.device(p.device):
-        _lib.check(_lib.lib().hyena_b200_decode_hist(
-            _ptr(p), _ptr(in_bias), _ptr(sw), _ptr(sb), _ptr(cache.h), _ptr(cache.tail), B, cache.batch_size,
-            cache.d_model, cache.order, P, cache.lcap, _stream()))
+        if row_start is None:
+            _lib.check(_lib.lib().hyena_b200_decode_hist(
+                _ptr(p), _ptr(in_bias), _ptr(sw), _ptr(sb), _ptr(cache.h), _ptr(cache.tail), B, cache.batch_size,
+                cache.d_model, cache.order, P, cache.lcap, _stream()))
+        else:
+            _lib.check(_lib.lib().hyena_b200_decode_hist_rows(
+                _ptr(p), _ptr(in_bias), _ptr(sw), _ptr(sb), _ptr(cache.h), _ptr(cache.tail), _ptr(row_start), B,
+                cache.batch_size, cache.d_model, cache.order, P, cache.lcap, _stream()))
 
 
 def decode_step(p_t, in_bias, sw, sb, cache):
@@ -983,15 +1002,19 @@ def decode_fork(cache, rows, horizon):
     if t0 > b:
         h[:, :, :, :t0 - b] = cache.h[:, ridx, :, b:t0]
     parent = torch.tensor([slot[r] for r in rows], dtype=torch.int32, device=dev)
-    return _branch_cache(cache, h, cache.tail.index_select(0, ridx), f, parent, b, hc)
+    new = _branch_cache(cache, h, cache.tail.index_select(0, ridx), f, parent, b, hc)
+    new.set_start(None if cache.start is None else [cache.start[r] for r in rows])
+    return new
 
 
 def decode_select(cache, index):
     """The branches ``index`` (host-validated, see DecodeCache.select) of the branched operator cache ``cache``: history,
     tail and parent row copied per row, F shared."""
     idx = torch.tensor(index, dtype=torch.long, device=cache.h.device)
-    return _branch_cache(cache, cache.h.index_select(1, idx), cache.tail.index_select(0, idx), cache.f,
-                         cache.parent.index_select(0, idx), cache.base, cache.hc)
+    new = _branch_cache(cache, cache.h.index_select(1, idx), cache.tail.index_select(0, idx), cache.f,
+                        cache.parent.index_select(0, idx), cache.base, cache.hc)
+    new.set_start(None if cache.start is None else [cache.start[i] for i in index])
+    return new
 
 
 def _branch_args(cache, B, what):

@@ -119,6 +119,18 @@ HY_API int hyena_b200_core_fwd(const float* p, const float* in_bias, const float
                         float* y_pre, float* c_save, float* gspec_save, int B, int D, int L,
                         void* workspace, size_t workspace_bytes, void* stream);
 
+/* core_fwd on left-padded rows (batched prefill of prompts of different lengths): row_start (B) int32 on the device,
+ * row b's real positions are [row_start[b], L).  A position t < row_start[b] reads as the short filters' padding before
+ * t = 0 (value 0, no in_proj bias), so g = 0 there, and y_pre and c_save are 0 there.  By time invariance, y_pre of row b
+ * at row_start[b] + j is the unpadded row's at j, whatever the pad values of p are.  The values are not checked (<= 0 masks
+ * nothing, >= L masks the whole row).  Pointers 4-byte aligned (kspec, gspec_save 8); the same three launches as core_fwd,
+ * counted under col_fwd<gate>, row_pass<conv_fwd> and col_inv<conv_fwd> (and under HYENA_B200_PIPE pipelined the same way);
+ * no allocation, no synchronisation. */
+HY_API int hyena_b200_core_fwd_rows(const float* p, const float* in_bias, const float* sw, const float* sb,
+                                    const float* kspec, const float* fbias, float* y_pre, float* c_save, float* gspec_save,
+                                    const int* row_start, int B, int D, int L, void* workspace, size_t workspace_bytes,
+                                    void* stream);
+
 /* backward of core_fwd (closed form: hyena.py:43-56 FFTConvFuncv2.backward,
  * csrc/fftconv/fftconv_cuda.cu:1157-1179).  dy_pre (B,D,L).  Outputs: dp (B,3D,L), dk (D,L);
  * (+=): dsw (3D,3), dsb (3D), dfbias (D), d_in_bias (3D, may be NULL).
@@ -262,6 +274,12 @@ HY_API int hyena_b200_add_layernorm_bwd(const float* dy, const float* dres, cons
  *                product over the history into part, then a fixed-order reduction and the epilogue; deterministic. */
 HY_API int hyena_b200_decode_hist(const float* p, const float* in_bias, const float* sw, const float* sb, float* h,
                                   float* tail, int B, int cache_B, int D, int order, int P, int Lcap, void* stream);
+/*   decode_hist_rows: decode_hist of a left-padded prefill (see core_fwd_rows): row_start (B) int32 on the device; row b's
+ *                positions t < row_start[b] are padding.  g_0 is 0 there, the short filter sees them as its padding
+ *                before t = 0 (0, no in_proj bias), and a pad position in the tail is 0.  One launch (kind decode_hist). */
+HY_API int hyena_b200_decode_hist_rows(const float* p, const float* in_bias, const float* sw, const float* sb, float* h,
+                                       float* tail, const int* row_start, int B, int cache_B, int D, int order, int P,
+                                       int Lcap, void* stream);
 HY_API int hyena_b200_decode_step(const float* p_t, const float* in_bias, const float* sw, const float* sb, const float* k,
                                   const float* fbias, float* h, float* tail, float* s_t, const float* v_in, float* out,
                                   float* part, int B, int cache_B, int D, int order, int o, int t, int Lcap, void* stream);
