@@ -29,9 +29,10 @@ namespace dec {
 // g[t] = short(v)[t] * short(x_gate)[t] for t < P into h (row stride ld); tail = P(P-2), P(P-1) of every channel.
 // ROWS: row b is left-padded, its positions t < s = row_start[b] read as the short filter's padding before t = 0 (0, no
 // in_proj bias): g is 0 there, and a pad position in the tail is 0.
+// Grid: (B * D rows, up to 64 position CTAs per row); the rows go on x, which has no 65535 limit.
 template <bool ROWS>
 __device__ __forceinline__ void hist_body(const HistArgs& a) {
-  const int row = blockIdx.y;                    // b * D + d
+  const int row = blockIdx.x;                    // b * D + d
   const int b = row / a.D, d = row - b * a.D;
   const int s = ROWS ? __ldg(a.row_start + b) : 0;
   const int cv = a.C - a.D + d, cg = a.gate + d;
@@ -41,7 +42,7 @@ __device__ __forceinline__ void hist_body(const HistArgs& a) {
   const float v0 = __ldg(a.sw + 3 * cv), v1 = __ldg(a.sw + 3 * cv + 1), v2 = __ldg(a.sw + 3 * cv + 2), vb = __ldg(a.sb + cv);
   const float g0 = __ldg(a.sw + 3 * cg), g1 = __ldg(a.sw + 3 * cg + 1), g2 = __ldg(a.sw + 3 * cg + 2), gb = __ldg(a.sb + cg);
   float* h = a.h + (size_t)row * a.ld;
-  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < a.P; t += gridDim.x * blockDim.x) {
+  for (int t = blockIdx.y * blockDim.x + threadIdx.x; t < a.P; t += gridDim.y * blockDim.x) {
     if (ROWS) {
       if (t < s) { h[t] = 0.f; continue; }
       const float vm2 = t - 2 >= s ? pv[t - 2] + ibv : 0.f, vm1 = t - 1 >= s ? pv[t - 1] + ibv : 0.f, vp = pv[t] + ibv;
@@ -55,7 +56,7 @@ __device__ __forceinline__ void hist_body(const HistArgs& a) {
   }
   // tail of channels d, D + d, ..., O D + d (one thread each, first CTA of the row)
   const int nj = a.C / a.D;
-  if (blockIdx.x == 0 && (int)threadIdx.x < nj) {
+  if (blockIdx.y == 0 && (int)threadIdx.x < nj) {
     const int c = threadIdx.x * a.D + d;
     const float* pc = a.p + ((size_t)b * a.C + c) * a.P;
     const float ib = a.in_bias ? __ldg(a.in_bias + c) : 0.f;

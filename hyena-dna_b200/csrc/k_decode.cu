@@ -6,7 +6,7 @@ namespace hy {
 
 cudaError_t launch_decode_hist(const dec::HistArgs& a, cudaStream_t s) {
   const int per_row = (a.P + 255) / 256;
-  dim3 grid(per_row < 64 ? per_row : 64, a.B * a.D);
+  dim3 grid(a.B * a.D, per_row < 64 ? per_row : 64);
   prof_begin(K_DECODE_HIST, s);
   if (a.row_start) dec::decode_hist_rows_kernel<<<grid, 256, 0, s>>>(a);
   else dec::decode_hist_kernel<<<grid, 256, 0, s>>>(a);

@@ -512,6 +512,10 @@ def private_weight_images(device, stream, keep):
             _wimg_cache[key] = shared
 
 
+def _aligned16(t):
+    return t if t is None or t.data_ptr() % 16 == 0 else t.clone()
+
+
 def proj_gemm(act, act_layout, W, w_transposed, out_layout, bias=None, fir=None, out=None, l_range=None, gelu=None,
               gelu_pre=None):
     """OUT[pos][n] = sum_k ACT[pos][k] Wl[n][k] (+ bias) on this library's wgmma kernel (csrc/proj_gemm.cuh, 3xTF32).
@@ -523,6 +527,9 @@ def proj_gemm(act, act_layout, W, w_transposed, out_layout, bias=None, fir=None,
     _need_cuda(act, W, bias, fir, gelu_pre)
     if act.dim() != 3 or W.dim() != 2 or not act.is_contiguous() or not W.is_contiguous():
         raise _lib.HyenaB200Error("proj_gemm: act must be contiguous 3-D, W contiguous 2-D")
+    # the kernel reads act and bias with 16-byte vector and TMA loads; a contiguous view that starts inside a row (u[:, t:]
+    # of a single sequence, at t D not a multiple of 4) is copied to a fresh allocation
+    act, bias = _aligned16(act), _aligned16(bias)
     B = act.shape[0]
     L, K = (act.shape[1], act.shape[2]) if act_layout == 0 else (act.shape[2], act.shape[1])
     N = W.shape[1] if w_transposed else W.shape[0]

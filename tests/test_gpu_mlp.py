@@ -84,7 +84,9 @@ def _compare(tag, ours, r32, r64):
 
 @pytest.mark.parametrize("approximate", ["tanh", "none"])
 @pytest.mark.parametrize("B,L,D,Hd", [(2, 1000, 128, 512), (1, 4096, 256, 1024), (3, 777, 64, 256), (1, 513, 32, 64),
-                                      (2, 1000, 100, 400), (1, 1001, 1024, 4096)])
+                                      (2, 1000, 100, 400), (1, 1001, 1024, 4096),
+                                      # a decoding step / short extend through Block.step / Block.extend
+                                      (5, 1, 100, 400), (3, 7, 3, 12)])
 def test_mlp_matches_torch_fp32_and_fp64(B, L, D, Hd, approximate):
     dev = _dev()
     args = _inputs(B, L, D, Hd, True, seed=B * 7 + L + D + Hd)

@@ -483,7 +483,9 @@ def test_validation_of_spectrum_and_filter_shapes():
                                      (2, 1000, 1, 129), (1, 999, 2, 3), (2, 1001, 3, 1), (1, 1000, 5, 129), (2, 998, 33, 3),
                                      # the fused FIR's K past 2624 (= 3 x 875), TMA and hand-staged
                                      (1, 1000, 2624, 875), (1, 1001, 2624, 875), (1, 1000, 3072, 1024),
-                                     (1, 999, 3072, 1024), (1, 1001, 2688, 896)])
+                                     (1, 999, 3072, 1024), (1, 1001, 2688, 896),
+                                     # the sizes of an extend's in_proj / out_proj: L = n of 1 to 9 positions
+                                     (3, 1, 100, 300), (2, 2, 3, 9), (5, 7, 1020, 3060), (2, 9, 1, 3)])
 def test_proj_gemm_tcgen05_matches_fp64(B, L, K, N):
     """csrc/proj_gemm.cuh (wgmma, 3xTF32, A operand in registers) against float64 matmuls, all four layout
     combinations, bias epilogue (and none, on row-major outputs), ragged shapes, and the fused transposed short filter."""

@@ -8,6 +8,7 @@ import torch
 
 from oracle import hyena_oracle as O
 from tests import parity_util as PU
+from tests.test_gpu_widths import NANS, _poison
 
 pytestmark = pytest.mark.gpu
 
@@ -37,13 +38,18 @@ def _make(D, l_max, order=2, seed=0):
     return op.to(_dev()), P
 
 
-def _padded(B, P, D, lengths, seed=0, pad_seed=None):
-    """u (B, P, D) on the CPU: row b's real tokens at [P - lengths[b], P), random pads (pad_seed) before them."""
+def _padded(B, P, D, lengths, seed=0, pad_seed=None, fill=None):
+    """u (B, P, D) on the CPU: row b's real tokens at [P - lengths[b], P), random pads (pad_seed) before them, or pads
+    filled with ``fill``: one of the NaN encodings of tests/test_gpu_widths.NANS or "inf" (random signs)."""
     u = O.nucleotide_activations(B, P, D, seed=2222 + seed)[0]
     g = torch.Generator().manual_seed(1000 + (seed if pad_seed is None else pad_seed))
     for b, n in enumerate(lengths):
-        u[b, :P - n] = 3.0 * torch.randn(P - n, D, generator=g)
+        u[b, :P - n] = 3.0 * torch.randn(P - n, D, generator=g) if fill is None else _poison(u[b, :P - n], fill, g)
     return u
+
+
+# non-finite pad fills: the outputs at real positions and the cache must not see them
+PAD_FILLS = [*NANS, "inf"]
 
 
 def _row_truth(u_row, P):
@@ -83,6 +89,15 @@ def test_operator_pad_independence_bitwise(order):
     assert ca.start == tuple(P - n for n in lengths) and ca.lengths == tuple(lengths)
     for b, n in enumerate(lengths):
         assert not ca.h[:, b, :, :P - n].any()
+    # NaN and +-inf pads: the same bits at the real positions and in the cache
+    for fill in PAD_FILLS:
+        u = _padded(B, P, D, lengths, fill=fill).to(dev)
+        c = op.allocate_decode_cache(B, 2048)
+        with torch.no_grad():
+            y = op.prefill(u, c, lengths=lengths)
+        for b, n in enumerate(lengths):
+            assert torch.equal(y[b, P - n:], ya[b, P - n:]), f"{fill} pads: row {b}"
+        assert torch.equal(c.h, ca.h) and torch.equal(c.tail, ca.tail), f"{fill} pads: cache"
 
 
 def test_block_and_backbone_pad_independence_bitwise():
@@ -97,8 +112,9 @@ def test_block_and_backbone_pad_independence_bitwise():
     bb = H.Backbone(D, 3, partial(H.HyenaOperator, l_max=2048, emb_dim=5, w=10.0),
                     mlp_cls=partial(H.Mlp, hidden_features=4 * D), residual_in_fp32=True).to(dev)
     res = {}
-    for pad_seed in (1, 2):
-        u = _padded(B, P, D, lengths, pad_seed=pad_seed).to(dev)
+    for pad_seed in (1, 2, *PAD_FILLS):   # random pads, then NaN and +-inf pads
+        fill = pad_seed if pad_seed in PAD_FILLS else None
+        u = _padded(B, P, D, lengths, pad_seed=None if fill else pad_seed, fill=fill).to(dev)
         cb, cs = block.mixer.allocate_decode_cache(B, 2048), bb.allocate_decode_cache(B, 2048)
         with torch.no_grad():
             hb, rb = block.prefill(u, None, cb, lengths=lengths)
@@ -106,14 +122,16 @@ def test_block_and_backbone_pad_independence_bitwise():
             ys = bb.prefill(u, cs, lengths=lengths)
             yf = bb(u, lengths=lengths)
         res[pad_seed] = (hb, rb, hf, rf, cb, ys, yf, cs)
-    a, b = res[1], res[2]
-    for i, n in enumerate(lengths):
-        s = P - n
-        for j in (0, 1, 2, 3, 5, 6):
-            assert torch.equal(a[j][i, s:], b[j][i, s:]), f"output {j} row {i}"
+    a = res[1]
+    for key in (2, *PAD_FILLS):           # real positions only: with NaN pads the pad outputs of a block may be NaN
+        b = res[key]
+        for i, n in enumerate(lengths):
+            s = P - n
+            for j in (0, 1, 2, 3, 5, 6):
+                assert torch.equal(a[j][i, s:], b[j][i, s:]), f"pads {key}: output {j} row {i}"
+        for ca, cb_ in ((a[4], b[4]),) + tuple(zip(a[7].layers, b[7].layers)):
+            assert torch.equal(ca.h, cb_.h) and torch.equal(ca.tail, cb_.tail), f"pads {key}: cache"
     assert torch.equal(a[0], a[2]) and torch.equal(a[5], a[6])          # forward(lengths) == prefill(lengths)
-    for ca, cb_ in ((a[4], b[4]),) + tuple(zip(a[7].layers, b[7].layers)):
-        assert torch.equal(ca.h, cb_.h) and torch.equal(ca.tail, cb_.tail)
     assert a[7].start == tuple(P - n for n in lengths) and a[7].lengths == tuple(lengths)
 
 
