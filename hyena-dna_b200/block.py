@@ -93,6 +93,14 @@ class Block(nn.Module):
             return self._decode(hidden_states, residual, lambda y: self.mixer.extend(y, cache, lengths))
         return self._decode(hidden_states, residual, lambda y: self.mixer.extend(y, cache))
 
+    def admit(self, hidden_states, residual, cache, rows, lengths=None):
+        """forward of k prompts (k, P, D) that join the running cache in the rows ``rows`` (HyenaOperator.admit); the
+        outputs are those of ``prefill`` on a fresh k-row cache."""
+        if not hasattr(self.mixer, "admit"):
+            raise HyenaB200Error(f"Block: the mixer {type(self.mixer).__name__} has no incremental decoding")
+        self.mixer.check_admit(hidden_states, cache, rows, lengths)
+        return self._decode(hidden_states, residual, lambda y: self.mixer.admit(y, cache, rows, lengths))
+
     def capture_step(self, cache, batch_size=None, dtype=torch.float32, residual=False):
         """A decode.StepGraph of ``step`` on the mixer's cache; ``residual`` says whether steps pass a residual (False for
         a first block)."""
@@ -159,6 +167,23 @@ class Backbone(nn.Module):
     def extend(self, hidden_states, cache, lengths=None):
         """The outputs of n more positions (B, n, D); on a fresh cache this is prefill (``lengths`` there only)."""
         return self._decode(hidden_states, cache, "extend", lengths)
+
+    def admit(self, hidden_states, cache, rows, lengths=None):
+        """k prompts (k, P, D) join the running ``cache`` in the rows ``rows`` (HyenaOperator.admit): the outputs of
+        ``prefill`` on a fresh k-row cache.  Every layer is checked, and shifted when P > t, before the first layer admits."""
+        if hidden_states.requires_grad:
+            raise HyenaB200Error("decoding is inference only: the input requires grad (run under torch.no_grad())")
+        for layer in self.layers:
+            if not hasattr(layer.mixer, "admit"):
+                raise HyenaB200Error(f"Block: the mixer {type(layer.mixer).__name__} has no incremental decoding")
+            layer.mixer.check_admit(hidden_states, cache, rows, lengths)
+        with torch.no_grad():
+            cache._admit_clock(hidden_states.shape[1])
+            residual = None
+            for layer in self.layers:
+                hidden_states, residual = layer.admit(hidden_states, residual, cache, rows, lengths)
+            y, _ = Block._add_norm(hidden_states, residual, self.ln_f)
+            return y.to(hidden_states.dtype)
 
     def capture_step(self, cache, batch_size=None, dtype=torch.float32):
         """A decode.StepGraph of ``step`` on ``cache``: every layer and ln_f in one CUDA graph per route."""

@@ -843,6 +843,37 @@ HY_API int hyena_b200_decode_hist_rows(const float* p, const float* in_bias, con
   return 0;
 }
 
+HY_API int hyena_b200_decode_admit(const float* p, const float* in_bias, const float* sw, const float* sb, float* h,
+                                   float* tail, const int* rows, const int* row_start, int k, int cache_B, int D, int order,
+                                   int P, int t, int Lcap, void* stream) {
+  if (check_decode_shape(k, k, D, order, Lcap)) return 1;
+  HY_CHECK(k <= cache_B, "%d prompts for a decode cache of %d rows", k, cache_B);
+  HY_CHECK(p && sw && sb && h && tail && rows, "null pointer");
+  HY_CHECK(aligned4(p) && aligned4(sw) && aligned4(sb) && aligned4(h) && aligned4(tail) && aligned4(rows) &&
+               (!in_bias || aligned4(in_bias)) && (!row_start || aligned4(row_start)),
+           "misaligned pointer: p, in_bias, sw, sb, h, tail, rows and row_start must be 4-byte aligned");
+  HY_CHECK(t >= 0 && t <= Lcap, "position %d outside the decode cache [0, %d]", t, Lcap);
+  HY_CHECK(P >= 1 && P <= t, "a prompt of %d positions cannot end at position %d (it needs 1 <= P <= t)", P, t);
+  dec::AdmitArgs a{{p, in_bias, sw, sb, h, tail, k, D, (order + 1) * D, P, dec::ld_for(Lcap), (order - 1) * D, row_start},
+                   rows, t - P, t};
+  HY_CUDA(launch_decode_admit(a, (cudaStream_t)stream));
+  return 0;
+}
+
+HY_API int hyena_b200_decode_shift(float* h, int B, int D, int order, int t, int shift, int Lcap, void* stream) {
+  if (check_decode_shape(B, B, D, order, Lcap)) return 1;
+  HY_CHECK(h, "null pointer");
+  HY_CHECK(aligned16(h), "h must be 16-byte aligned");
+  HY_CHECK(t >= 0 && t <= Lcap, "position %d outside the decode cache [0, %d]", t, Lcap);
+  HY_CHECK((shift & 3) == 0, "shift %d is not a multiple of 4", shift);
+  HY_CHECK(shift >= -t, "left shift by %d past the start of a history of %d positions", -shift, t);
+  HY_CHECK(shift <= Lcap - t, "right shift by %d moves position %d past the decode cache's %d", shift, t, Lcap);
+  if (shift == 0) return 0;
+  dec::ShiftArgs a{h, dec::ld_for(Lcap), t, shift};
+  HY_CUDA(launch_decode_shift(a, (long long)(order - 1) * B * D, (cudaStream_t)stream));
+  return 0;
+}
+
 HY_API int hyena_b200_decode_step(const float* p_t, const float* in_bias, const float* sw, const float* sb, const float* k,
                                   const float* fbias, float* h, float* tail, float* s_t, const float* v_in, float* out,
                                   float* part, int B, int cache_B, int D, int order, int o, int t, int Lcap, void* stream) {

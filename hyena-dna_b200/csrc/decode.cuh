@@ -4,6 +4,8 @@
 //     out[t] = sum_{s<=t} k[t-s] g[s] + bias g[t],      g = v * x_gate (short-filtered in_proj channels),
 // so a step is one dot product per (b, channel) over the stored history g[0..t) plus O(1) work at position t.
 //   decode_hist_kernel     after a prefill of P positions: g[0..P) of recurrence 0 and the short-filter tail
+//   decode_admit_kernel    the same for prompts placed into chosen rows of a running cache so that they end at its position
+//   decode_shift_kernel    in-place shift of every history row by a multiple of 4 positions (compaction, room for a prompt)
 //   decode_dot_kernel      split over positions: one warp per (1024-position chunk, channel), each k row read once for
 //                          all batch rows of its group; the filter is stored time-reversed so that h and k both stream in
 //                          ascending order (k[t-s] = krev[ld-1-t+s]); the k offset's misalignment R = (ld-1-t) mod 4 is a
@@ -68,6 +70,90 @@ __device__ __forceinline__ void hist_body(const HistArgs& a) {
 
 __global__ void __launch_bounds__(256) decode_hist_kernel(const HistArgs a) { hist_body<false>(a); }
 __global__ void __launch_bounds__(256) decode_hist_rows_kernel(const HistArgs a) { hist_body<true>(a); }
+
+// Admission of prompt i into cache row rows[i] at the placement offset off = t - P (AdmitArgs): the arithmetic of hist_body
+// on the prompt's positions j = tau - off, written at cache positions tau in [off, t), and 0 at tau < off + s (s the prompt's
+// first real position, 0 without row_start) in the same pass, so no separate memset runs.  A row whose history is zero
+// before its first real position decodes like the unpadded prompt (time invariance, DESIGN.md section 4.15).  The tail of
+// all C channels of row rows[i] is the prompt's last two positions, a pad position there 0.
+// Grid: (k * D rows, up to 64 position CTAs per row); the rows go on x, which has no 65535 limit.
+__global__ void __launch_bounds__(256) decode_admit_kernel(const AdmitArgs w) {
+  const HistArgs& a = w.hist;
+  const int row = blockIdx.x;                    // i * D + d
+  const int i = row / a.D, d = row - i * a.D;
+  const int s = a.row_start ? __ldg(a.row_start + i) : 0;
+  const int s0 = w.off + s;                      // first real position in cache positions
+  const int r = __ldg(w.rows + i);
+  const int cv = a.C - a.D + d, cg = a.gate + d;
+  const float* pv = a.p + ((size_t)i * a.C + cv) * a.P;
+  const float* pg = a.p + ((size_t)i * a.C + cg) * a.P;
+  const float ibv = a.in_bias ? __ldg(a.in_bias + cv) : 0.f, ibg = a.in_bias ? __ldg(a.in_bias + cg) : 0.f;
+  const float v0 = __ldg(a.sw + 3 * cv), v1 = __ldg(a.sw + 3 * cv + 1), v2 = __ldg(a.sw + 3 * cv + 2), vb = __ldg(a.sb + cv);
+  const float g0 = __ldg(a.sw + 3 * cg), g1 = __ldg(a.sw + 3 * cg + 1), g2 = __ldg(a.sw + 3 * cg + 2), gb = __ldg(a.sb + cg);
+  float* h = a.h + ((size_t)r * a.D + d) * a.ld;
+  for (int t = blockIdx.y * blockDim.x + threadIdx.x; t < w.t; t += gridDim.y * blockDim.x) {
+    if (t < s0) { h[t] = 0.f; continue; }
+    const int j = t - w.off;
+    const float vm2 = j - 2 >= s ? pv[j - 2] + ibv : 0.f, vm1 = j - 1 >= s ? pv[j - 1] + ibv : 0.f, vp = pv[j] + ibv;
+    const float gm2 = j - 2 >= s ? pg[j - 2] + ibg : 0.f, gm1 = j - 1 >= s ? pg[j - 1] + ibg : 0.f, gp = pg[j] + ibg;
+    h[t] = short3(v0, v1, v2, vb, vm2, vm1, vp) * short3(g0, g1, g2, gb, gm2, gm1, gp);
+  }
+  // tail of channels d, D + d, ..., O D + d (one thread each, first CTA of the row)
+  const int nj = a.C / a.D;
+  if (blockIdx.y == 0 && (int)threadIdx.x < nj) {
+    const int c = threadIdx.x * a.D + d;
+    const float* pc = a.p + ((size_t)i * a.C + c) * a.P;
+    const float ib = a.in_bias ? __ldg(a.in_bias + c) : 0.f;
+    float* tl = a.tail + ((size_t)r * a.C + c) * 2;
+    tl[0] = a.P - 2 >= s ? pc[a.P - 2] + ib : 0.f;
+    tl[1] = pc[a.P - 1] + ib;
+  }
+}
+
+// In-place shift of one history row per CTA (ShiftArgs) over the float4s of [0, round4(t)); shift is a multiple of 4, so
+// whole float4s move.  Left (shift = -m): h[tau] = h[tau + m], tiles in ascending order.  Right (shift = d): h[tau + d] =
+// h[tau], tiles in descending order, then [0, d) zeroed.  Each tile's loads complete (__syncthreads) before its stores, and
+// no later tile reads a word an earlier tile stored (left: later tiles read above every earlier destination; right: below
+// it), so the shift is race-free without a scratch copy.  Plain loads: the row is written in place (no read-only path).
+__global__ void __launch_bounds__(kShiftThreads) decode_shift_kernel(const ShiftArgs a) {
+  float4* h = reinterpret_cast<float4*>(a.h + (size_t)blockIdx.x * a.ld);
+  const int n4 = (a.t + 3) >> 2;
+  constexpr int kTile = kShiftThreads * kShiftVec;
+  float4 v[kShiftVec];
+  if (a.shift < 0) {
+    const int m4 = (-a.shift) >> 2, w4 = n4 - m4;          // destinations [0, w4) <- sources [m4, n4)
+    for (int q0 = 0; q0 < w4; q0 += kTile) {
+#pragma unroll
+      for (int u = 0; u < kShiftVec; ++u) {
+        const int q = q0 + u * kShiftThreads + threadIdx.x;
+        if (q < w4) v[u] = h[q + m4];
+      }
+      __syncthreads();
+#pragma unroll
+      for (int u = 0; u < kShiftVec; ++u) {
+        const int q = q0 + u * kShiftThreads + threadIdx.x;
+        if (q < w4) h[q] = v[u];
+      }
+    }
+  } else {
+    const int d4 = a.shift >> 2;                           // destinations [d4, d4 + n4) <- sources [0, n4)
+    for (int q1 = n4; q1 > 0; q1 -= kTile) {
+#pragma unroll
+      for (int u = 0; u < kShiftVec; ++u) {
+        const int q = q1 - 1 - (u * kShiftThreads + (int)threadIdx.x);
+        if (q >= 0) v[u] = h[q];
+      }
+      __syncthreads();
+#pragma unroll
+      for (int u = 0; u < kShiftVec; ++u) {
+        const int q = q1 - 1 - (u * kShiftThreads + (int)threadIdx.x);
+        if (q >= 0) h[q + d4] = v[u];
+      }
+    }
+    // every load happened before the last tile's barrier, and the stores went to [d4, d4 + n4): [0, d4) is free
+    for (int q = threadIdx.x; q < d4; q += kShiftThreads) h[q] = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+}
 
 // part[b][d][chunk] = sum_{s in chunk, s < t} h[b][d][s] k[t-s]   for the batch rows [z*BG, z*BG + BG)
 template <int BG, int R>

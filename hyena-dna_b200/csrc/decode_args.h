@@ -20,6 +20,8 @@ constexpr int kChunk = 1024;              // positions per partial: one warp, 32
 constexpr int kDotWarps = 8;              // channels per CTA of the dot kernel (one warp each)
 constexpr int kStepWarps = 8;             // (b, channel) pairs per CTA of the combine kernel
 constexpr int kMaxOrder = 31;             // the combine kernel gives one lane to each of the O+1 in_proj channel groups
+constexpr int kShiftThreads = 256;        // threads of the history shift kernel (one CTA per row)
+constexpr int kShiftVec = 4;              // float4s per thread per tile of the shift kernel
 
 inline int ld_for(int Lcap) { return (Lcap + 3) & ~3; }
 inline int chunks_for(int Lcap) { return (Lcap + kChunk - 1) / kChunk; }
@@ -34,6 +36,23 @@ struct HistArgs {
   int B, D, C, P, ld;
   int gate;              // channel offset of the gate of recurrence 0: (O-1) D
   const int* row_start;  // (B) first real position of each left-padded row (decode_hist_rows_kernel), or null
+};
+
+// Admission of k prompts of P positions into rows of a running cache at position t >= P (decode_admit_kernel): prompt i
+// goes to cache row rows[i] at the placement offset off = t - P, so that it ends at t.  hist.B = k and hist.p is (k, C, P);
+// hist.h and hist.tail address the whole cache (cache_B rows); hist.row_start (k) is the ragged prompts' first real
+// positions within the prompt, or null.
+struct AdmitArgs {
+  HistArgs hist;
+  const int* rows;       // (k) destination cache row of each prompt
+  int off, t;
+};
+
+// In-place shift of every history row (rows of ld floats) by `shift` positions (a multiple of 4; < 0 left, > 0 right) over
+// the positions [0, round4(t)) (decode_shift_kernel)
+struct ShiftArgs {
+  float* h;              // (rows, ld)
+  int ld, t, shift;
 };
 
 struct DotArgs {

@@ -14,6 +14,23 @@ cudaError_t launch_decode_hist(const dec::HistArgs& a, cudaStream_t s) {
   return cudaGetLastError();
 }
 
+// the history fill of admitted prompts: counted and timed as decode_hist (the kind list callers enumerate stays as it is)
+cudaError_t launch_decode_admit(const dec::AdmitArgs& a, cudaStream_t s) {
+  const int per_row = (a.t + 255) / 256;
+  dim3 grid(a.hist.B * a.hist.D, per_row < 64 ? per_row : 64);
+  prof_begin(K_DECODE_HIST, s);
+  dec::decode_admit_kernel<<<grid, 256, 0, s>>>(a);
+  prof_end(K_DECODE_HIST, s);
+  return cudaGetLastError();
+}
+
+// counted by launch_count under no kind, as the position advance: it belongs to no existing kernel class
+cudaError_t launch_decode_shift(const dec::ShiftArgs& a, long long rows, cudaStream_t s) {
+  dec::decode_shift_kernel<<<(unsigned)rows, dec::kShiftThreads, 0, s>>>(a);
+  count_launch();
+  return cudaGetLastError();
+}
+
 template <int BG>
 static cudaError_t dot_bg(const dec::DotArgs& a, int R, dim3 grid, cudaStream_t s) {
   const int threads = 32 * dec::kDotWarps;

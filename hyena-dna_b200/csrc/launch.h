@@ -61,6 +61,8 @@ cudaError_t launch_add_ln_fwd(const ln::FwdArgs& a, cudaStream_t s);
 cudaError_t launch_add_ln_bwd(ln::BwdArgs a, float* dw, float* db, cudaStream_t s);
 // k_decode.cu: incremental decoding (decode.cuh)
 cudaError_t launch_decode_hist(const dec::HistArgs& a, cudaStream_t s);
+cudaError_t launch_decode_admit(const dec::AdmitArgs& a, cudaStream_t s);
+cudaError_t launch_decode_shift(const dec::ShiftArgs& a, long long rows, cudaStream_t s);
 cudaError_t launch_decode_step(const dec::DotArgs& dot, const dec::StepArgs& st, cudaStream_t s);
 cudaError_t launch_decode_win_step(const dec::DotArgs& dot, const dec::WinStepArgs& w, cudaStream_t s);
 cudaError_t launch_decode_branch_step(const dec::DotArgs& dot, const dec::BranchStepArgs& w, cudaStream_t s);

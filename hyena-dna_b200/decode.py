@@ -112,6 +112,11 @@ class DecodeCache:
     every later operation runs unchanged; ``lengths`` = t - start is the number of real positions each row holds.  Row b
     can hold at most Lcap - s_b real positions.  ``fork`` gives each branch its parent row's start, ``select`` permutes them.
 
+    Continuous batching (``HyenaOperator.admit``, ``release``, ``compact``; DESIGN.md section 4.15): the rows keep the one
+    position t.  A prompt joins a row by being placed so that it ends at t with a zero history before it; ``release`` frees
+    a row (``free``, host only) and ``compact`` shifts the history left so that t drops by the smallest live start.  Once a
+    cache has been admitted into, ``start`` is defined for every row.
+
     Device position (``sync_position``, StepGraph): ``pos`` (3,) int32 on the device holds [t, win_b, base] for the step
     kernels that read the position on the device.  One tensor serves every layer of a stack.  It is allocated on first
     use and written only by ``sync_position`` and by a replayed StepGraph; ``t`` on the host stays authoritative."""
@@ -127,6 +132,7 @@ class DecodeCache:
         self._branched, self.base, self.hc, self.f, self.parent = False, 0, 0, None, None
         self.pos, self._pos_state = None, None
         self._start, self.start_dev = None, None
+        self._free = frozenset()
         if owner is not None:
             self.d_model, self.order = owner.d_model, owner.order
 
@@ -244,9 +250,70 @@ class DecodeCache:
 
     @property
     def lengths(self):
-        """Real positions each row holds: t - start (t for every row of a cache prefilled without lengths)."""
-        start = self.start
-        return tuple(self.t - s for s in start) if start is not None else (self.t,) * self.batch_size
+        """Real positions each row holds: t - start (t for every row of a cache prefilled without lengths), 0 for a row
+        released by ``release``."""
+        start, free = self.start, self.free
+        return tuple(0 if b in free else self.t - (start[b] if start is not None else 0) for b in range(self.batch_size))
+
+    # ------------------------------------------------------------------------ continuous batching (DESIGN.md section 4.15)
+    @property
+    def free(self):
+        """The rows released since they last took a prompt (a frozenset); one set for all layers of a stack."""
+        return self.layers[0].free if self.layers else self._free
+
+    def _no_branch(self, what):
+        if self.branched:
+            raise HyenaB200Error(f"{what}: this cache is branched; admission, release and compaction need a full cache")
+
+    def release(self, rows):
+        """Mark ``rows`` free (host only, no device work): they no longer pin compaction, their ``lengths`` read 0, and
+        they go on being stepped with the others until ``HyenaOperator.admit`` gives them a new prompt."""
+        self._no_branch("release")
+        rows = _host_index(rows, self.batch_size, "release: rows")
+        for c in (self.layers or [self]):
+            c._free = c._free | frozenset(rows)
+
+    def compact(self):
+        """Shift the history of every layer left by m, the smallest first real position of a live row rounded down to a
+        multiple of 4 (ops.decode_compact_plan), so that t drops by m and every row gains m positions of room; returns m.
+        The window is kept when it still holds the position, else closed (the next step refreshes by the usual rule)."""
+        self._no_branch("compact")
+        from . import ops
+        start = self.start if self.start is not None else (0,) * self.batch_size
+        shift, _, keep = ops.decode_compact_plan(self.t, start, self.free, *self._window())
+        for c in (self.layers or [self]):
+            c._reposition(shift, keep)
+        return -shift
+
+    def _window(self):
+        c = self.layers[0] if self.layers else self
+        return c.win_b, c.win_wc
+
+    def _admit_clock(self, P):
+        """Make room for prompts of P positions that end at the position (ops.decode_admit_plan), in every layer: at t = 0
+        the position moves to P and every row is free until it takes a prompt; when P > t the history shifts right first."""
+        from . import ops
+        t0 = self.t
+        shift, t_new, keep = ops.decode_admit_plan(t0, self.lcap, P, *self._window())
+        for c in (self.layers or [self]):
+            c._reposition(shift, keep)
+            if t0 == 0:
+                c._t, c._free = t_new, frozenset(range(c.batch_size))
+                c.set_start((t_new,) * c.batch_size)
+
+    def _reposition(self, shift, keep):
+        from . import ops
+        ops.decode_shift(self, shift)
+        if not keep:
+            self.win_b, self.win_wc = 0, 0
+
+    def _took(self, rows, starts):
+        """Rows ``rows`` of this operator cache took prompts whose first real positions are ``starts``."""
+        start = list(self.start) if self.start is not None else [0] * self.batch_size
+        for r, s in zip(rows, starts):
+            start[r] = s
+        self.set_start(start)
+        self._free = self._free - frozenset(rows)
 
     @property
     def t(self):
@@ -301,7 +368,8 @@ class StepGraph:
     and none holds it, the window is refreshed eagerly, outside the graph, on the current stream: the first step at
     t >= WINDOW_MIN_T opens one, with no run of plain steps before it.  After each replay the host advances ``t`` of every
     layer cache (and the step count of an unbranched one), so eager ``step``, ``extend``, ``fork`` and ``select`` go on
-    from there; steps taken eagerly in between are picked up at the next replay.
+    from there; steps taken eagerly in between are picked up at the next replay.  ``admit``, ``release`` and ``compact``
+    between replays write every captured buffer in place and need no recapture; a window they close is reopened at once.
 
     ``step`` returns static output tensors that the next ``step`` of this object overwrites: copy what you keep.  It
     raises before any device work on an input of another shape, dtype or device than the captured one, at Lcap or a

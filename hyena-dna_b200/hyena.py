@@ -13,7 +13,7 @@ import torch.nn as nn
 
 from . import ops
 from ._lib import HyenaB200Error
-from .decode import DecodeCache, StepGraph, host_lengths
+from .decode import DecodeCache, StepGraph, _host_index, host_lengths
 
 
 class OptimModule(nn.Module):
@@ -542,31 +542,89 @@ class HyenaOperator(nn.Module):
             return self._prefill_left_padded(u, cache, lengths)
         c = self._decode_checks(u, cache, u.shape[1] if u.dim() == 3 else -1, fresh=True)
         with torch.no_grad():
-            in_dtype = u.dtype
-            u32 = u.to(torch.float32)
-            P = u32.shape[1]
-            if self.order == 2:
-                y = self.forward(u)
-                y = y[0] if isinstance(y, tuple) else y
-                # the in_proj output the forward consumed (the projections are deterministic: same bits)
-                if ops.proj_mode() == "tc":
-                    p = ops.proj_gemm(u32.contiguous(), 0, self.in_proj.weight.contiguous(), False, 0)
-                else:
-                    p = _InProj.apply(u32, self.in_proj.weight)
-                gs = []
-            else:                               # forward's order >= 3 route, keeping its intermediates
-                k = self.filter_fn.filter_channel_major(P)
-                fb = self.filter_fn.bias if self.filter_fn.use_bias else 0 * self.filter_fn.bias
-                cap = {}
-                y_pre = self._forward_chained(u32, k, fb, P, capture=cap)
-                y = _OutProj.apply(y_pre, self.out_proj.weight, self.out_proj.bias).to(in_dtype)
-                p, gs = cap["p"], cap["g"]
+            P = u.shape[1]
+            y, p, gs = self._prefill_run(u)
             ib, sw, sb = self._decode_params()
             ops.decode_hist(p.contiguous(), ib, sw, sb, c)
             for o in range(1, self.order - 1):
                 c.h[o, :, :, :P].copy_(gs[o])
             c.t = P
             c.reset_window()
+        return y
+
+    def _prefill_run(self, u):
+        """The forward of an unpadded u (B, P, D) as prefill runs it, under no_grad -> (y, the in_proj output p without its
+        bias, g_o of the recurrences o >= 1 (order >= 3))."""
+        in_dtype = u.dtype
+        u32 = u.to(torch.float32)
+        P = u32.shape[1]
+        if self.order == 2:
+            y = self.forward(u)
+            y = y[0] if isinstance(y, tuple) else y
+            # the in_proj output the forward consumed (the projections are deterministic: same bits)
+            if ops.proj_mode() == "tc":
+                p = ops.proj_gemm(u32.contiguous(), 0, self.in_proj.weight.contiguous(), False, 0)
+            else:
+                p = _InProj.apply(u32, self.in_proj.weight)
+            gs = []
+        else:                               # forward's order >= 3 route, keeping its intermediates
+            k = self.filter_fn.filter_channel_major(P)
+            fb = self.filter_fn.bias if self.filter_fn.use_bias else 0 * self.filter_fn.bias
+            cap = {}
+            y_pre = self._forward_chained(u32, k, fb, P, capture=cap)
+            y = _OutProj.apply(y_pre, self.out_proj.weight, self.out_proj.bias).to(in_dtype)
+            p, gs = cap["p"], cap["g"]
+        return y, p, gs
+
+    def check_admit(self, u, cache, rows, lengths=None):
+        """Every host check of ``admit(u, cache, rows, lengths)`` without device work (Block and Backbone run it before
+        their first kernel) -> (the operator's cache, the rows as a list, the prompts' first real positions)."""
+        if not isinstance(cache, DecodeCache):
+            raise HyenaB200Error(f"admit needs a DecodeCache (allocate_decode_cache), got {type(cache).__name__}")
+        c = cache.for_module(self)
+        if c.branched:
+            raise HyenaB200Error("admit: this cache is branched; admission, release and compaction need a full cache")
+        if u.requires_grad:
+            raise HyenaB200Error("decoding is inference only: the input requires grad (run under torch.no_grad())")
+        if self.filter_fn.bidirectional:
+            raise HyenaB200Error("decoding needs a causal filter; this HyenaFilter is bidirectional")
+        if u.dim() != 3 or u.shape[-1] != self.d_model or u.shape[0] < 1 or u.shape[1] < 1:
+            raise HyenaB200Error(f"admit: prompts must be (k, P, {self.d_model}); got {tuple(u.shape)}")
+        k, P = u.shape[0], u.shape[1]
+        rows = _host_index(rows, c.batch_size, "admit: rows")
+        if len(set(rows)) != len(rows):
+            raise HyenaB200Error(f"admit: rows {rows} repeat a row")
+        if len(rows) != k:
+            raise HyenaB200Error(f"admit: {len(rows)} rows for {k} prompts")
+        starts = [P - n for n in host_lengths(lengths, k, P)] if lengths is not None else [0] * k
+        ops.decode_admit_plan(c.t, c.lcap, P, c.win_b, c.win_wc)        # P <= Lcap, and the right shift fits
+        if not u.is_cuda or not c.k.is_cuda:
+            raise HyenaB200Error("decoding runs on CUDA sm_90a only; there is no CPU fallback")
+        return c, rows, starts
+
+    def admit(self, u, cache, rows, lengths=None):
+        """Prompts join a running cache: u (k, P, D) goes into the cache rows ``rows`` (k distinct rows, typically ones
+        freed by ``DecodeCache.release``) -> y (k, P, D), the bits ``prefill`` of u gives on a fresh k-row cache.  Each
+        prompt is placed so that it ends at the cache's position t, with a zero history before it, so its row decodes
+        exactly as after that prefill while the other rows go on unchanged (DESIGN.md section 4.15).  When P > t the whole
+        cache first shifts right by P - t rounded up to a multiple of 4 (at t = 0 the position becomes P, and every row
+        that takes no prompt is free).  ``lengths`` (k integers in [1, P]): the prompts are left-padded, as for prefill.
+        The other rows' history, tail and window are not touched; an open window stays open (the admitted rows' part of
+        it is recomputed).  Every row can hold up to Lcap - (t - m) more positions after a ``compact`` by m: the room is
+        bounded by the longest live row, not by the row's own length."""
+        c, rows, starts = self.check_admit(u, cache, rows, lengths)
+        P = u.shape[1]
+        with torch.no_grad():
+            if lengths is None:
+                row_start = None
+                y, p, gs = self._prefill_run(u)
+            else:
+                row_start = torch.tensor(starts, dtype=torch.int32, device=u.device)
+                y, p, gs = self._run_left_padded(u, row_start)
+            c._admit_clock(P)
+            ib, sw, sb = self._decode_params()
+            ops.decode_admit(p.contiguous(), ib, sw, sb, gs, c, rows, row_start)
+            c._took(rows, [c.t - P + s for s in starts])
         return y
 
     def _prefill_left_padded(self, u, cache, lengths):

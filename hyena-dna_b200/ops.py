@@ -1051,6 +1051,103 @@ def decode_branch_step(p_t, in_bias, sw, sb, cache):
     return out[-1]
 
 
+# ------------------------------------------------------------------------------------------ admission and compaction
+# The rows of a cache share one position t.  A prompt of P <= t positions joins row r by being placed at [t - P, t) with a
+# zero history before it: by time invariance (section 4.14) the row then decodes exactly like the unpadded prompt, and every
+# step, extend, window and StepGraph replay runs unchanged.  Room is reclaimed by shifting the whole history left by the
+# smallest first real position of the live rows (rounded down to a multiple of 4); a prompt longer than t shifts it right
+# first.  F of an open window is translation invariant, so the window survives a shift that keeps t inside it.  DESIGN.md
+# section 4.15.
+def _window_holds(t, win_b, win_wc):
+    return win_wc > 0 and win_b <= t < win_b + win_wc
+
+
+def decode_admit_plan(t, lcap, P, win_b=0, win_wc=0):
+    """(shift, t', keep) of admitting prompts of P positions into a cache at position t with Lcap = lcap and the window
+    [win_b, win_b + win_wc): shift > 0 is the right shift d = P - t rounded up to a multiple of 4 when P > t > 0 (0 when the
+    prompt fits before t, or at t = 0 where nothing is shifted and the clock moves to P); t' >= P the position after it; keep
+    whether the window, moved by the shift, still holds t' (within Lcap).  Raises when P > Lcap or t' would pass Lcap."""
+    t, lcap, P = int(t), int(lcap), int(P)
+    if P > lcap:
+        raise _lib.HyenaB200Error(f"admit: a prompt of {P} positions exceeds Lcap = {lcap}")
+    if P <= t:
+        return 0, t, _window_holds(t, win_b, win_wc)
+    if t == 0:
+        return 0, P, False
+    shift = (P - t + 3) // 4 * 4
+    if t + shift > lcap:
+        raise _lib.HyenaB200Error(f"admit: a prompt of {P} positions needs a right shift of {shift} at position {t}, past "
+                                  f"Lcap = {lcap}")
+    return shift, t + shift, _window_holds(t, win_b, win_wc) and win_b + shift + win_wc <= lcap
+
+
+def decode_compact_plan(t, starts, free, win_b=0, win_wc=0):
+    """(shift, t', keep) of compacting a cache at position t whose rows start at ``starts`` (one per row), with the rows
+    ``free`` released: shift = -m, m the smallest start of a live row rounded down to a multiple of 4 (t rounded down when
+    no row is live); keep whether the window, moved by -m, still holds t' = t - m (it does unless m > win_b)."""
+    t = int(t)
+    free = set(free)
+    live = [int(s) for b, s in enumerate(starts) if b not in free]
+    m = min(min(live), t) if live else t
+    m -= m % 4
+    return -m, t - m, _window_holds(t, win_b, win_wc) and m <= win_b
+
+
+def decode_shift(cache, shift):
+    """Move every history row of the operator cache by ``shift`` positions (a multiple of 4; < 0 left, > 0 right) over [0, t)
+    in place (csrc/decode.cuh decode_shift_kernel), and the position t, the row starts and the window base with it.  The
+    window is kept as it is (its F is translation invariant); whether it still holds t is the caller's plan."""
+    shift = int(shift)
+    if shift == 0:
+        return
+    with torch.cuda.device(cache.h.device):
+        _lib.check(_lib.lib().hyena_b200_decode_shift(_ptr(cache.h), cache.batch_size, cache.d_model, cache.order,
+                                                      int(cache.t), shift, cache.lcap, _stream()))
+    start = cache.start if cache.start is not None else (0,) * cache.batch_size
+    cache.set_start([max(s + shift, 0) for s in start])
+    cache.t += shift
+    cache.win_b = max(cache.win_b + shift, 0)
+
+
+def decode_admit(p, in_bias, sw, sb, gs, cache, rows, row_start=None):
+    """Write prompts into rows of a running operator cache at position t = cache.t so that each ends at t: p (k, (O+1) D, P)
+    the prompts' in_proj output without its bias, gs the prompts' g_o of the recurrences o >= 1 (order >= 3; zero at pads),
+    ``rows`` (k host integers) the destination rows, ``row_start`` ((k,) int32 on the device, or None) the ragged prompts'
+    first real positions.  Recurrence 0: one decode_admit launch (the zero prefix, g_0 and the tail); the later recurrences'
+    g copied with a zero prefix in torch.  With a window open, the admitted rows' F is rewritten in place: zero when the
+    prompts start at or after the window base, else the convolution of their history [floor4(t - P), win_b) -- O(P + W)."""
+    _need_cuda(p, in_bias, sw, sb)
+    k, C, P = p.shape
+    D, O, t = cache.d_model, cache.order, int(cache.t)
+    if not p.is_contiguous() or C != (O + 1) * D or k != len(rows):
+        raise _lib.HyenaB200Error(f"decode_admit: p must be contiguous ({len(rows)}, {(O + 1) * D}, P)")
+    if row_start is not None and (row_start.dtype != torch.int32 or row_start.device != p.device
+                                  or tuple(row_start.shape) != (k,) or not row_start.is_contiguous()):
+        raise _lib.HyenaB200Error(f"decode_admit: row_start must be a contiguous ({k},) int32 tensor on {p.device}")
+    dev = p.device
+    rows_dev = torch.tensor(rows, dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().hyena_b200_decode_admit(
+            _ptr(p), _ptr(in_bias), _ptr(sw), _ptr(sb), _ptr(cache.h), _ptr(cache.tail), _ptr(rows_dev), _ptr(row_start), k,
+            cache.batch_size, D, O, P, t, cache.lcap, _stream()))
+    off = t - P
+    ridx = rows_dev.to(torch.long)
+    for o in range(1, O - 1):
+        g = torch.zeros(k, D, t, dtype=torch.float32, device=dev)
+        g[:, :, off:] = gs[o]
+        cache.h[o, ridx, :, :t] = g
+    if cache.win_wc > 0:
+        b, wc = cache.win_b, cache.win_wc
+        if off >= b:
+            cache.win_f[:, ridx, :, :wc] = 0.0
+        else:
+            a = off - off % 4
+            ld = cache.h.shape[-1]
+            for o in range(O - 1):
+                conv = _history_conv(cache, ld, cache.h[o, ridx, :, a:b], o, b - a, b - a + wc)
+                cache.win_f[o, ridx, :, :wc] = conv[:, :, b - a:]
+
+
 # ------------------------------------------------------------------------------------------ device-position steps
 # The steps above take the position from the host (cache.t), so a captured CUDA graph would replay one position forever.
 # These variants read t, the window base and the branch base from cache.pos ([t, win_b, base], int32 on the device) inside

@@ -280,6 +280,21 @@ HY_API int hyena_b200_decode_hist(const float* p, const float* in_bias, const fl
 HY_API int hyena_b200_decode_hist_rows(const float* p, const float* in_bias, const float* sw, const float* sb, float* h,
                                        float* tail, const int* row_start, int B, int cache_B, int D, int order, int P,
                                        int Lcap, void* stream);
+/*   decode_admit: k prompts of P positions join a running cache at position t (P <= t <= Lcap) so that each ends at t:
+ *                p (k, C, P) channel-major WITHOUT in_proj.bias; rows (k) int32 on the device gives each prompt's cache row
+ *                (not checked here: distinct, in [0, cache_B)); row_start (k) int32 on the device or NULL: prompt i's
+ *                positions j < row_start[i] are padding, as in decode_hist_rows.  Row rows[i] of h (recurrence 0) gets 0 at
+ *                positions [0, t - P + row_start[i]) and g_0 of the prompt's real positions from there to t; its tail (all C
+ *                channels) gets the prompt's last two in_proj outputs.  Other rows are not touched.  One launch, counted
+ *                under the kind decode_hist.
+ *   decode_shift: every row of h (O-1, B, D, ld), 16-byte aligned, moves in place by `shift` positions, a multiple of 4:
+ *                left (shift = -m, m <= t): h[tau] = h[tau + m] for tau < round4(t) - m; right (shift = d, t + d <= Lcap):
+ *                h[tau + d] = h[tau] for tau < round4(t), then [0, d) is zeroed.  Positions past round4(t) and every other
+ *                buffer stay.  One launch (none for shift 0), counted by launch_count under no kind. */
+HY_API int hyena_b200_decode_admit(const float* p, const float* in_bias, const float* sw, const float* sb, float* h,
+                                   float* tail, const int* rows, const int* row_start, int k, int cache_B, int D, int order,
+                                   int P, int t, int Lcap, void* stream);
+HY_API int hyena_b200_decode_shift(float* h, int B, int D, int order, int t, int shift, int Lcap, void* stream);
 HY_API int hyena_b200_decode_step(const float* p_t, const float* in_bias, const float* sw, const float* sb, const float* k,
                                   const float* fbias, float* h, float* tail, float* s_t, const float* v_in, float* out,
                                   float* part, int B, int cache_B, int D, int order, int o, int t, int Lcap, void* stream);
