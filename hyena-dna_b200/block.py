@@ -43,6 +43,8 @@ class Block(nn.Module):
         for n in (self.norm1, getattr(self, "norm2", None)):
             if n is not None and not isinstance(n, nn.LayerNorm):
                 raise HyenaB200Error("Block: only nn.LayerNorm is supported by the fused add + norm kernel")
+            if n is not None and not n.elementwise_affine:
+                raise HyenaB200Error("Block: the fused add + norm kernel needs an affine LayerNorm (elementwise_affine=True)")
         if mark_shared_params:
             for p in list(self.norm1.parameters()) + (list(self.norm2.parameters()) if hasattr(self, "norm2") else []):
                 p._shared_params = True

@@ -36,7 +36,7 @@ cudaError_t launch_add_ln_bwd(ln::BwdArgs a, float* dw, float* db, cudaStream_t 
                    aligned16p(a.w) && (!a.dres || aligned16p(a.dres));
   prof_begin(K_ADD_LN, s);
   if (!vec) {
-    ln::add_ln_bwd_generic_kernel<<<grid, 32 * ln::kWarps, 2 * a.D * sizeof(float), s>>>(a);
+    ln::add_ln_bwd_generic_kernel<<<grid, 32 * ln::kWarps, 0, s>>>(a);
   } else {
     const size_t sh = (size_t)ln::kWarps * 2 * a.D * sizeof(float);     // <= 64 KB at D = 1024
     cudaError_t e = cudaSuccess;

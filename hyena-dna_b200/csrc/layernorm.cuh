@@ -9,8 +9,10 @@
 //             one warp per row, the row lives in registers (two sweeps: mean, then centred sum of squares);
 //             HBM traffic 4 x 4 D bytes per row (x, res in; r, y out) + 8 bytes of statistics
 //   backward  g = dy * w;  dr = rstd * (g - mean_D(g) - xhat * mean_D(g * xhat)) + dres;  dx = dres_in = dr
-//             dw += sum_rows dy * xhat,  db += sum_rows dy: per-CTA partials in shared memory, written to a
-//             (CTAs, 2, D) scratch and summed in fixed order by ln_reduce_kernel (deterministic, no atomics)
+//             dw += sum_rows dy * xhat,  db += sum_rows dy: per-CTA partials written to a (CTAs, 2, D) scratch and
+//             summed in fixed order by ln_reduce_kernel (deterministic, no atomics).  Register path: per-lane sums over
+//             the CTA's rows, combined across its warps in shared memory.  Generic path: per-thread column sums over a
+//             contiguous block of rows, no shared memory.
 // fp32 throughout (residual_in_fp32 semantics).  Memory-bound elementwise work: coalesced float4 rows, grid = a multiple
 // of the SM count, no shared-memory staging needed.
 #pragma once
@@ -175,11 +177,11 @@ __global__ void __launch_bounds__(32 * kWarps) add_ln_bwd_kernel(const BwdArgs a
   }
 }
 
+// any D and any alignment, scalar accesses, no shared memory (so no limit on D).  Two independent sweeps: dx row by row
+// (one warp per row, grid-stride, as the forward); then dw / db by columns over a contiguous block of rows per CTA, each
+// thread summing its columns in row order into part[CTA] -- fixed order, deterministic, no atomics
 __global__ void __launch_bounds__(32 * kWarps) add_ln_bwd_generic_kernel(const BwdArgs a) {
-  extern __shared__ float sh[];                       // [2][D] accumulated with shared atomics per CTA (then one store)
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int j = threadIdx.x; j < 2 * a.D; j += blockDim.x) sh[j] = 0.f;
-  __syncthreads();
   const float invD = 1.0f / (float)a.D;
   for (long long row = (long long)blockIdx.x * kWarps + warp; row < a.rows; row += (long long)gridDim.x * kWarps) {
     const float mean = __ldg(a.mean + row), rstd = __ldg(a.rstd + row);
@@ -192,14 +194,24 @@ __global__ void __launch_bounds__(32 * kWarps) add_ln_bwd_generic_kernel(const B
     }
     const float m1 = warp_sum(s1) * invD, m2 = warp_sum(s2) * invD;
     for (int c = lane; c < a.D; c += 32) {
-      const float xh = (rr[c] - mean) * rstd, d = dyr[c], g = d * __ldg(a.w + c);
+      const float xh = (rr[c] - mean) * rstd, g = dyr[c] * __ldg(a.w + c);
       a.dx[row * a.D + c] = rstd * (g - m1 - xh * m2) + (a.dres ? a.dres[row * a.D + c] : 0.f);
-      atomicAdd(sh + c, d * xh);
-      atomicAdd(sh + a.D + c, d);
     }
   }
-  __syncthreads();
-  for (int j = threadIdx.x; j < 2 * a.D; j += blockDim.x) a.part[(size_t)blockIdx.x * 2 * a.D + j] = sh[j];
+  const long long per = (a.rows + gridDim.x - 1) / gridDim.x;
+  const long long r0 = min(a.rows, (long long)blockIdx.x * per), r1 = min(a.rows, r0 + per);
+  float* out = a.part + (size_t)blockIdx.x * 2 * a.D;
+  for (int c = threadIdx.x; c < a.D; c += blockDim.x) {
+    float sw = 0.f, sb = 0.f;
+#pragma unroll 4
+    for (long long row = r0; row < r1; ++row) {
+      const float d = a.dy[row * a.D + c];
+      sw = fmaf(d, (a.r[row * a.D + c] - __ldg(a.mean + row)) * __ldg(a.rstd + row), sw);
+      sb += d;
+    }
+    out[c] = sw;
+    out[a.D + c] = sb;
+  }
 }
 
 // dw[j] (+)= sum over CTAs of part[cta][0][j]; db likewise (fixed order)
