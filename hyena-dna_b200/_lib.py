@@ -80,6 +80,11 @@ SIGNATURES = {
     "hyena_b200_decode_branch_step_dev": (_i, [c_fp] * 15 + [_i] * 6 + [_vp]),
     "hyena_b200_decode_pos_advance": (_i, [c_fp, _vp]),
 }
+# the entry points of a 16-bit decode history: the fp32 twin's arguments after a history dtype code (HIST_F16, HIST_BF16)
+SIGNATURES.update({f"{name}_h16": (res, [_i] + args) for name, (res, args) in list(SIGNATURES.items())
+                   if name.startswith("hyena_b200_decode_") and name not in
+                   ("hyena_b200_decode_extend_groups", "hyena_b200_decode_pos_advance")})
+HIST_F16, HIST_BF16 = 1, 2    # include/hyena_b200.h HYENA_B200_HIST_F16 / _BF16
 
 
 class HyenaB200Error(RuntimeError):

@@ -15,7 +15,7 @@ import torch.nn as nn
 
 from . import ops
 from ._lib import HyenaB200Error
-from .decode import DecodeCache, StepGraph
+from .decode import DecodeCache, StepGraph, check_history_dtype
 
 
 class Block(nn.Module):
@@ -153,9 +153,11 @@ class Backbone(nn.Module):
         y, _ = Block._add_norm(hidden_states, residual, self.ln_f)
         return y.to(hidden_states.dtype)
 
-    def allocate_decode_cache(self, batch_size, max_seqlen):
-        """One DecodeCache holding the state of every layer's mixer (decode.py)."""
-        return DecodeCache.stack(layer.mixer.allocate_decode_cache(batch_size, max_seqlen) for layer in self.layers)
+    def allocate_decode_cache(self, batch_size, max_seqlen, history_dtype=torch.float32):
+        """One DecodeCache holding the state of every layer's mixer (decode.py), each history stored as ``history_dtype``."""
+        check_history_dtype(history_dtype)
+        return DecodeCache.stack(layer.mixer.allocate_decode_cache(batch_size, max_seqlen, history_dtype)
+                                 for layer in self.layers)
 
     def prefill(self, hidden_states, cache, lengths=None):
         """forward over the first P positions (B, P, D), filling ``cache`` for step(); ``lengths``: left-padded prompts of

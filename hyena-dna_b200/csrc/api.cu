@@ -6,8 +6,12 @@
 #include <cstring>
 #include <map>
 #include <mutex>
+#include <type_traits>
 #include <utility>
 #include <vector>
+
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 
 #include "../../include/hyena_b200.h"
 #include "launch.h"
@@ -141,6 +145,13 @@ static int channels_per_group(size_t bytes_for_A, int B, int D, int L) {
 static bool aligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3u) == 0; }
 static bool aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7u) == 0; }
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+// a decode history of element type T: one element, and the 4 positions the vector loads and the shift move at once
+template <class T> static bool elem_aligned(const T* p) { return reinterpret_cast<uintptr_t>(p) % sizeof(T) == 0; }
+template <class T> static bool hist_aligned(const T* p) { return reinterpret_cast<uintptr_t>(p) % (4 * sizeof(T)) == 0; }
+template <class T> constexpr bool kFp32 = std::is_same<T, float>::value;
+template <class T> constexpr const char* kAlignH = kFp32<T> ? "h must be 16-byte aligned" : "h must be 8-byte aligned";
+template <class T> constexpr const char* kAlignKH =
+    kFp32<T> ? "k and h must be 16-byte aligned" : "k must be 16-byte aligned and h 8-byte aligned";
 
 struct Carve { float2* A; float2* A2; float2* A3; int nch; };
 
@@ -810,6 +821,9 @@ HY_API int hyena_b200_add_layernorm_bwd(const float* dy, const float* dres, cons
   return 0;
 }
 
+}  // extern "C"
+
+// ---- incremental decoding: the checks and launches of every entry point, templates over the history element type
 /* incremental decoding of the causal operator (the reference's HyenaOperator.recurrence hook, hyena.py:384-386) */
 static int check_decode_shape(int B, int cache_B, int D, int order, int Lcap) {
   HY_CHECK(B >= 1 && D >= 1 && Lcap >= 1, "bad shape B=%d D=%d Lcap=%d", B, D, Lcap);
@@ -819,64 +833,70 @@ static int check_decode_shape(int B, int cache_B, int D, int order, int Lcap) {
   return 0;
 }
 
-HY_API int hyena_b200_decode_hist(const float* p, const float* in_bias, const float* sw, const float* sb, float* h,
-                                  float* tail, int B, int cache_B, int D, int order, int P, int Lcap, void* stream) {
+template <class T>
+static int decode_hist(const float* p, const float* in_bias, const float* sw, const float* sb, T* h, float* tail, int B,
+                       int cache_B, int D, int order, int P, int Lcap, void* stream) {
   if (check_decode_shape(B, cache_B, D, order, Lcap)) return 1;
   HY_CHECK(p && sw && sb && h && tail, "null pointer");
   HY_CHECK(P >= 1 && P <= Lcap, "prefill of %d positions outside [1, %d]", P, Lcap);
-  dec::HistArgs a{p, in_bias, sw, sb, h, tail, B, D, (order + 1) * D, P, dec::ld_for(Lcap), (order - 1) * D, nullptr};
+  dec::HistArgsT<T> a{p, in_bias, sw, sb, h, tail, B, D, (order + 1) * D, P, dec::ld_for(Lcap), (order - 1) * D,
+                      nullptr};
   HY_CUDA(launch_decode_hist(a, (cudaStream_t)stream));
   return 0;
 }
 
-HY_API int hyena_b200_decode_hist_rows(const float* p, const float* in_bias, const float* sw, const float* sb, float* h,
-                                       float* tail, const int* row_start, int B, int cache_B, int D, int order, int P,
-                                       int Lcap, void* stream) {
+template <class T>
+static int decode_hist_rows(const float* p, const float* in_bias, const float* sw, const float* sb, T* h, float* tail,
+                            const int* row_start, int B, int cache_B, int D, int order, int P, int Lcap, void* stream) {
   if (check_decode_shape(B, cache_B, D, order, Lcap)) return 1;
   HY_CHECK(p && sw && sb && h && tail && row_start, "null pointer");
   HY_CHECK(P >= 1 && P <= Lcap, "prefill of %d positions outside [1, %d]", P, Lcap);
-  HY_CHECK(aligned4(p) && aligned4(sw) && aligned4(sb) && aligned4(h) && aligned4(tail) && aligned4(row_start) &&
+  HY_CHECK(aligned4(p) && aligned4(sw) && aligned4(sb) && elem_aligned(h) && aligned4(tail) && aligned4(row_start) &&
                (!in_bias || aligned4(in_bias)),
            "misaligned pointer: p, in_bias, sw, sb, h, tail and row_start must be 4-byte aligned");
-  dec::HistArgs a{p, in_bias, sw, sb, h, tail, B, D, (order + 1) * D, P, dec::ld_for(Lcap), (order - 1) * D, row_start};
+  dec::HistArgsT<T> a{p, in_bias, sw, sb, h, tail, B, D, (order + 1) * D, P, dec::ld_for(Lcap), (order - 1) * D,
+                      row_start};
   HY_CUDA(launch_decode_hist(a, (cudaStream_t)stream));
   return 0;
 }
 
-HY_API int hyena_b200_decode_admit(const float* p, const float* in_bias, const float* sw, const float* sb, float* h,
-                                   float* tail, const int* rows, const int* row_start, int k, int cache_B, int D, int order,
-                                   int P, int t, int Lcap, void* stream) {
+template <class T>
+static int decode_admit(const float* p, const float* in_bias, const float* sw, const float* sb, T* h, float* tail,
+                        const int* rows, const int* row_start, int k, int cache_B, int D, int order, int P, int t,
+                        int Lcap, void* stream) {
   if (check_decode_shape(k, k, D, order, Lcap)) return 1;
   HY_CHECK(k <= cache_B, "%d prompts for a decode cache of %d rows", k, cache_B);
   HY_CHECK(p && sw && sb && h && tail && rows, "null pointer");
-  HY_CHECK(aligned4(p) && aligned4(sw) && aligned4(sb) && aligned4(h) && aligned4(tail) && aligned4(rows) &&
+  HY_CHECK(aligned4(p) && aligned4(sw) && aligned4(sb) && elem_aligned(h) && aligned4(tail) && aligned4(rows) &&
                (!in_bias || aligned4(in_bias)) && (!row_start || aligned4(row_start)),
            "misaligned pointer: p, in_bias, sw, sb, h, tail, rows and row_start must be 4-byte aligned");
   HY_CHECK(t >= 0 && t <= Lcap, "position %d outside the decode cache [0, %d]", t, Lcap);
   HY_CHECK(P >= 1 && P <= t, "a prompt of %d positions cannot end at position %d (it needs 1 <= P <= t)", P, t);
-  dec::AdmitArgs a{{p, in_bias, sw, sb, h, tail, k, D, (order + 1) * D, P, dec::ld_for(Lcap), (order - 1) * D, row_start},
-                   rows, t - P, t};
+  dec::AdmitArgsT<T> a{{p, in_bias, sw, sb, h, tail, k, D, (order + 1) * D, P, dec::ld_for(Lcap), (order - 1) * D,
+                        row_start}, rows, t - P, t};
   HY_CUDA(launch_decode_admit(a, (cudaStream_t)stream));
   return 0;
 }
 
-HY_API int hyena_b200_decode_shift(float* h, int B, int D, int order, int t, int shift, int Lcap, void* stream) {
+template <class T>
+static int decode_shift(T* h, int B, int D, int order, int t, int shift, int Lcap, void* stream) {
   if (check_decode_shape(B, B, D, order, Lcap)) return 1;
   HY_CHECK(h, "null pointer");
-  HY_CHECK(aligned16(h), "h must be 16-byte aligned");
+  HY_CHECK(hist_aligned(h), "%s", kAlignH<T>);
   HY_CHECK(t >= 0 && t <= Lcap, "position %d outside the decode cache [0, %d]", t, Lcap);
   HY_CHECK((shift & 3) == 0, "shift %d is not a multiple of 4", shift);
   HY_CHECK(shift >= -t, "left shift by %d past the start of a history of %d positions", -shift, t);
   HY_CHECK(shift <= Lcap - t, "right shift by %d moves position %d past the decode cache's %d", shift, t, Lcap);
   if (shift == 0) return 0;
-  dec::ShiftArgs a{h, dec::ld_for(Lcap), t, shift};
+  dec::ShiftArgsT<T> a{h, dec::ld_for(Lcap), t, shift};
   HY_CUDA(launch_decode_shift(a, (long long)(order - 1) * B * D, (cudaStream_t)stream));
   return 0;
 }
 
-HY_API int hyena_b200_decode_step(const float* p_t, const float* in_bias, const float* sw, const float* sb, const float* k,
-                                  const float* fbias, float* h, float* tail, float* s_t, const float* v_in, float* out,
-                                  float* part, int B, int cache_B, int D, int order, int o, int t, int Lcap, void* stream) {
+template <class T>
+static int decode_step(const float* p_t, const float* in_bias, const float* sw, const float* sb, const float* k,
+                       const float* fbias, T* h, float* tail, float* s_t, const float* v_in, float* out, float* part,
+                       int B, int cache_B, int D, int order, int o, int t, int Lcap, void* stream) {
   if (check_decode_shape(B, cache_B, D, order, Lcap)) return 1;
   HY_CHECK(k && fbias && h && s_t && out && part, "null pointer");
   HY_CHECK(o >= 0 && o < order - 1, "recurrence %d outside [0, %d)", o, order - 1);
@@ -884,20 +904,21 @@ HY_API int hyena_b200_decode_step(const float* p_t, const float* in_bias, const 
            o == 0 ? "null pointer: recurrence 0 needs p_t, sw, sb, tail (and no v_in)" : "null pointer: v_in");
   HY_CHECK(t >= 0 && t < Lcap, "position %d outside the decode cache [0, %d)", t, Lcap);
   const int ld = dec::ld_for(Lcap);
-  HY_CHECK(aligned16(k) && aligned16(h), "k and h must be 16-byte aligned");
+  HY_CHECK(aligned16(k) && hist_aligned(h), "%s", kAlignKH<T>);
   const int F = order - 1;
-  dec::DotArgs dot{h, k + (size_t)o * ld, part, B, D, t, ld, F * ld, dec::chunks_for(Lcap)};
-  dec::StepArgs st{part, (t + dec::kChunk - 1) / dec::kChunk, dec::chunks_for(Lcap), k + (size_t)o * ld, fbias + o, F * ld, F,
-                   ld, p_t, in_bias, sw, sb, tail, s_t, v_in, h, out, B, D, (order + 1) * D, order, t, (order - 1 - o) * D,
-                   o == order - 2};
+  dec::DotArgsT<T> dot{h, k + (size_t)o * ld, part, B, D, t, ld, F * ld, dec::chunks_for(Lcap)};
+  dec::StepArgsT<T> st{part, (t + dec::kChunk - 1) / dec::kChunk, dec::chunks_for(Lcap), k + (size_t)o * ld, fbias + o,
+                       F * ld, F, ld, p_t, in_bias, sw, sb, tail, s_t, v_in, h, out, B, D, (order + 1) * D, order, t,
+                       (order - 1 - o) * D, o == order - 2};
   HY_CUDA(launch_decode_step(dot, st, (cudaStream_t)stream));
   return 0;
 }
 
-HY_API int hyena_b200_decode_win_step(const float* p_t, const float* in_bias, const float* sw, const float* sb,
-                                      const float* k, const float* fbias, float* h, float* tail, float* s_t,
-                                      const float* v_in, float* out, float* part, const float* win, int B, int cache_B,
-                                      int D, int order, int o, int t, int b, int Wc, int W, int Lcap, void* stream) {
+template <class T>
+static int decode_win_step(const float* p_t, const float* in_bias, const float* sw, const float* sb, const float* k,
+                           const float* fbias, T* h, float* tail, float* s_t, const float* v_in, float* out,
+                           float* part, const float* win, int B, int cache_B, int D, int order, int o, int t, int b,
+                           int Wc, int W, int Lcap, void* stream) {
   if (check_decode_shape(B, cache_B, D, order, Lcap)) return 1;
   HY_CHECK(k && fbias && h && s_t && out && part && win, "null pointer");
   HY_CHECK(o >= 0 && o < order - 1, "recurrence %d outside [0, %d)", o, order - 1);
@@ -908,13 +929,12 @@ HY_API int hyena_b200_decode_win_step(const float* p_t, const float* in_bias, co
            b + Wc, W, Lcap);
   HY_CHECK(t - b >= 0 && t - b < Wc, "position %d outside the window [%d, %d)", t, b, b + Wc);
   const int ld = dec::ld_for(Lcap);
-  HY_CHECK(aligned16(k) && aligned16(h), "k and h must be 16-byte aligned");
+  HY_CHECK(aligned16(k) && hist_aligned(h), "%s", kAlignKH<T>);
   const int F = order - 1;
-  dec::DotArgs dot{h + b, k + (size_t)o * ld, part, B, D, t - b, ld, F * ld, dec::chunks_for(Lcap)};
-  dec::WinStepArgs w{{part, (t - b + dec::kChunk - 1) / dec::kChunk, dec::chunks_for(Lcap), k + (size_t)o * ld, fbias + o,
-                      F * ld, F, ld, p_t, in_bias, sw, sb, tail, s_t, v_in, h, out, B, D, (order + 1) * D, order, t,
-                      (order - 1 - o) * D, o == order - 2},
-                     win, W, t - b};
+  dec::DotArgsT<T> dot{h + b, k + (size_t)o * ld, part, B, D, t - b, ld, F * ld, dec::chunks_for(Lcap)};
+  dec::WinStepArgsT<T> w{{part, (t - b + dec::kChunk - 1) / dec::kChunk, dec::chunks_for(Lcap), k + (size_t)o * ld,
+                          fbias + o, F * ld, F, ld, p_t, in_bias, sw, sb, tail, s_t, v_in, h, out, B, D,
+                          (order + 1) * D, order, t, (order - 1 - o) * D, o == order - 2}, win, W, t - b};
   HY_CUDA(launch_decode_win_step(dot, w, (cudaStream_t)stream));
   return 0;
 }
@@ -931,49 +951,57 @@ HY_API int hyena_b200_decode_extend_groups(int B, int D, int t, int n) {
   return dec::ext_groups(B, D, t, n);
 }
 
-HY_API int hyena_b200_decode_extend_hist(const float* p, const float* in_bias, const float* sw, const float* sb, float* h,
-                                         float* tail, float* s, int B, int cache_B, int D, int order, int t, int n, int Lcap,
-                                         void* stream) {
+template <class T>
+static int decode_extend_hist(const float* p, const float* in_bias, const float* sw, const float* sb, T* h, float* tail,
+                              float* s, int B, int cache_B, int D, int order, int t, int n, int Lcap, void* stream) {
   if (check_decode_shape(B, cache_B, D, order, Lcap) || check_extend_range(t, n, Lcap)) return 1;
   HY_CHECK(p && sw && sb && h && tail && s, "null pointer");
-  dec::ExtHistArgs a{p, in_bias, sw, sb, tail, s, h, B, D, (order + 1) * D, t, n, dec::ld_for(Lcap), (order - 1) * D};
+  dec::ExtHistArgsT<T> a{p, in_bias, sw, sb, tail, s, h, B, D, (order + 1) * D, t, n, dec::ld_for(Lcap),
+                         (order - 1) * D};
   HY_CUDA(launch_decode_ext_hist(a, (cudaStream_t)stream));
   return 0;
 }
 
-HY_API int hyena_b200_decode_extend_dot(const float* h, const float* k, float* part, int groups, int B, int cache_B, int D,
-                                        int order, int o, int t, int n, int Lcap, void* stream) {
+template <class T>
+static int decode_extend_dot(const T* h, const float* k, float* part, int groups, int B, int cache_B, int D, int order,
+                             int o, int t, int n, int Lcap, void* stream) {
   if (check_decode_shape(B, cache_B, D, order, Lcap) || check_extend_range(t, n, Lcap)) return 1;
   HY_CHECK(h && k && part, "null pointer");
   HY_CHECK(o >= 0 && o < order - 1, "recurrence %d outside [0, %d)", o, order - 1);
   HY_CHECK(groups == dec::ext_groups(B, D, t, n), "partials sized for %d groups; this extend needs %d "
            "(hyena_b200_decode_extend_groups)", groups, dec::ext_groups(B, D, t, n));
-  HY_CHECK(aligned16(k) && aligned16(h), "k and h must be 16-byte aligned");
+  HY_CHECK(aligned16(k) && hist_aligned(h), "%s", kAlignKH<T>);
   const int ld = dec::ld_for(Lcap), F = order - 1;
   const int NT = dec::ext_tile(n);
-  dec::ExtDotArgs a{h, k + (size_t)o * ld, part, B, D, t, n, ld, F * ld, (-t) & 3, (n + NT - 1) / NT,
-                    dec::ext_chunks_per_cta(B, D, t, n), dec::chunks_for(t + n), groups};
+  dec::ExtDotArgsT<T> a{h, k + (size_t)o * ld, part, B, D, t, n, ld, F * ld, (-t) & 3, (n + NT - 1) / NT,
+                        dec::ext_chunks_per_cta(B, D, t, n), dec::chunks_for(t + n), groups};
   HY_CUDA(launch_decode_ext_dot(a, (cudaStream_t)stream));
   return 0;
 }
 
-HY_API int hyena_b200_decode_extend_combine(const float* part, long long row_stride, int j_stride, int groups,
-                                            const float* fbias, const float* h, const float* s, float* out, int B,
-                                            int cache_B, int D, int order, int o, int t, int n, int Lcap, void* stream) {
+template <class T>
+static int decode_extend_combine(const float* part, long long row_stride, int j_stride, int groups, const float* fbias,
+                                 const T* h, const float* s, void* out, int B, int cache_B, int D, int order, int o,
+                                 int t, int n, int Lcap, void* stream) {
   if (check_decode_shape(B, cache_B, D, order, Lcap) || check_extend_range(t, n, Lcap)) return 1;
   HY_CHECK(part && fbias && h && s && out, "null pointer");
   HY_CHECK(o >= 0 && o < order - 1, "recurrence %d outside [0, %d)", o, order - 1);
   HY_CHECK(groups >= 1 && j_stride >= 0 && row_stride >= 0, "bad partial layout: groups %d, strides %lld / %d", groups,
            row_stride, j_stride);
+  if constexpr (!kFp32<T>)
+    HY_CHECK(elem_aligned(h) && elem_aligned(static_cast<T*>(out)),
+             "misaligned pointer: h and out must be 2-byte aligned");
   const int ld = dec::ld_for(Lcap), last = o == order - 2;
-  dec::ExtCombineArgs a{part, row_stride, j_stride, groups, fbias + o, order - 1, h, s, last ? nullptr : out,
-                        last ? out : nullptr, B, D, (order + 1) * D, t, n, ld, (order - 2 - o) * D, last};
+  dec::ExtCombineArgsT<T> a{part, row_stride, j_stride, groups, fbias + o, order - 1, h, s,
+                            last ? nullptr : static_cast<T*>(out), last ? static_cast<float*>(out) : nullptr, B, D,
+                            (order + 1) * D, t, n, ld, (order - 2 - o) * D, last};
   HY_CUDA(launch_decode_ext_combine(a, (cudaStream_t)stream));
   return 0;
 }
 
-/* decoding a branched cache (DecodeCache.fork): each of the R rows holds positions [b, b + Hc) of one branch with row stride
-   H; the filter is the parent cache's (row stride ld = ld_for(Lcap)) and is addressed from k + ld - H (decode_args.h) */
+/* decoding a branched cache (DecodeCache.fork): each of the R rows holds positions [b, b + Hc) of one branch with row
+   stride H; the filter is the parent cache's (row stride ld = ld_for(Lcap)) and is addressed from k + ld - H
+   (decode_args.h) */
 static int check_branch(int R, int D, int order, int o, int t, int n, int b, int Hc, int H, int Lcap) {
   if (check_decode_shape(R, R, D, order, Lcap)) return 1;
   HY_CHECK(o >= 0 && o < order - 1, "recurrence %d outside [0, %d)", o, order - 1);
@@ -986,126 +1014,134 @@ static int check_branch(int R, int D, int order, int o, int t, int n, int b, int
   return 0;
 }
 
-HY_API int hyena_b200_decode_branch_step(const float* p_t, const float* in_bias, const float* sw, const float* sb,
-                                         const float* k, const float* fbias, float* h, float* tail, float* s_t,
-                                         const float* v_in, float* out, float* part, const float* f, const int* parent,
-                                         int R, int D, int order, int o, int t, int b, int Hc, int H, int Lcap,
-                                         void* stream) {
+template <class T>
+static int decode_branch_step(const float* p_t, const float* in_bias, const float* sw, const float* sb, const float* k,
+                              const float* fbias, T* h, float* tail, float* s_t, const float* v_in, float* out,
+                              float* part, const float* f, const int* parent, int R, int D, int order, int o, int t,
+                              int b, int Hc, int H, int Lcap, void* stream) {
   if (check_branch(R, D, order, o, t, 1, b, Hc, H, Lcap)) return 1;
   HY_CHECK(k && fbias && h && s_t && out && part && f && parent, "null pointer");
   HY_CHECK(o == 0 ? (p_t && sw && sb && tail && !v_in) : (v_in != nullptr),
            o == 0 ? "null pointer: recurrence 0 needs p_t, sw, sb, tail (and no v_in)" : "null pointer: v_in");
-  HY_CHECK(aligned16(k) && aligned16(h), "k and h must be 16-byte aligned");
+  HY_CHECK(aligned16(k) && hist_aligned(h), "%s", kAlignKH<T>);
   const int ld = dec::ld_for(Lcap), F = order - 1;
   const float* kb = k + (size_t)o * ld + (ld - H);
-  dec::DotArgs dot{h, kb, part, R, D, t - b, H, F * ld, dec::chunks_for(H)};
-  dec::BranchStepArgs w{{part, (t - b + dec::kChunk - 1) / dec::kChunk, dec::chunks_for(H), kb, fbias + o, F * ld, F, H,
-                         p_t, in_bias, sw, sb, tail, s_t, v_in, h, out, R, D, (order + 1) * D, order, t - b,
-                         (order - 1 - o) * D, o == order - 2},
-                        f, parent};
+  dec::DotArgsT<T> dot{h, kb, part, R, D, t - b, H, F * ld, dec::chunks_for(H)};
+  dec::BranchStepArgsT<T> w{{part, (t - b + dec::kChunk - 1) / dec::kChunk, dec::chunks_for(H), kb, fbias + o, F * ld,
+                             F, H, p_t, in_bias, sw, sb, tail, s_t, v_in, h, out, R, D, (order + 1) * D, order, t - b,
+                             (order - 1 - o) * D, o == order - 2}, f, parent};
   HY_CUDA(launch_decode_branch_step(dot, w, (cudaStream_t)stream));
   return 0;
 }
 
-HY_API int hyena_b200_decode_branch_extend_hist(const float* p, const float* in_bias, const float* sw, const float* sb,
-                                                float* h, float* tail, float* s, int R, int D, int order, int t, int n,
-                                                int b, int Hc, int H, int Lcap, void* stream) {
+template <class T>
+static int decode_branch_extend_hist(const float* p, const float* in_bias, const float* sw, const float* sb, T* h,
+                                     float* tail, float* s, int R, int D, int order, int t, int n, int b, int Hc, int H,
+                                     int Lcap, void* stream) {
   if (check_branch(R, D, order, 0, t, n, b, Hc, H, Lcap)) return 1;
   HY_CHECK(p && sw && sb && h && tail && s, "null pointer");
-  dec::ExtHistArgs a{p, in_bias, sw, sb, tail, s, h, R, D, (order + 1) * D, t - b, n, H, (order - 1) * D};
+  dec::ExtHistArgsT<T> a{p, in_bias, sw, sb, tail, s, h, R, D, (order + 1) * D, t - b, n, H, (order - 1) * D};
   HY_CUDA(launch_decode_ext_hist(a, (cudaStream_t)stream));
   return 0;
 }
 
-HY_API int hyena_b200_decode_branch_extend_dot(const float* h, const float* k, float* part, int groups, int R, int D,
-                                               int order, int o, int t, int n, int b, int Hc, int H, int Lcap,
-                                               void* stream) {
+template <class T>
+static int decode_branch_extend_dot(const T* h, const float* k, float* part, int groups, int R, int D, int order, int o,
+                                    int t, int n, int b, int Hc, int H, int Lcap, void* stream) {
   if (check_branch(R, D, order, o, t, n, b, Hc, H, Lcap)) return 1;
   HY_CHECK(h && k && part, "null pointer");
   HY_CHECK(groups == dec::ext_groups(R, D, t - b, n), "partials sized for %d groups; this extend needs %d "
            "(hyena_b200_decode_extend_groups with t - b)", groups, dec::ext_groups(R, D, t - b, n));
-  HY_CHECK(aligned16(k) && aligned16(h), "k and h must be 16-byte aligned");
+  HY_CHECK(aligned16(k) && hist_aligned(h), "%s", kAlignKH<T>);
   const int ld = dec::ld_for(Lcap), F = order - 1, NT = dec::ext_tile(n), j = t - b;
-  dec::ExtDotArgs a{h, k + (size_t)o * ld + (ld - H), part, R, D, j, n, H, F * ld, (-j) & 3, (n + NT - 1) / NT,
-                    dec::ext_chunks_per_cta(R, D, j, n), dec::chunks_for(j + n), groups};
+  dec::ExtDotArgsT<T> a{h, k + (size_t)o * ld + (ld - H), part, R, D, j, n, H, F * ld, (-j) & 3, (n + NT - 1) / NT,
+                        dec::ext_chunks_per_cta(R, D, j, n), dec::chunks_for(j + n), groups};
   HY_CUDA(launch_decode_ext_dot(a, (cudaStream_t)stream));
   return 0;
 }
 
-HY_API int hyena_b200_decode_branch_combine(const float* part, long long row_stride, int j_stride, int groups,
-                                            const float* fbias, const float* h, const float* s, float* out,
-                                            const float* f, const int* parent, int R, int D, int order, int o, int t,
-                                            int n, int b, int Hc, int H, int Lcap, void* stream) {
+template <class T>
+static int decode_branch_combine(const float* part, long long row_stride, int j_stride, int groups, const float* fbias,
+                                 const T* h, const float* s, void* out, const float* f, const int* parent, int R, int D,
+                                 int order, int o, int t, int n, int b, int Hc, int H, int Lcap, void* stream) {
   if (check_branch(R, D, order, o, t, n, b, Hc, H, Lcap)) return 1;
   HY_CHECK(part && fbias && h && s && out && f && parent, "null pointer");
   HY_CHECK(groups >= 1 && j_stride >= 0 && row_stride >= 0, "bad partial layout: groups %d, strides %lld / %d", groups,
            row_stride, j_stride);
+  if constexpr (!kFp32<T>)
+    HY_CHECK(elem_aligned(h) && elem_aligned(static_cast<T*>(out)),
+             "misaligned pointer: h and out must be 2-byte aligned");
   const int last = o == order - 2;
-  dec::BranchCombineArgs a{{part, row_stride, j_stride, groups, fbias + o, order - 1, h, s, last ? nullptr : out,
-                            last ? out : nullptr, R, D, (order + 1) * D, t - b, n, H, (order - 2 - o) * D, last},
-                           f, parent};
+  dec::BranchCombineArgsT<T> a{{part, row_stride, j_stride, groups, fbias + o, order - 1, h, s,
+                                last ? nullptr : static_cast<T*>(out), last ? static_cast<float*>(out) : nullptr, R, D,
+                                (order + 1) * D, t - b, n, H, (order - 2 - o) * D, last}, f, parent};
   HY_CUDA(launch_decode_branch_combine(a, (cudaStream_t)stream));
   return 0;
 }
 
 /* device-position steps (a step captured once in a CUDA graph): the kernels read pos = [t, win_b, base] */
+template <class T>
 static int check_dev_step(int o, int order, const float* p_t, const float* sw, const float* sb, const float* tail,
-                          const float* v_in, const float* k, const float* h, const int* pos) {
+                          const float* v_in, const float* k, const T* h, const int* pos) {
   HY_CHECK(o >= 0 && o < order - 1, "recurrence %d outside [0, %d)", o, order - 1);
   HY_CHECK(o == 0 ? (p_t && sw && sb && tail && !v_in) : (v_in != nullptr),
            o == 0 ? "null pointer: recurrence 0 needs p_t, sw, sb, tail (and no v_in)" : "null pointer: v_in");
   HY_CHECK(pos && (reinterpret_cast<uintptr_t>(pos) & 3u) == 0, "null or misaligned device position");
-  HY_CHECK(aligned16(k) && aligned16(h), "k and h must be 16-byte aligned");
+  HY_CHECK(aligned16(k) && hist_aligned(h), "%s", kAlignKH<T>);
   return 0;
 }
 
-HY_API int hyena_b200_decode_step_dev(const float* p_t, const float* in_bias, const float* sw, const float* sb,
-                                      const float* k, const float* fbias, float* h, float* tail, float* s_t,
-                                      const float* v_in, float* out, float* part, const int* pos, int B, int cache_B, int D,
-                                      int order, int o, int t_max, int Lcap, void* stream) {
+template <class T>
+static int decode_step_dev(const float* p_t, const float* in_bias, const float* sw, const float* sb, const float* k,
+                           const float* fbias, T* h, float* tail, float* s_t, const float* v_in, float* out,
+                           float* part, const int* pos, int B, int cache_B, int D, int order, int o, int t_max,
+                           int Lcap, void* stream) {
   if (check_decode_shape(B, cache_B, D, order, Lcap)) return 1;
   HY_CHECK(k && fbias && h && s_t && out && part, "null pointer");
   if (check_dev_step(o, order, p_t, sw, sb, tail, v_in, k, h, pos)) return 1;
   HY_CHECK(t_max >= 1 && t_max <= Lcap, "position bound %d outside [1, %d]", t_max, Lcap);
   const int ld = dec::ld_for(Lcap), F = order - 1;
-  dec::DotArgs dot{h, k + (size_t)o * ld, part, B, D, 0, ld, F * ld, dec::chunks_for(Lcap)};
-  dec::StepArgs st{part, 0, dec::chunks_for(Lcap), k + (size_t)o * ld, fbias + o, F * ld, F, ld, p_t, in_bias, sw, sb, tail,
-                   s_t, v_in, h, out, B, D, (order + 1) * D, order, 0, (order - 1 - o) * D, o == order - 2};
+  dec::DotArgsT<T> dot{h, k + (size_t)o * ld, part, B, D, 0, ld, F * ld, dec::chunks_for(Lcap)};
+  dec::StepArgsT<T> st{part, 0, dec::chunks_for(Lcap), k + (size_t)o * ld, fbias + o, F * ld, F, ld, p_t, in_bias, sw,
+                       sb, tail, s_t, v_in, h, out, B, D, (order + 1) * D, order, 0, (order - 1 - o) * D,
+                       o == order - 2};
   HY_CUDA(launch_decode_step_dev(dot, st, pos, dec::chunks_for(t_max), (cudaStream_t)stream));
   return 0;
 }
 
-HY_API int hyena_b200_decode_win_step_dev(const float* p_t, const float* in_bias, const float* sw, const float* sb,
-                                          const float* k, const float* fbias, float* h, float* tail, float* s_t,
-                                          const float* v_in, float* out, float* part, const float* win, const int* pos, int B,
-                                          int cache_B, int D, int order, int o, int W, int Lcap, void* stream) {
+template <class T>
+static int decode_win_step_dev(const float* p_t, const float* in_bias, const float* sw, const float* sb, const float* k,
+                               const float* fbias, T* h, float* tail, float* s_t, const float* v_in, float* out,
+                               float* part, const float* win, const int* pos, int B, int cache_B, int D, int order,
+                               int o, int W, int Lcap, void* stream) {
   if (check_decode_shape(B, cache_B, D, order, Lcap)) return 1;
   HY_CHECK(k && fbias && h && s_t && out && part && win, "null pointer");
   if (check_dev_step(o, order, p_t, sw, sb, tail, v_in, k, h, pos)) return 1;
   HY_CHECK(W >= 1 && W <= Lcap, "window width %d outside [1, %d]", W, Lcap);
   const int ld = dec::ld_for(Lcap), F = order - 1;
-  dec::DotArgs dot{h, k + (size_t)o * ld, part, B, D, 0, ld, F * ld, dec::chunks_for(Lcap)};
-  dec::WinStepArgs w{{part, 0, dec::chunks_for(Lcap), k + (size_t)o * ld, fbias + o, F * ld, F, ld, p_t, in_bias, sw, sb,
-                      tail, s_t, v_in, h, out, B, D, (order + 1) * D, order, 0, (order - 1 - o) * D, o == order - 2},
-                     win, W, 0};
+  dec::DotArgsT<T> dot{h, k + (size_t)o * ld, part, B, D, 0, ld, F * ld, dec::chunks_for(Lcap)};
+  dec::WinStepArgsT<T> w{{part, 0, dec::chunks_for(Lcap), k + (size_t)o * ld, fbias + o, F * ld, F, ld, p_t, in_bias,
+                          sw, sb, tail, s_t, v_in, h, out, B, D, (order + 1) * D, order, 0, (order - 1 - o) * D,
+                          o == order - 2}, win, W, 0};
   HY_CUDA(launch_decode_win_step_dev(dot, w, pos, dec::chunks_for(W), (cudaStream_t)stream));
   return 0;
 }
 
-HY_API int hyena_b200_decode_branch_step_dev(const float* p_t, const float* in_bias, const float* sw, const float* sb,
-                                             const float* k, const float* fbias, float* h, float* tail, float* s_t,
-                                             const float* v_in, float* out, float* part, const float* f, const int* parent,
-                                             const int* pos, int R, int D, int order, int o, int H, int Lcap, void* stream) {
+template <class T>
+static int decode_branch_step_dev(const float* p_t, const float* in_bias, const float* sw, const float* sb,
+                                  const float* k, const float* fbias, T* h, float* tail, float* s_t, const float* v_in,
+                                  float* out, float* part, const float* f, const int* parent, const int* pos, int R,
+                                  int D, int order, int o, int H, int Lcap, void* stream) {
   if (check_decode_shape(R, R, D, order, Lcap)) return 1;
   HY_CHECK(k && fbias && h && s_t && out && part && f && parent, "null pointer");
   if (check_dev_step(o, order, p_t, sw, sb, tail, v_in, k, h, pos)) return 1;
   const int ld = dec::ld_for(Lcap), F = order - 1;
   HY_CHECK((H & 3) == 0 && H >= 4 && H <= ld, "branch history width %d must be a multiple of 4 in [4, %d]", H, ld);
   const float* kb = k + (size_t)o * ld + (ld - H);
-  dec::DotArgs dot{h, kb, part, R, D, 0, H, F * ld, dec::chunks_for(H)};
-  dec::BranchStepArgs w{{part, 0, dec::chunks_for(H), kb, fbias + o, F * ld, F, H, p_t, in_bias, sw, sb, tail, s_t, v_in, h,
-                         out, R, D, (order + 1) * D, order, 0, (order - 1 - o) * D, o == order - 2},
-                        f, parent};
+  dec::DotArgsT<T> dot{h, kb, part, R, D, 0, H, F * ld, dec::chunks_for(H)};
+  dec::BranchStepArgsT<T> w{{part, 0, dec::chunks_for(H), kb, fbias + o, F * ld, F, H, p_t, in_bias, sw, sb, tail, s_t,
+                             v_in, h, out, R, D, (order + 1) * D, order, 0, (order - 1 - o) * D, o == order - 2}, f,
+                            parent};
   HY_CUDA(launch_decode_branch_step_dev(dot, w, pos, dec::chunks_for(H), (cudaStream_t)stream));
   return 0;
 }
@@ -1114,6 +1150,265 @@ HY_API int hyena_b200_decode_pos_advance(int* pos, void* stream) {
   HY_CHECK(pos && (reinterpret_cast<uintptr_t>(pos) & 3u) == 0, "null or misaligned device position");
   HY_CUDA(launch_decode_pos_advance(pos, (cudaStream_t)stream));
   return 0;
+}
+
+/* ---- the C entry points of the decoding kernels: fp32 history (hyena_b200_decode_*) and 16-bit history
+   (hyena_b200_decode_*_h16, the same arguments after a history dtype code; include/hyena_b200.h) */
+template <class F>
+static int with_hist_type(int hist_dtype, F&& f) {
+  if (hist_dtype == HYENA_B200_HIST_F16) return f(__half());
+  if (hist_dtype == HYENA_B200_HIST_BF16) return f(__nv_bfloat16());
+  return fail("unknown history dtype code %d (%d: fp16, %d: bf16; an fp32 history uses the entry points without _h16)",
+              hist_dtype, HYENA_B200_HIST_F16, HYENA_B200_HIST_BF16);
+}
+
+extern "C" {
+
+HY_API int hyena_b200_decode_hist(const float* p, const float* in_bias, const float* sw, const float* sb, float* h,
+                                  float* tail, int B, int cache_B, int D, int order, int P, int Lcap, void* stream) {
+  return decode_hist<float>(p, in_bias, sw, sb, h, tail, B, cache_B, D, order, P, Lcap, stream);
+}
+HY_API int hyena_b200_decode_hist_h16(int hist_dtype, const float* p, const float* in_bias, const float* sw,
+                                      const float* sb, void* h, float* tail, int B, int cache_B, int D, int order,
+                                      int P, int Lcap, void* stream) {
+  return with_hist_type(hist_dtype, [&](auto tag) { using T = decltype(tag);
+    return decode_hist<T>(p, in_bias, sw, sb, static_cast<T*>(h), tail, B, cache_B, D, order, P, Lcap, stream);
+  });
+}
+
+HY_API int hyena_b200_decode_hist_rows(const float* p, const float* in_bias, const float* sw, const float* sb, float* h,
+                                       float* tail, const int* row_start, int B, int cache_B, int D, int order, int P,
+                                       int Lcap, void* stream) {
+  return decode_hist_rows<float>(p, in_bias, sw, sb, h, tail, row_start, B, cache_B, D, order, P, Lcap, stream);
+}
+HY_API int hyena_b200_decode_hist_rows_h16(int hist_dtype, const float* p, const float* in_bias, const float* sw,
+                                           const float* sb, void* h, float* tail, const int* row_start, int B,
+                                           int cache_B, int D, int order, int P, int Lcap, void* stream) {
+  return with_hist_type(hist_dtype, [&](auto tag) { using T = decltype(tag);
+    return decode_hist_rows<T>(p, in_bias, sw, sb, static_cast<T*>(h), tail, row_start, B, cache_B, D, order, P, Lcap,
+                               stream);
+  });
+}
+
+HY_API int hyena_b200_decode_admit(const float* p, const float* in_bias, const float* sw, const float* sb, float* h,
+                                   float* tail, const int* rows, const int* row_start, int k, int cache_B, int D,
+                                   int order, int P, int t, int Lcap, void* stream) {
+  return decode_admit<float>(p, in_bias, sw, sb, h, tail, rows, row_start, k, cache_B, D, order, P, t, Lcap, stream);
+}
+HY_API int hyena_b200_decode_admit_h16(int hist_dtype, const float* p, const float* in_bias, const float* sw,
+                                       const float* sb, void* h, float* tail, const int* rows, const int* row_start,
+                                       int k, int cache_B, int D, int order, int P, int t, int Lcap, void* stream) {
+  return with_hist_type(hist_dtype, [&](auto tag) { using T = decltype(tag);
+    return decode_admit<T>(p, in_bias, sw, sb, static_cast<T*>(h), tail, rows, row_start, k, cache_B, D, order, P, t,
+                           Lcap, stream);
+  });
+}
+
+HY_API int hyena_b200_decode_shift(float* h, int B, int D, int order, int t, int shift, int Lcap, void* stream) {
+  return decode_shift<float>(h, B, D, order, t, shift, Lcap, stream);
+}
+HY_API int hyena_b200_decode_shift_h16(int hist_dtype, void* h, int B, int D, int order, int t, int shift, int Lcap,
+                                       void* stream) {
+  return with_hist_type(hist_dtype, [&](auto tag) { using T = decltype(tag);
+    return decode_shift<T>(static_cast<T*>(h), B, D, order, t, shift, Lcap, stream);
+  });
+}
+
+HY_API int hyena_b200_decode_step(const float* p_t, const float* in_bias, const float* sw, const float* sb,
+                                  const float* k, const float* fbias, float* h, float* tail, float* s_t,
+                                  const float* v_in, float* out, float* part, int B, int cache_B, int D, int order,
+                                  int o, int t, int Lcap, void* stream) {
+  return decode_step<float>(p_t, in_bias, sw, sb, k, fbias, h, tail, s_t, v_in, out, part, B, cache_B, D, order, o, t,
+                            Lcap, stream);
+}
+HY_API int hyena_b200_decode_step_h16(int hist_dtype, const float* p_t, const float* in_bias, const float* sw,
+                                      const float* sb, const float* k, const float* fbias, void* h, float* tail,
+                                      float* s_t, const float* v_in, float* out, float* part, int B, int cache_B, int D,
+                                      int order, int o, int t, int Lcap, void* stream) {
+  return with_hist_type(hist_dtype, [&](auto tag) { using T = decltype(tag);
+    return decode_step<T>(p_t, in_bias, sw, sb, k, fbias, static_cast<T*>(h), tail, s_t, v_in, out, part, B, cache_B, D,
+                          order, o, t, Lcap, stream);
+  });
+}
+
+HY_API int hyena_b200_decode_win_step(const float* p_t, const float* in_bias, const float* sw, const float* sb,
+                                      const float* k, const float* fbias, float* h, float* tail, float* s_t,
+                                      const float* v_in, float* out, float* part, const float* win, int B, int cache_B,
+                                      int D, int order, int o, int t, int b, int Wc, int W, int Lcap, void* stream) {
+  return decode_win_step<float>(p_t, in_bias, sw, sb, k, fbias, h, tail, s_t, v_in, out, part, win, B, cache_B, D,
+                                order, o, t, b, Wc, W, Lcap, stream);
+}
+HY_API int hyena_b200_decode_win_step_h16(int hist_dtype, const float* p_t, const float* in_bias, const float* sw,
+                                          const float* sb, const float* k, const float* fbias, void* h, float* tail,
+                                          float* s_t, const float* v_in, float* out, float* part, const float* win,
+                                          int B, int cache_B, int D, int order, int o, int t, int b, int Wc, int W,
+                                          int Lcap, void* stream) {
+  return with_hist_type(hist_dtype, [&](auto tag) { using T = decltype(tag);
+    return decode_win_step<T>(p_t, in_bias, sw, sb, k, fbias, static_cast<T*>(h), tail, s_t, v_in, out, part, win, B,
+                              cache_B, D, order, o, t, b, Wc, W, Lcap, stream);
+  });
+}
+
+HY_API int hyena_b200_decode_extend_hist(const float* p, const float* in_bias, const float* sw, const float* sb,
+                                         float* h, float* tail, float* s, int B, int cache_B, int D, int order, int t,
+                                         int n, int Lcap, void* stream) {
+  return decode_extend_hist<float>(p, in_bias, sw, sb, h, tail, s, B, cache_B, D, order, t, n, Lcap, stream);
+}
+HY_API int hyena_b200_decode_extend_hist_h16(int hist_dtype, const float* p, const float* in_bias, const float* sw,
+                                             const float* sb, void* h, float* tail, float* s, int B, int cache_B, int D,
+                                             int order, int t, int n, int Lcap, void* stream) {
+  return with_hist_type(hist_dtype, [&](auto tag) { using T = decltype(tag);
+    return decode_extend_hist<T>(p, in_bias, sw, sb, static_cast<T*>(h), tail, s, B, cache_B, D, order, t, n, Lcap,
+                                 stream);
+  });
+}
+
+HY_API int hyena_b200_decode_extend_dot(const float* h, const float* k, float* part, int groups, int B, int cache_B,
+                                        int D, int order, int o, int t, int n, int Lcap, void* stream) {
+  return decode_extend_dot<float>(h, k, part, groups, B, cache_B, D, order, o, t, n, Lcap, stream);
+}
+HY_API int hyena_b200_decode_extend_dot_h16(int hist_dtype, const void* h, const float* k, float* part, int groups,
+                                            int B, int cache_B, int D, int order, int o, int t, int n, int Lcap,
+                                            void* stream) {
+  return with_hist_type(hist_dtype, [&](auto tag) { using T = decltype(tag);
+    return decode_extend_dot<T>(static_cast<const T*>(h), k, part, groups, B, cache_B, D, order, o, t, n, Lcap, stream);
+  });
+}
+
+HY_API int hyena_b200_decode_extend_combine(const float* part, long long row_stride, int j_stride, int groups,
+                                            const float* fbias, const float* h, const float* s, float* out, int B,
+                                            int cache_B, int D, int order, int o, int t, int n, int Lcap,
+                                            void* stream) {
+  return decode_extend_combine<float>(part, row_stride, j_stride, groups, fbias, h, s, out, B, cache_B, D, order, o, t,
+                                      n, Lcap, stream);
+}
+HY_API int hyena_b200_decode_extend_combine_h16(int hist_dtype, const float* part, long long row_stride, int j_stride,
+                                                int groups, const float* fbias, const void* h, const float* s,
+                                                void* out, int B, int cache_B, int D, int order, int o, int t, int n,
+                                                int Lcap, void* stream) {
+  return with_hist_type(hist_dtype, [&](auto tag) { using T = decltype(tag);
+    return decode_extend_combine<T>(part, row_stride, j_stride, groups, fbias, static_cast<const T*>(h), s, out, B,
+                                    cache_B, D, order, o, t, n, Lcap, stream);
+  });
+}
+
+HY_API int hyena_b200_decode_branch_step(const float* p_t, const float* in_bias, const float* sw, const float* sb,
+                                         const float* k, const float* fbias, float* h, float* tail, float* s_t,
+                                         const float* v_in, float* out, float* part, const float* f, const int* parent,
+                                         int R, int D, int order, int o, int t, int b, int Hc, int H, int Lcap,
+                                         void* stream) {
+  return decode_branch_step<float>(p_t, in_bias, sw, sb, k, fbias, h, tail, s_t, v_in, out, part, f, parent, R, D,
+                                   order, o, t, b, Hc, H, Lcap, stream);
+}
+HY_API int hyena_b200_decode_branch_step_h16(int hist_dtype, const float* p_t, const float* in_bias, const float* sw,
+                                             const float* sb, const float* k, const float* fbias, void* h, float* tail,
+                                             float* s_t, const float* v_in, float* out, float* part, const float* f,
+                                             const int* parent, int R, int D, int order, int o, int t, int b, int Hc,
+                                             int H, int Lcap, void* stream) {
+  return with_hist_type(hist_dtype, [&](auto tag) { using T = decltype(tag);
+    return decode_branch_step<T>(p_t, in_bias, sw, sb, k, fbias, static_cast<T*>(h), tail, s_t, v_in, out, part, f,
+                                 parent, R, D, order, o, t, b, Hc, H, Lcap, stream);
+  });
+}
+
+HY_API int hyena_b200_decode_branch_extend_hist(const float* p, const float* in_bias, const float* sw, const float* sb,
+                                                float* h, float* tail, float* s, int R, int D, int order, int t, int n,
+                                                int b, int Hc, int H, int Lcap, void* stream) {
+  return decode_branch_extend_hist<float>(p, in_bias, sw, sb, h, tail, s, R, D, order, t, n, b, Hc, H, Lcap, stream);
+}
+HY_API int hyena_b200_decode_branch_extend_hist_h16(int hist_dtype, const float* p, const float* in_bias,
+                                                    const float* sw, const float* sb, void* h, float* tail, float* s,
+                                                    int R, int D, int order, int t, int n, int b, int Hc, int H,
+                                                    int Lcap, void* stream) {
+  return with_hist_type(hist_dtype, [&](auto tag) { using T = decltype(tag);
+    return decode_branch_extend_hist<T>(p, in_bias, sw, sb, static_cast<T*>(h), tail, s, R, D, order, t, n, b, Hc, H,
+                                        Lcap, stream);
+  });
+}
+
+HY_API int hyena_b200_decode_branch_extend_dot(const float* h, const float* k, float* part, int groups, int R, int D,
+                                               int order, int o, int t, int n, int b, int Hc, int H, int Lcap,
+                                               void* stream) {
+  return decode_branch_extend_dot<float>(h, k, part, groups, R, D, order, o, t, n, b, Hc, H, Lcap, stream);
+}
+HY_API int hyena_b200_decode_branch_extend_dot_h16(int hist_dtype, const void* h, const float* k, float* part,
+                                                   int groups, int R, int D, int order, int o, int t, int n, int b,
+                                                   int Hc, int H, int Lcap, void* stream) {
+  return with_hist_type(hist_dtype, [&](auto tag) { using T = decltype(tag);
+    return decode_branch_extend_dot<T>(static_cast<const T*>(h), k, part, groups, R, D, order, o, t, n, b, Hc, H, Lcap,
+                                       stream);
+  });
+}
+
+HY_API int hyena_b200_decode_branch_combine(const float* part, long long row_stride, int j_stride, int groups,
+                                            const float* fbias, const float* h, const float* s, float* out,
+                                            const float* f, const int* parent, int R, int D, int order, int o, int t,
+                                            int n, int b, int Hc, int H, int Lcap, void* stream) {
+  return decode_branch_combine<float>(part, row_stride, j_stride, groups, fbias, h, s, out, f, parent, R, D, order, o,
+                                      t, n, b, Hc, H, Lcap, stream);
+}
+HY_API int hyena_b200_decode_branch_combine_h16(int hist_dtype, const float* part, long long row_stride, int j_stride,
+                                                int groups, const float* fbias, const void* h, const float* s,
+                                                void* out, const float* f, const int* parent, int R, int D, int order,
+                                                int o, int t, int n, int b, int Hc, int H, int Lcap, void* stream) {
+  return with_hist_type(hist_dtype, [&](auto tag) { using T = decltype(tag);
+    return decode_branch_combine<T>(part, row_stride, j_stride, groups, fbias, static_cast<const T*>(h), s, out, f,
+                                    parent, R, D, order, o, t, n, b, Hc, H, Lcap, stream);
+  });
+}
+
+HY_API int hyena_b200_decode_step_dev(const float* p_t, const float* in_bias, const float* sw, const float* sb,
+                                      const float* k, const float* fbias, float* h, float* tail, float* s_t,
+                                      const float* v_in, float* out, float* part, const int* pos, int B, int cache_B,
+                                      int D, int order, int o, int t_max, int Lcap, void* stream) {
+  return decode_step_dev<float>(p_t, in_bias, sw, sb, k, fbias, h, tail, s_t, v_in, out, part, pos, B, cache_B, D,
+                                order, o, t_max, Lcap, stream);
+}
+HY_API int hyena_b200_decode_step_dev_h16(int hist_dtype, const float* p_t, const float* in_bias, const float* sw,
+                                          const float* sb, const float* k, const float* fbias, void* h, float* tail,
+                                          float* s_t, const float* v_in, float* out, float* part, const int* pos, int B,
+                                          int cache_B, int D, int order, int o, int t_max, int Lcap, void* stream) {
+  return with_hist_type(hist_dtype, [&](auto tag) { using T = decltype(tag);
+    return decode_step_dev<T>(p_t, in_bias, sw, sb, k, fbias, static_cast<T*>(h), tail, s_t, v_in, out, part, pos, B,
+                              cache_B, D, order, o, t_max, Lcap, stream);
+  });
+}
+
+HY_API int hyena_b200_decode_win_step_dev(const float* p_t, const float* in_bias, const float* sw, const float* sb,
+                                          const float* k, const float* fbias, float* h, float* tail, float* s_t,
+                                          const float* v_in, float* out, float* part, const float* win, const int* pos,
+                                          int B, int cache_B, int D, int order, int o, int W, int Lcap, void* stream) {
+  return decode_win_step_dev<float>(p_t, in_bias, sw, sb, k, fbias, h, tail, s_t, v_in, out, part, win, pos, B, cache_B,
+                                    D, order, o, W, Lcap, stream);
+}
+HY_API int hyena_b200_decode_win_step_dev_h16(int hist_dtype, const float* p_t, const float* in_bias, const float* sw,
+                                              const float* sb, const float* k, const float* fbias, void* h, float* tail,
+                                              float* s_t, const float* v_in, float* out, float* part, const float* win,
+                                              const int* pos, int B, int cache_B, int D, int order, int o, int W,
+                                              int Lcap, void* stream) {
+  return with_hist_type(hist_dtype, [&](auto tag) { using T = decltype(tag);
+    return decode_win_step_dev<T>(p_t, in_bias, sw, sb, k, fbias, static_cast<T*>(h), tail, s_t, v_in, out, part, win,
+                                  pos, B, cache_B, D, order, o, W, Lcap, stream);
+  });
+}
+
+HY_API int hyena_b200_decode_branch_step_dev(const float* p_t, const float* in_bias, const float* sw, const float* sb,
+                                             const float* k, const float* fbias, float* h, float* tail, float* s_t,
+                                             const float* v_in, float* out, float* part, const float* f,
+                                             const int* parent, const int* pos, int R, int D, int order, int o, int H,
+                                             int Lcap, void* stream) {
+  return decode_branch_step_dev<float>(p_t, in_bias, sw, sb, k, fbias, h, tail, s_t, v_in, out, part, f, parent, pos, R,
+                                       D, order, o, H, Lcap, stream);
+}
+HY_API int hyena_b200_decode_branch_step_dev_h16(int hist_dtype, const float* p_t, const float* in_bias,
+                                                 const float* sw, const float* sb, const float* k, const float* fbias,
+                                                 void* h, float* tail, float* s_t, const float* v_in, float* out,
+                                                 float* part, const float* f, const int* parent, const int* pos, int R,
+                                                 int D, int order, int o, int H, int Lcap, void* stream) {
+  return with_hist_type(hist_dtype, [&](auto tag) { using T = decltype(tag);
+    return decode_branch_step_dev<T>(p_t, in_bias, sw, sb, k, fbias, static_cast<T*>(h), tail, s_t, v_in, out, part, f,
+                                     parent, pos, R, D, order, o, H, Lcap, stream);
+  });
 }
 
 }  // extern "C"

@@ -18,7 +18,9 @@
 //                          its own history from b on, and F is read from the row of the branch's parent
 //   *_dev_kernel           the same steps with the position read on the device (decode_args.h DevPos), for a step captured
 //                          once in a CUDA graph and replayed at every position; decode_pos_advance_kernel moves it
-// fp32 throughout, no atomics: every sum has a fixed order, so a step is bitwise reproducible.
+// fp32 arithmetic, no atomics: every sum has a fixed order, so a step is bitwise reproducible.  Every kernel that reads or
+// writes the history is a template over its element type T (float, __half, __nv_bfloat16; decode_args.h): a value is
+// rounded once when it is stored, g^ = round(g), and every read and the step's own s = t term use g^ widened to fp32.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -32,8 +34,8 @@ namespace dec {
 // ROWS: row b is left-padded, its positions t < s = row_start[b] read as the short filter's padding before t = 0 (0, no
 // in_proj bias): g is 0 there, and a pad position in the tail is 0.
 // Grid: (B * D rows, up to 64 position CTAs per row); the rows go on x, which has no 65535 limit.
-template <bool ROWS>
-__device__ __forceinline__ void hist_body(const HistArgs& a) {
+template <bool ROWS, class T>
+__device__ __forceinline__ void hist_body(const HistArgsT<T>& a) {
   const int row = blockIdx.x;                    // b * D + d
   const int b = row / a.D, d = row - b * a.D;
   const int s = ROWS ? __ldg(a.row_start + b) : 0;
@@ -43,17 +45,17 @@ __device__ __forceinline__ void hist_body(const HistArgs& a) {
   const float ibv = a.in_bias ? __ldg(a.in_bias + cv) : 0.f, ibg = a.in_bias ? __ldg(a.in_bias + cg) : 0.f;
   const float v0 = __ldg(a.sw + 3 * cv), v1 = __ldg(a.sw + 3 * cv + 1), v2 = __ldg(a.sw + 3 * cv + 2), vb = __ldg(a.sb + cv);
   const float g0 = __ldg(a.sw + 3 * cg), g1 = __ldg(a.sw + 3 * cg + 1), g2 = __ldg(a.sw + 3 * cg + 2), gb = __ldg(a.sb + cg);
-  float* h = a.h + (size_t)row * a.ld;
+  T* h = a.h + (size_t)row * a.ld;
   for (int t = blockIdx.y * blockDim.x + threadIdx.x; t < a.P; t += gridDim.y * blockDim.x) {
     if (ROWS) {
-      if (t < s) { h[t] = 0.f; continue; }
+      if (t < s) { h[t] = hround<T>(0.f); continue; }
       const float vm2 = t - 2 >= s ? pv[t - 2] + ibv : 0.f, vm1 = t - 1 >= s ? pv[t - 1] + ibv : 0.f, vp = pv[t] + ibv;
       const float gm2 = t - 2 >= s ? pg[t - 2] + ibg : 0.f, gm1 = t - 1 >= s ? pg[t - 1] + ibg : 0.f, gp = pg[t] + ibg;
-      h[t] = short3(v0, v1, v2, vb, vm2, vm1, vp) * short3(g0, g1, g2, gb, gm2, gm1, gp);
+      h[t] = hround<T>(short3(v0, v1, v2, vb, vm2, vm1, vp) * short3(g0, g1, g2, gb, gm2, gm1, gp));
     } else {
       const float vm2 = t >= 2 ? pv[t - 2] + ibv : 0.f, vm1 = t >= 1 ? pv[t - 1] + ibv : 0.f, vp = pv[t] + ibv;
       const float gm2 = t >= 2 ? pg[t - 2] + ibg : 0.f, gm1 = t >= 1 ? pg[t - 1] + ibg : 0.f, gp = pg[t] + ibg;
-      h[t] = short3(v0, v1, v2, vb, vm2, vm1, vp) * short3(g0, g1, g2, gb, gm2, gm1, gp);
+      h[t] = hround<T>(short3(v0, v1, v2, vb, vm2, vm1, vp) * short3(g0, g1, g2, gb, gm2, gm1, gp));
     }
   }
   // tail of channels d, D + d, ..., O D + d (one thread each, first CTA of the row)
@@ -68,8 +70,10 @@ __device__ __forceinline__ void hist_body(const HistArgs& a) {
   }
 }
 
-__global__ void __launch_bounds__(256) decode_hist_kernel(const HistArgs a) { hist_body<false>(a); }
-__global__ void __launch_bounds__(256) decode_hist_rows_kernel(const HistArgs a) { hist_body<true>(a); }
+template <class T>
+__global__ void __launch_bounds__(256) decode_hist_kernel(const HistArgsT<T> a) { hist_body<false>(a); }
+template <class T>
+__global__ void __launch_bounds__(256) decode_hist_rows_kernel(const HistArgsT<T> a) { hist_body<true>(a); }
 
 // Admission of prompt i into cache row rows[i] at the placement offset off = t - P (AdmitArgs): the arithmetic of hist_body
 // on the prompt's positions j = tau - off, written at cache positions tau in [off, t), and 0 at tau < off + s (s the prompt's
@@ -77,8 +81,9 @@ __global__ void __launch_bounds__(256) decode_hist_rows_kernel(const HistArgs a)
 // before its first real position decodes like the unpadded prompt (time invariance, DESIGN.md section 4.15).  The tail of
 // all C channels of row rows[i] is the prompt's last two positions, a pad position there 0.
 // Grid: (k * D rows, up to 64 position CTAs per row); the rows go on x, which has no 65535 limit.
-__global__ void __launch_bounds__(256) decode_admit_kernel(const AdmitArgs w) {
-  const HistArgs& a = w.hist;
+template <class T>
+__global__ void __launch_bounds__(256) decode_admit_kernel(const AdmitArgsT<T> w) {
+  const HistArgsT<T>& a = w.hist;
   const int row = blockIdx.x;                    // i * D + d
   const int i = row / a.D, d = row - i * a.D;
   const int s = a.row_start ? __ldg(a.row_start + i) : 0;
@@ -90,13 +95,13 @@ __global__ void __launch_bounds__(256) decode_admit_kernel(const AdmitArgs w) {
   const float ibv = a.in_bias ? __ldg(a.in_bias + cv) : 0.f, ibg = a.in_bias ? __ldg(a.in_bias + cg) : 0.f;
   const float v0 = __ldg(a.sw + 3 * cv), v1 = __ldg(a.sw + 3 * cv + 1), v2 = __ldg(a.sw + 3 * cv + 2), vb = __ldg(a.sb + cv);
   const float g0 = __ldg(a.sw + 3 * cg), g1 = __ldg(a.sw + 3 * cg + 1), g2 = __ldg(a.sw + 3 * cg + 2), gb = __ldg(a.sb + cg);
-  float* h = a.h + ((size_t)r * a.D + d) * a.ld;
+  T* h = a.h + ((size_t)r * a.D + d) * a.ld;
   for (int t = blockIdx.y * blockDim.x + threadIdx.x; t < w.t; t += gridDim.y * blockDim.x) {
-    if (t < s0) { h[t] = 0.f; continue; }
+    if (t < s0) { h[t] = hround<T>(0.f); continue; }
     const int j = t - w.off;
     const float vm2 = j - 2 >= s ? pv[j - 2] + ibv : 0.f, vm1 = j - 1 >= s ? pv[j - 1] + ibv : 0.f, vp = pv[j] + ibv;
     const float gm2 = j - 2 >= s ? pg[j - 2] + ibg : 0.f, gm1 = j - 1 >= s ? pg[j - 1] + ibg : 0.f, gp = pg[j] + ibg;
-    h[t] = short3(v0, v1, v2, vb, vm2, vm1, vp) * short3(g0, g1, g2, gb, gm2, gm1, gp);
+    h[t] = hround<T>(short3(v0, v1, v2, vb, vm2, vm1, vp) * short3(g0, g1, g2, gb, gm2, gm1, gp));
   }
   // tail of channels d, D + d, ..., O D + d (one thread each, first CTA of the row)
   const int nj = a.C / a.D;
@@ -110,16 +115,18 @@ __global__ void __launch_bounds__(256) decode_admit_kernel(const AdmitArgs w) {
   }
 }
 
-// In-place shift of one history row per CTA (ShiftArgs) over the float4s of [0, round4(t)); shift is a multiple of 4, so
-// whole float4s move.  Left (shift = -m): h[tau] = h[tau + m], tiles in ascending order.  Right (shift = d): h[tau + d] =
+// In-place shift of one history row per CTA (ShiftArgs) over the 4-position vectors V of [0, round4(t)) (a float4, or 8
+// bytes of a 16-bit history); shift is a multiple of 4, so whole vectors move.  Left (shift = -m): h[tau] = h[tau + m], tiles in ascending order.  Right (shift = d): h[tau + d] =
 // h[tau], tiles in descending order, then [0, d) zeroed.  Each tile's loads complete (__syncthreads) before its stores, and
 // no later tile reads a word an earlier tile stored (left: later tiles read above every earlier destination; right: below
 // it), so the shift is race-free without a scratch copy.  Plain loads: the row is written in place (no read-only path).
-__global__ void __launch_bounds__(kShiftThreads) decode_shift_kernel(const ShiftArgs a) {
-  float4* h = reinterpret_cast<float4*>(a.h + (size_t)blockIdx.x * a.ld);
+template <class T>
+__global__ void __launch_bounds__(kShiftThreads) decode_shift_kernel(const ShiftArgsT<T> a) {
+  using V = typename HVec4<T>::type;
+  V* h = reinterpret_cast<V*>(a.h + (size_t)blockIdx.x * a.ld);
   const int n4 = (a.t + 3) >> 2;
   constexpr int kTile = kShiftThreads * kShiftVec;
-  float4 v[kShiftVec];
+  V v[kShiftVec];
   if (a.shift < 0) {
     const int m4 = (-a.shift) >> 2, w4 = n4 - m4;          // destinations [0, w4) <- sources [m4, n4)
     for (int q0 = 0; q0 < w4; q0 += kTile) {
@@ -151,13 +158,13 @@ __global__ void __launch_bounds__(kShiftThreads) decode_shift_kernel(const Shift
       }
     }
     // every load happened before the last tile's barrier, and the stores went to [d4, d4 + n4): [0, d4) is free
-    for (int q = threadIdx.x; q < d4; q += kShiftThreads) h[q] = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int q = threadIdx.x; q < d4; q += kShiftThreads) h[q] = V{};
   }
 }
 
 // part[b][d][chunk] = sum_{s in chunk, s < t} h[b][d][s] k[t-s]   for the batch rows [z*BG, z*BG + BG)
-template <int BG, int R>
-__device__ __forceinline__ void dot_body(const DotArgs a) {
+template <int BG, int R, class T>
+__device__ __forceinline__ void dot_body(const DotArgsT<T> a) {
   const int lane = threadIdx.x & 31;
   const int d = blockIdx.y * kDotWarps + (threadIdx.x >> 5);
   if (d >= a.D) return;
@@ -184,7 +191,7 @@ __device__ __forceinline__ void dot_body(const DotArgs a) {
       for (int i = 0; i < BG; ++i) {
         const int b = b0 + i;
         if (b < a.B) {
-          float4 hv = ld4(a.h + ((size_t)b * a.D + d) * a.ld + s0);
+          float4 hv = hld4(a.h + ((size_t)b * a.D + d) * a.ld + s0);
           if (!full) {                           // positions >= t hold no history yet
             hv.y = s0 + 1 < a.t ? hv.y : 0.f;
             hv.z = s0 + 2 < a.t ? hv.z : 0.f;
@@ -208,13 +215,13 @@ __device__ __forceinline__ void dot_body(const DotArgs a) {
   }
 }
 
-template <int BG, int R>
-__global__ void __launch_bounds__(32 * kDotWarps) decode_dot_kernel(const DotArgs a) { dot_body<BG, R>(a); }
+template <int BG, int R, class T>
+__global__ void __launch_bounds__(32 * kDotWarps) decode_dot_kernel(const DotArgsT<T> a) { dot_body<BG, R>(a); }
 
 // decode_dot_kernel with t (and the history offset) read from the device position: the grid covers a fixed chunk bound and
 // the CTAs of chunks at or past t leave at once (the combine reads only the ceil(t / kChunk) partials below them)
-template <int BG>
-__global__ void __launch_bounds__(32 * kDotWarps) decode_dot_dev_kernel(DotArgs a, const DevPos p) {
+template <int BG, class T>
+__global__ void __launch_bounds__(32 * kDotWarps) decode_dot_dev_kernel(DotArgsT<T> a, const DevPos p) {
   const int t0 = p.pos[0];
   const int off = p.mode == kPosWindow ? p.pos[1] : p.mode == kPosBranch ? p.pos[2] : 0;
   a.t = t0 - off;
@@ -229,7 +236,8 @@ __global__ void __launch_bounds__(32 * kDotWarps) decode_dot_dev_kernel(DotArgs 
 }
 
 // fixed-order reduction of the chunk partials of one (b, channel) row: lane-strided chains, then a butterfly
-__device__ __forceinline__ float reduce_partials(const StepArgs& a, int row, int lane) {
+template <class T>
+__device__ __forceinline__ float reduce_partials(const StepArgsT<T>& a, int row, int lane) {
   float acc = 0.f;
   const float* part = a.part + (size_t)row * a.nchunk_max;
   for (int i = lane; i < a.nchunk; i += 32) acc += part[i];
@@ -238,8 +246,10 @@ __device__ __forceinline__ float reduce_partials(const StepArgs& a, int row, int
   return acc;
 }
 
-// everything of a step at position t once acc = sum_{s<t} k[t-s] g[s] is known (one warp per (b, channel) row)
-__device__ __forceinline__ void step_epilogue(const StepArgs& a, int row, int b, int d, int lane, float acc) {
+// everything of a step at position t once acc = sum_{s<t} k[t-s] g[s] is known (one warp per (b, channel) row); the
+// s = t term and the bias use the stored g^[t], as every later read of it does
+template <class T>
+__device__ __forceinline__ void step_epilogue(const StepArgsT<T>& a, int row, int b, int d, int lane, float acc) {
   float v, gate, x0;
   if (a.v_in == nullptr) {
     // recurrence 0: lane j < O+1 runs the short filter of channel j D + d from the tail and p_t, and shifts the tail
@@ -264,8 +274,9 @@ __device__ __forceinline__ void step_epilogue(const StepArgs& a, int row, int b,
     x0 = a.s_t[(size_t)b * a.C + d];
   }
   if (lane == 0) {
-    const float g = v * gate;
-    a.h[(size_t)row * a.ld + a.t] = g;
+    const T gs = hround<T>(v * gate);
+    a.h[(size_t)row * a.ld + a.t] = gs;
+    const float g = hwiden(gs);
     const float k0 = a.k[(size_t)d * a.kstride + a.ld - 1];
     float y = fmaf(k0, g, acc);
     y = fmaf(a.fbias[(size_t)d * a.fstride], g, y);
@@ -273,7 +284,8 @@ __device__ __forceinline__ void step_epilogue(const StepArgs& a, int row, int b,
   }
 }
 
-__global__ void __launch_bounds__(32 * kStepWarps) decode_step_kernel(const StepArgs a) {
+template <class T>
+__global__ void __launch_bounds__(32 * kStepWarps) decode_step_kernel(const StepArgsT<T> a) {
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * kStepWarps + (threadIdx.x >> 5);      // b * D + d
   if (row >= a.B * a.D) return;
@@ -284,7 +296,8 @@ __global__ void __launch_bounds__(32 * kStepWarps) decode_step_kernel(const Step
 
 // a step inside an open window: the partials of the window positions [b, t), then F[t-b] (the history before b), then
 // the same epilogue as decode_step_kernel; the summation order is fixed, so a windowed step is bitwise reproducible
-__global__ void __launch_bounds__(32 * kStepWarps) decode_win_step_kernel(const WinStepArgs w) {
+template <class T>
+__global__ void __launch_bounds__(32 * kStepWarps) decode_win_step_kernel(const WinStepArgsT<T> w) {
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * kStepWarps + (threadIdx.x >> 5);      // b * D + d
   if (row >= w.st.B * w.st.D) return;
@@ -295,7 +308,8 @@ __global__ void __launch_bounds__(32 * kStepWarps) decode_win_step_kernel(const 
 
 // a step of a branched cache: the partials of the branch's own positions [b, t), then F[parent[row b]][d][t-b] (the shared
 // context before b), then the same epilogue on the branch's history row (stride H); fixed order, bitwise reproducible
-__global__ void __launch_bounds__(32 * kStepWarps) decode_branch_step_kernel(const BranchStepArgs w) {
+template <class T>
+__global__ void __launch_bounds__(32 * kStepWarps) decode_branch_step_kernel(const BranchStepArgsT<T> w) {
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * kStepWarps + (threadIdx.x >> 5);      // b * D + d
   if (row >= w.st.B * w.st.D) return;
@@ -306,12 +320,14 @@ __global__ void __launch_bounds__(32 * kStepWarps) decode_branch_step_kernel(con
 }
 
 // the combine kernels of a device-position step: t (and win_b, base) from pos, then the same bodies as above
-__device__ __forceinline__ void dev_position(StepArgs& st, int t) {
+template <class T>
+__device__ __forceinline__ void dev_position(StepArgsT<T>& st, int t) {
   st.t = t;
   st.nchunk = (t + kChunk - 1) / kChunk;
 }
 
-__global__ void __launch_bounds__(32 * kStepWarps) decode_step_dev_kernel(StepArgs a, const int* pos) {
+template <class T>
+__global__ void __launch_bounds__(32 * kStepWarps) decode_step_dev_kernel(StepArgsT<T> a, const int* pos) {
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * kStepWarps + (threadIdx.x >> 5);      // b * D + d
   if (row >= a.B * a.D) return;
@@ -322,7 +338,8 @@ __global__ void __launch_bounds__(32 * kStepWarps) decode_step_dev_kernel(StepAr
 }
 
 // the partials cover [win_b, t); st.t stays absolute (g_t is written at h[t]) while the partial count follows t - win_b
-__global__ void __launch_bounds__(32 * kStepWarps) decode_win_step_dev_kernel(WinStepArgs w, const int* pos) {
+template <class T>
+__global__ void __launch_bounds__(32 * kStepWarps) decode_win_step_dev_kernel(WinStepArgsT<T> w, const int* pos) {
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * kStepWarps + (threadIdx.x >> 5);      // b * D + d
   if (row >= w.st.B * w.st.D) return;
@@ -334,7 +351,8 @@ __global__ void __launch_bounds__(32 * kStepWarps) decode_win_step_dev_kernel(Wi
   step_epilogue(w.st, row, b, d, lane, acc);
 }
 
-__global__ void __launch_bounds__(32 * kStepWarps) decode_branch_step_dev_kernel(BranchStepArgs w, const int* pos) {
+template <class T>
+__global__ void __launch_bounds__(32 * kStepWarps) decode_branch_step_dev_kernel(BranchStepArgsT<T> w, const int* pos) {
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * kStepWarps + (threadIdx.x >> 5);      // b * D + d
   if (row >= w.st.B * w.st.D) return;

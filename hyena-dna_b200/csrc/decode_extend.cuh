@@ -12,7 +12,8 @@
 //                              g_{o+1} into the next recurrence's history, or y_pre = out * x_0 after the last recurrence
 //   decode_branch_combine_kernel the combine of a branched cache: + the parent row's F[t-b+j] (decode_args.h); the hist and
 //                              dot kernels run unchanged on a branch's history row with shifted arguments
-// fp32, no atomics: every sum has a fixed order for a given (B, D, t, n), so an extend is bitwise reproducible.
+// fp32 arithmetic, no atomics: every sum has a fixed order for a given (B, D, t, n), so an extend is bitwise reproducible.
+// The kernels that touch the history are templates over its element type T (decode.cuh): stores round, reads widen.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -23,7 +24,8 @@ namespace hy {
 namespace dec {
 
 // one CTA per (b, d): channels d, D + d, ..., O D + d of positions [t, t+n)
-__global__ void __launch_bounds__(256) decode_ext_hist_kernel(const ExtHistArgs a) {
+template <class T>
+__global__ void __launch_bounds__(256) decode_ext_hist_kernel(const ExtHistArgsT<T> a) {
   const int row = blockIdx.x;                    // b * D + d
   const int b = row / a.D, d = row - b * a.D;
   const int nj = a.C / a.D;
@@ -42,8 +44,8 @@ __global__ void __launch_bounds__(256) decode_ext_hist_kernel(const ExtHistArgs 
   __syncthreads();                               // every read of the tail is done; s of this row is visible to the CTA
   const float* sv = a.s + ((size_t)b * a.C + a.C - a.D + d) * a.n;
   const float* sg = a.s + ((size_t)b * a.C + a.gate + d) * a.n;
-  float* h = a.h + (size_t)row * a.ld + a.t;
-  for (int j = threadIdx.x; j < a.n; j += blockDim.x) h[j] = sv[j] * sg[j];
+  T* h = a.h + (size_t)row * a.ld + a.t;
+  for (int j = threadIdx.x; j < a.n; j += blockDim.x) h[j] = hround<T>(sv[j] * sg[j]);
   if ((int)threadIdx.x < nj) {
     const int c = threadIdx.x * a.D + d;
     const size_t bc = (size_t)b * a.C + c;
@@ -73,8 +75,8 @@ __device__ __forceinline__ int sk(int x) { return x + (x >> 5); }
 // chunk into consecutive runs of QL positions.  Along a run the 8 taps a lane needs slide by one per position: one new
 // shared-memory load per position feeds 8 * BG FMAs.  The lanes' sums are reduced by a butterfly, the column's warps in a
 // fixed order through shared memory.
-template <int BG, int NT>
-__global__ void __launch_bounds__(32 * kExtWarps, 1) decode_ext_dot_kernel(const ExtDotArgs a) {
+template <int BG, int NT, class T>
+__global__ void __launch_bounds__(32 * kExtWarps, 1) decode_ext_dot_kernel(const ExtDotArgsT<T> a) {
   constexpr int RJ = kExtRJ;
   constexpr int JT = NT / RJ;
   constexpr int WPC = kExtWarps / JT;
@@ -109,8 +111,8 @@ __global__ void __launch_bounds__(32 * kExtWarps, 1) decode_ext_dot_kernel(const
       const int i = v / (kChunk / 4), q = (v - i * (kChunk / 4)) * 4;
       const int b = b0 + i, s = s0 + q;
       float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (b < a.B && s < L) {                    // s < L <= ld, ld % 4 == 0: the whole float4 lies inside the row
-        x = ld4(a.h + ((size_t)b * a.D + d) * a.ld + s);
+      if (b < a.B && s < L) {                    // s < L <= ld, ld % 4 == 0: the whole vector lies inside the row
+        x = hld4(a.h + ((size_t)b * a.D + d) * a.ld + s);
         if (s + 4 > L) {                         // positions >= t + n hold no history yet
           x.y = s + 1 < L ? x.y : 0.f;
           x.z = s + 2 < L ? x.z : 0.f;
@@ -181,7 +183,8 @@ __global__ void __launch_bounds__(32 * kExtWarps, 1) decode_ext_dot_kernel(const
 }
 
 // fixed-order sum of the partials of output j of one (b, channel) row
-__device__ __forceinline__ float ext_partial_sum(const ExtCombineArgs& a, int row, int j) {
+template <class T>
+__device__ __forceinline__ float ext_partial_sum(const ExtCombineArgsT<T>& a, int row, int j) {
   const float* pp = a.part + (size_t)row * a.prow + (size_t)j * a.pj;
   float acc = 0.f;
   for (int g = 0; g < a.groups; ++g) acc += pp[g];
@@ -189,16 +192,18 @@ __device__ __forceinline__ float ext_partial_sum(const ExtCombineArgs& a, int ro
 }
 
 // everything of output j once acc = sum_{s<t+j} k[t+j-s] g[s] is known: + bias g, times the gate, into h_next or y
-__device__ __forceinline__ void ext_combine_epilogue(const ExtCombineArgs& a, int row, int b, int d, int j, float acc) {
-  const float gv = a.h[(size_t)row * a.ld + a.t + j];
+template <class T>
+__device__ __forceinline__ void ext_combine_epilogue(const ExtCombineArgsT<T>& a, int row, int b, int d, int j, float acc) {
+  const float gv = hwiden(a.h[(size_t)row * a.ld + a.t + j]);
   const float y = fmaf(__ldg(a.fbias + (size_t)d * a.fstride), gv, acc);
   const float x = a.s[((size_t)b * a.C + a.xch + d) * a.n + j];
   if (a.last) a.y[(size_t)row * a.n + j] = y * x;
-  else a.h_next[(size_t)row * a.ld + a.t + j] = y * x;
+  else a.h_next[(size_t)row * a.ld + a.t + j] = hround<T>(y * x);
 }
 
 // one thread per (b, d, j)
-__global__ void __launch_bounds__(256) decode_ext_combine_kernel(const ExtCombineArgs a) {
+template <class T>
+__global__ void __launch_bounds__(256) decode_ext_combine_kernel(const ExtCombineArgsT<T> a) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (long long)a.B * a.D * a.n) return;
   const int row = (int)(idx / a.n), j = (int)(idx - (long long)row * a.n);
@@ -208,8 +213,9 @@ __global__ void __launch_bounds__(256) decode_ext_combine_kernel(const ExtCombin
 
 // the combine of a branched cache (decode_args.h BranchCombineArgs): the partials over the branch's positions [b, t+j), then
 // F[parent[row b]][d][t-b+j] (the shared context before b), then the same epilogue; one thread per (b, d, j)
-__global__ void __launch_bounds__(256) decode_branch_combine_kernel(const BranchCombineArgs w) {
-  const ExtCombineArgs& a = w.c;
+template <class T>
+__global__ void __launch_bounds__(256) decode_branch_combine_kernel(const BranchCombineArgsT<T> w) {
+  const ExtCombineArgsT<T>& a = w.c;
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (long long)a.B * a.D * a.n) return;
   const int row = (int)(idx / a.n), j = (int)(idx - (long long)row * a.n);

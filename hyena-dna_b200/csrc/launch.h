@@ -60,25 +60,31 @@ int ln_partials(long long rows);                     // CTAs (= rows of the dw/d
 cudaError_t launch_add_ln_fwd(const ln::FwdArgs& a, cudaStream_t s);
 cudaError_t launch_add_ln_bwd(ln::BwdArgs a, float* dw, float* db, cudaStream_t s);
 // k_decode.cu: incremental decoding (decode.cuh)
-cudaError_t launch_decode_hist(const dec::HistArgs& a, cudaStream_t s);
-cudaError_t launch_decode_admit(const dec::AdmitArgs& a, cudaStream_t s);
-cudaError_t launch_decode_shift(const dec::ShiftArgs& a, long long rows, cudaStream_t s);
-cudaError_t launch_decode_step(const dec::DotArgs& dot, const dec::StepArgs& st, cudaStream_t s);
-cudaError_t launch_decode_win_step(const dec::DotArgs& dot, const dec::WinStepArgs& w, cudaStream_t s);
-cudaError_t launch_decode_branch_step(const dec::DotArgs& dot, const dec::BranchStepArgs& w, cudaStream_t s);
+template <class T> cudaError_t launch_decode_hist(const dec::HistArgsT<T>& a, cudaStream_t s);
+template <class T> cudaError_t launch_decode_admit(const dec::AdmitArgsT<T>& a, cudaStream_t s);
+template <class T> cudaError_t launch_decode_shift(const dec::ShiftArgsT<T>& a, long long rows, cudaStream_t s);
+template <class T>
+cudaError_t launch_decode_step(const dec::DotArgsT<T>& dot, const dec::StepArgsT<T>& st, cudaStream_t s);
+template <class T>
+cudaError_t launch_decode_win_step(const dec::DotArgsT<T>& dot, const dec::WinStepArgsT<T>& w, cudaStream_t s);
+template <class T>
+cudaError_t launch_decode_branch_step(const dec::DotArgsT<T>& dot, const dec::BranchStepArgsT<T>& w, cudaStream_t s);
 // the same steps with the position read on the device from pos = [t, win_b, base]; the dot kernel's grid is nchunk chunks
-cudaError_t launch_decode_step_dev(const dec::DotArgs& dot, const dec::StepArgs& st, const int* pos, int nchunk,
+template <class T>
+cudaError_t launch_decode_step_dev(const dec::DotArgsT<T>& dot, const dec::StepArgsT<T>& st, const int* pos, int nchunk,
                                    cudaStream_t s);
-cudaError_t launch_decode_win_step_dev(const dec::DotArgs& dot, const dec::WinStepArgs& w, const int* pos, int nchunk,
-                                       cudaStream_t s);
-cudaError_t launch_decode_branch_step_dev(const dec::DotArgs& dot, const dec::BranchStepArgs& w, const int* pos, int nchunk,
-                                          cudaStream_t s);
+template <class T>
+cudaError_t launch_decode_win_step_dev(const dec::DotArgsT<T>& dot, const dec::WinStepArgsT<T>& w, const int* pos,
+                                       int nchunk, cudaStream_t s);
+template <class T>
+cudaError_t launch_decode_branch_step_dev(const dec::DotArgsT<T>& dot, const dec::BranchStepArgsT<T>& w, const int* pos,
+                                          int nchunk, cudaStream_t s);
 cudaError_t launch_decode_pos_advance(int* pos, cudaStream_t s);
 // k_decode_extend.cu: extending a decode cache by n positions (decode_extend.cuh)
-cudaError_t launch_decode_ext_hist(const dec::ExtHistArgs& a, cudaStream_t s);
-cudaError_t launch_decode_ext_dot(const dec::ExtDotArgs& a, cudaStream_t s);
-cudaError_t launch_decode_ext_combine(const dec::ExtCombineArgs& a, cudaStream_t s);
-cudaError_t launch_decode_branch_combine(const dec::BranchCombineArgs& a, cudaStream_t s);
+template <class T> cudaError_t launch_decode_ext_hist(const dec::ExtHistArgsT<T>& a, cudaStream_t s);
+template <class T> cudaError_t launch_decode_ext_dot(const dec::ExtDotArgsT<T>& a, cudaStream_t s);
+template <class T> cudaError_t launch_decode_ext_combine(const dec::ExtCombineArgsT<T>& a, cudaStream_t s);
+template <class T> cudaError_t launch_decode_branch_combine(const dec::BranchCombineArgsT<T>& a, cudaStream_t s);
 // k_convert.cu: reference filter-spectrum convention (rfft(k, fft_size), natural order) <-> packed spectrum
 cudaError_t launch_rfft_to_packed(const float2* X, float2* Z, int H, int logM, int logM1, cudaStream_t s);
 cudaError_t launch_packed_to_rfft(const float2* Z, float2* X, int H, int logM, int logM1, float scale, cudaStream_t s);

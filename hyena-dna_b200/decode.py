@@ -27,6 +27,16 @@ def _chunks(lcap):
     return (lcap + CHUNK - 1) // CHUNK
 
 
+HISTORY_DTYPES = (torch.float32, torch.float16, torch.bfloat16)
+
+
+def check_history_dtype(history_dtype):
+    """The element type of a cache's stored history h (DESIGN.md section 4.16): fp32 (the default), fp16 or bf16."""
+    if history_dtype not in HISTORY_DTYPES:
+        raise HyenaB200Error(f"history_dtype must be torch.float32, torch.float16 or torch.bfloat16; got {history_dtype!r}")
+    return history_dtype
+
+
 def _host_index(index, n, what):
     """index (a sequence or 1-D tensor of integers) -> list of ints in [0, n), checked on the host before any device work."""
     if torch.is_tensor(index):
@@ -80,11 +90,13 @@ class DecodeCache:
     (``Backbone.allocate_decode_cache``: ``layers`` holds one per layer, looked up by module identity).
 
     Per operator, with O = order, D = d_model, F = (O-1) D filter channels, C = (O+1) D in_proj channels and ld = Lcap
-    rounded up to a multiple of 4 (all fp32, on the operator's device):
+    rounded up to a multiple of 4 (all fp32 but h, on the operator's device):
       k     (F * ld + 4,)       the filter, each row time-reversed (k[c][j] at c*ld + ld-1-j) so that the step kernel streams
                                 history and filter in ascending order; 4 floats of padding
       bias  (F,)                the effective filter bias (0 * bias when use_bias is false, as in forward)
-      h     (O-1, B, D, ld)     g_o of every recurrence by position
+      h     (O-1, B, D, ld)     g_o of every recurrence by position, in ``history_dtype``: fp32 by default; fp16 or bf16
+                                hold g^_o = g_o rounded to nearest even, and every route then computes
+                                out_o[t] = sum_{s<=t} k_o[t-s] g^_o[s] + bias_o g^_o[t] in fp32 (DESIGN.md section 4.16)
       tail  (B, C, 2)           in_proj outputs (with bias) of the last two positions
       s_t   (B, C)              short-filter outputs of the current position
       part  (B, D, ceil(Lcap / 1024))  partial dot products of one step
@@ -137,8 +149,10 @@ class DecodeCache:
             self.d_model, self.order = owner.d_model, owner.order
 
     @classmethod
-    def allocate(cls, op, batch_size, max_seqlen):
-        """Decoding state of ``op`` for ``batch_size`` rows and up to min(max_seqlen, op.l_max) positions."""
+    def allocate(cls, op, batch_size, max_seqlen, history_dtype=torch.float32):
+        """Decoding state of ``op`` for ``batch_size`` rows and up to min(max_seqlen, op.l_max) positions, with the history
+        stored as ``history_dtype`` (torch.float32, torch.float16 or torch.bfloat16)."""
+        check_history_dtype(history_dtype)
         if op.filter_fn.bidirectional:
             raise HyenaB200Error("decoding needs a causal filter; this HyenaFilter is bidirectional")
         if batch_size < 1 or max_seqlen < 1:
@@ -157,7 +171,7 @@ class DecodeCache:
             krev[:F * ld].view(F, ld)[:, ld - lcap:] = k.flip(-1)
             fb = op.filter_fn.bias if op.filter_fn.use_bias else 0 * op.filter_fn.bias
             fb = fb.detach().reshape(-1).to(torch.float32).contiguous().clone()
-        h = torch.zeros(O - 1, B, D, ld, dtype=torch.float32, device=dev)
+        h = torch.zeros(O - 1, B, D, ld, dtype=history_dtype, device=dev)
         tail = torch.zeros(B, (O + 1) * D, 2, dtype=torch.float32, device=dev)
         s_t = torch.zeros(B, (O + 1) * D, dtype=torch.float32, device=dev)
         part = torch.zeros(B, D, _chunks(lcap), dtype=torch.float32, device=dev)
@@ -172,11 +186,17 @@ class DecodeCache:
         return cls(None, caches[0].batch_size, caches[0].max_seqlen, min(c.lcap for c in caches), layers=caches)
 
     @staticmethod
-    def layout_nbytes(batch_size, d_model, order, lcap):
-        """Bytes one operator's cache takes (the layout in the class docstring)."""
+    def layout_nbytes(batch_size, d_model, order, lcap, history_dtype=torch.float32):
+        """Bytes one operator's cache takes (the layout in the class docstring), its history stored as ``history_dtype``."""
+        e = torch.empty(0, dtype=check_history_dtype(history_dtype)).element_size()
         B, D, O = batch_size, d_model, order
         ld, F, C = _ld(lcap), (order - 1) * d_model, (order + 1) * d_model
-        return 4 * ((F * ld + 4) + F + (O - 1) * B * D * ld + B * C * 2 + B * C + B * D * _chunks(lcap))
+        return 4 * ((F * ld + 4) + F + B * C * 2 + B * C + B * D * _chunks(lcap)) + e * (O - 1) * B * D * ld
+
+    @property
+    def history_dtype(self):
+        """The element type of the stored history h: torch.float32, torch.float16 or torch.bfloat16."""
+        return self.layers[0].history_dtype if self.layers else self.h.dtype
 
     @property
     def nbytes(self):

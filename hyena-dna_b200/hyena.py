@@ -494,9 +494,10 @@ class HyenaOperator(nn.Module):
         return (v * x[0]).contiguous()
 
     # ------------------------------------------------------------------------------ incremental decoding
-    def allocate_decode_cache(self, batch_size, max_seqlen):
-        """A DecodeCache for ``batch_size`` rows and up to min(max_seqlen, l_max) positions (decode.py)."""
-        return DecodeCache.allocate(self, batch_size, max_seqlen)
+    def allocate_decode_cache(self, batch_size, max_seqlen, history_dtype=torch.float32):
+        """A DecodeCache for ``batch_size`` rows and up to min(max_seqlen, l_max) positions (decode.py), its history stored
+        as ``history_dtype``: torch.float32, or torch.float16 / torch.bfloat16 for half the state (DESIGN.md section 4.16)."""
+        return DecodeCache.allocate(self, batch_size, max_seqlen, history_dtype)
 
     def _decode_checks(self, u, cache, n, fresh=False):
         if not isinstance(cache, DecodeCache):

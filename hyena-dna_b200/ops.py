@@ -740,6 +740,19 @@ def add_layer_norm(x, res, weight, bias, eps):
 
 
 # ------------------------------------------------------------------------------------------ incremental decoding
+_HIST_CODES = {torch.float16: _lib.HIST_F16, torch.bfloat16: _lib.HIST_BF16}
+
+
+def _decode_fn(name, h):
+    """The entry point hyena_b200_decode_<name> for a history h of the cache's dtype: the fp32 function itself, or its
+    _h16 twin bound to the dtype code of a 16-bit history (DecodeCache history_dtype, DESIGN.md section 4.16)."""
+    L = _lib.lib()
+    if h.dtype == torch.float32:
+        return getattr(L, f"hyena_b200_decode_{name}")
+    fn, code = getattr(L, f"hyena_b200_decode_{name}_h16"), _HIST_CODES[h.dtype]
+    return lambda *args: fn(code, *args)
+
+
 def decode_hist(p, in_bias, sw, sb, cache, row_start=None):
     """After a prefill of P positions: g_0 = short(v) * short(x_{O-1}) of positions [0, P) into cache.h[0] and the last two
     in_proj outputs (with bias) into cache.tail (csrc/decode.cuh).  p (B, (O+1) D, P) without in_proj.bias.  row_start
@@ -753,11 +766,11 @@ def decode_hist(p, in_bias, sw, sb, cache, row_start=None):
         raise _lib.HyenaB200Error(f"decode_hist: row_start must be a contiguous ({B},) int32 tensor on {p.device}")
     with torch.cuda.device(p.device):
         if row_start is None:
-            _lib.check(_lib.lib().hyena_b200_decode_hist(
+            _lib.check(_decode_fn("hist", cache.h)(
                 _ptr(p), _ptr(in_bias), _ptr(sw), _ptr(sb), _ptr(cache.h), _ptr(cache.tail), B, cache.batch_size,
                 cache.d_model, cache.order, P, cache.lcap, _stream()))
         else:
-            _lib.check(_lib.lib().hyena_b200_decode_hist_rows(
+            _lib.check(_decode_fn("hist_rows", cache.h)(
                 _ptr(p), _ptr(in_bias), _ptr(sw), _ptr(sb), _ptr(cache.h), _ptr(cache.tail), _ptr(row_start), B,
                 cache.batch_size, cache.d_model, cache.order, P, cache.lcap, _stream()))
 
@@ -774,7 +787,7 @@ def decode_step(p_t, in_bias, sw, sb, cache):
     with torch.cuda.device(p_t.device):
         for o in range(O - 1):
             first = o == 0
-            _lib.check(_lib.lib().hyena_b200_decode_step(
+            _lib.check(_decode_fn("step", cache.h)(
                 _ptr(p_t) if first else 0, _ptr(in_bias) if first else 0, _ptr(sw) if first else 0,
                 _ptr(sb) if first else 0, _ptr(cache.k), _ptr(cache.bias), _ptr(cache.h[o]), _ptr(cache.tail) if first else 0,
                 _ptr(cache.s_t), 0 if first else _ptr(out[o - 1]), _ptr(out[o]), _ptr(cache.part), B, cache.batch_size, D, O,
@@ -816,11 +829,12 @@ def _history_conv(cache, ld, h, o, hist, L):
     """Causal convolution of h[:, :, 0:hist) (zero from hist on) with the first L filter taps of recurrence o -> (B, D, L), on
     the library's filter_spectrum + fftconv_forward with a zero skip term.  h (B, D, >= hist) is g_o by position; ld is the
     row stride of the cache's filter, which is kept reversed, so the filter rows are un-reversed and the history compacted or
-    zero-padded first (O(L) copies beside the transforms); h is not read at positions >= hist."""
+    zero-padded first (O(L) copies beside the transforms); h is not read at positions >= hist.  The transform runs in fp32:
+    a 16-bit history (DESIGN.md section 4.16) is widened into that copy, B D L fp32 of transient memory."""
     D, O = cache.d_model, cache.order
     k = cache.k[:(O - 1) * D * ld].view(D, O - 1, ld)[:, o, ld - L:].flip(-1).contiguous()
     if hist == L:
-        u = h[:, :, :L].contiguous()
+        u = h[:, :, :L].to(torch.float32).contiguous()        # a 16-bit history is widened into a fresh fp32 copy
     else:
         u = torch.zeros(h.shape[0], D, L, dtype=torch.float32, device=h.device)
         u[:, :, :hist] = h[:, :, :hist]
@@ -857,7 +871,7 @@ def decode_win_step(p_t, in_bias, sw, sb, cache):
     with torch.cuda.device(p_t.device):
         for o in range(O - 1):
             first = o == 0
-            _lib.check(_lib.lib().hyena_b200_decode_win_step(
+            _lib.check(_decode_fn("win_step", cache.h)(
                 _ptr(p_t) if first else 0, _ptr(in_bias) if first else 0, _ptr(sw) if first else 0,
                 _ptr(sb) if first else 0, _ptr(cache.k), _ptr(cache.bias), _ptr(cache.h[o]), _ptr(cache.tail) if first else 0,
                 _ptr(cache.s_t), 0 if first else _ptr(out[o - 1]), _ptr(out[o]), _ptr(cache.part),
@@ -907,7 +921,7 @@ def decode_extend_hist(p, in_bias, sw, sb, cache):
     B, n = _extend_check(p, cache, "decode_extend_hist")
     s = torch.empty_like(p)
     with torch.cuda.device(p.device):
-        _lib.check(_lib.lib().hyena_b200_decode_extend_hist(
+        _lib.check(_decode_fn("extend_hist", cache.h)(
             _ptr(p), _ptr(in_bias), _ptr(sw), _ptr(sb), _ptr(cache.h), _ptr(cache.tail), _ptr(s), B, cache.batch_size,
             cache.d_model, cache.order, int(cache.t), n, cache.lcap, _stream()))
     return s
@@ -915,7 +929,7 @@ def decode_extend_hist(p, in_bias, sw, sb, cache):
 
 def _extend_combine(part, row_stride, j_stride, groups, s, out, o, B, n, cache):
     with torch.cuda.device(s.device):
-        _lib.check(_lib.lib().hyena_b200_decode_extend_combine(
+        _lib.check(_decode_fn("extend_combine", cache.h)(
             _ptr(part), int(row_stride), int(j_stride), int(groups), _ptr(cache.bias), _ptr(cache.h[o]), _ptr(s), _ptr(out),
             B, cache.batch_size, cache.d_model, cache.order, o, int(cache.t), n, cache.lcap, _stream()))
 
@@ -937,7 +951,7 @@ def _decode_extend(p, in_bias, sw, sb, cache, fft):
             _extend_combine(conv[:, :, t:], L, 1, 1, s, out, o, B, n, cache)
         else:
             with torch.cuda.device(p.device):
-                _lib.check(_lib.lib().hyena_b200_decode_extend_dot(
+                _lib.check(_decode_fn("extend_dot", cache.h)(
                     _ptr(cache.h[o]), _ptr(cache.k), _ptr(part), groups, B, cache.batch_size, D, O, o, t, n, cache.lcap,
                     _stream()))
             _extend_combine(part, n * groups, groups, groups, s, out, o, B, n, cache)
@@ -1005,7 +1019,7 @@ def decode_fork(cache, rows, horizon):
             hist = cache.h[o] if uniq == list(range(cache.batch_size)) else cache.h[o, uniq, :, :b]
             f[o, :, :, :hc] = _history_conv(cache, ld, hist, o, b, b + hc)[:, :, b:]
     ridx = torch.tensor(rows, dtype=torch.long, device=dev)
-    h = torch.zeros(O - 1, len(rows), D, H, dtype=torch.float32, device=dev)
+    h = torch.zeros(O - 1, len(rows), D, H, dtype=cache.h.dtype, device=dev)
     if t0 > b:
         h[:, :, :, :t0 - b] = cache.h[:, ridx, :, b:t0]
     parent = torch.tensor([slot[r] for r in rows], dtype=torch.int32, device=dev)
@@ -1043,7 +1057,7 @@ def decode_branch_step(p_t, in_bias, sw, sb, cache):
     with torch.cuda.device(p_t.device):
         for o in range(O - 1):
             first = o == 0
-            _lib.check(_lib.lib().hyena_b200_decode_branch_step(
+            _lib.check(_decode_fn("branch_step", cache.h)(
                 _ptr(p_t) if first else 0, _ptr(in_bias) if first else 0, _ptr(sw) if first else 0,
                 _ptr(sb) if first else 0, _ptr(cache.k), _ptr(cache.bias), _ptr(cache.h[o]), _ptr(cache.tail) if first else 0,
                 _ptr(cache.s_t), 0 if first else _ptr(out[o - 1]), _ptr(out[o]), _ptr(cache.part), _ptr(cache.f[o]),
@@ -1101,7 +1115,7 @@ def decode_shift(cache, shift):
     if shift == 0:
         return
     with torch.cuda.device(cache.h.device):
-        _lib.check(_lib.lib().hyena_b200_decode_shift(_ptr(cache.h), cache.batch_size, cache.d_model, cache.order,
+        _lib.check(_decode_fn("shift", cache.h)(_ptr(cache.h), cache.batch_size, cache.d_model, cache.order,
                                                       int(cache.t), shift, cache.lcap, _stream()))
     start = cache.start if cache.start is not None else (0,) * cache.batch_size
     cache.set_start([max(s + shift, 0) for s in start])
@@ -1127,14 +1141,14 @@ def decode_admit(p, in_bias, sw, sb, gs, cache, rows, row_start=None):
     dev = p.device
     rows_dev = torch.tensor(rows, dtype=torch.int32, device=dev)
     with torch.cuda.device(dev):
-        _lib.check(_lib.lib().hyena_b200_decode_admit(
+        _lib.check(_decode_fn("admit", cache.h)(
             _ptr(p), _ptr(in_bias), _ptr(sw), _ptr(sb), _ptr(cache.h), _ptr(cache.tail), _ptr(rows_dev), _ptr(row_start), k,
             cache.batch_size, D, O, P, t, cache.lcap, _stream()))
     off = t - P
     ridx = rows_dev.to(torch.long)
     for o in range(1, O - 1):
-        g = torch.zeros(k, D, t, dtype=torch.float32, device=dev)
-        g[:, :, off:] = gs[o]
+        g = torch.zeros(k, D, t, dtype=cache.h.dtype, device=dev)
+        g[:, :, off:] = gs[o]                       # rounded to a 16-bit history here
         cache.h[o, ridx, :, :t] = g
     if cache.win_wc > 0:
         b, wc = cache.win_b, cache.win_wc
@@ -1172,7 +1186,7 @@ def decode_step_dev(p_t, in_bias, sw, sb, cache, t_max):
     with torch.cuda.device(p_t.device):
         for o in range(O - 1):
             first = o == 0
-            _lib.check(_lib.lib().hyena_b200_decode_step_dev(
+            _lib.check(_decode_fn("step_dev", cache.h)(
                 _ptr(p_t) if first else 0, _ptr(in_bias) if first else 0, _ptr(sw) if first else 0,
                 _ptr(sb) if first else 0, _ptr(cache.k), _ptr(cache.bias), _ptr(cache.h[o]), _ptr(cache.tail) if first else 0,
                 _ptr(cache.s_t), 0 if first else _ptr(out[o - 1]), _ptr(out[o]), _ptr(cache.part), _ptr(cache.pos), B,
@@ -1189,7 +1203,7 @@ def decode_win_step_dev(p_t, in_bias, sw, sb, cache):
     with torch.cuda.device(p_t.device):
         for o in range(O - 1):
             first = o == 0
-            _lib.check(_lib.lib().hyena_b200_decode_win_step_dev(
+            _lib.check(_decode_fn("win_step_dev", cache.h)(
                 _ptr(p_t) if first else 0, _ptr(in_bias) if first else 0, _ptr(sw) if first else 0,
                 _ptr(sb) if first else 0, _ptr(cache.k), _ptr(cache.bias), _ptr(cache.h[o]), _ptr(cache.tail) if first else 0,
                 _ptr(cache.s_t), 0 if first else _ptr(out[o - 1]), _ptr(out[o]), _ptr(cache.part), _ptr(cache.win_f[o]),
@@ -1204,7 +1218,7 @@ def decode_branch_step_dev(p_t, in_bias, sw, sb, cache):
     with torch.cuda.device(p_t.device):
         for o in range(O - 1):
             first = o == 0
-            _lib.check(_lib.lib().hyena_b200_decode_branch_step_dev(
+            _lib.check(_decode_fn("branch_step_dev", cache.h)(
                 _ptr(p_t) if first else 0, _ptr(in_bias) if first else 0, _ptr(sw) if first else 0,
                 _ptr(sb) if first else 0, _ptr(cache.k), _ptr(cache.bias), _ptr(cache.h[o]), _ptr(cache.tail) if first else 0,
                 _ptr(cache.s_t), 0 if first else _ptr(out[o - 1]), _ptr(out[o]), _ptr(cache.part), _ptr(cache.f[o]),
@@ -1233,7 +1247,7 @@ def decode_branch_extend(p, in_bias, sw, sb, cache, fft=None):
     s = torch.empty_like(p)
     y = torch.empty(B, D, n, dtype=torch.float32, device=p.device)
     with torch.cuda.device(p.device):
-        _lib.check(lib.hyena_b200_decode_branch_extend_hist(
+        _lib.check(_decode_fn("branch_extend_hist", cache.h)(
             _ptr(p), _ptr(in_bias), _ptr(sw), _ptr(sb), _ptr(cache.h), _ptr(cache.tail), _ptr(s), B, D, O, t, n, b, hc, H,
             lcap, _stream()))
         if not fft:
@@ -1245,10 +1259,10 @@ def decode_branch_extend(p, in_bias, sw, sb, cache, fft=None):
                 conv = _history_conv(cache, (lcap + 3) // 4 * 4, cache.h[o], o, j + n, j + n)
                 src, row_stride, j_stride, g = conv[:, :, j:], j + n, 1, 1
             else:
-                _lib.check(lib.hyena_b200_decode_branch_extend_dot(
+                _lib.check(_decode_fn("branch_extend_dot", cache.h)(
                     _ptr(cache.h[o]), _ptr(cache.k), _ptr(part), groups, B, D, O, o, t, n, b, hc, H, lcap, _stream()))
                 src, row_stride, j_stride, g = part, n * groups, groups, groups
-            _lib.check(lib.hyena_b200_decode_branch_combine(
+            _lib.check(_decode_fn("branch_combine", cache.h)(
                 _ptr(src), int(row_stride), int(j_stride), int(g), _ptr(cache.bias), _ptr(cache.h[o]), _ptr(s), _ptr(out),
                 _ptr(cache.f[o]), _ptr(cache.parent), B, D, O, o, t, n, b, hc, H, lcap, _stream()))
     return y

@@ -385,6 +385,79 @@ HY_API int hyena_b200_decode_branch_step_dev(const float* p_t, const float* in_b
                                              const int* pos, int R, int D, int order, int o, int H, int Lcap, void* stream);
 HY_API int hyena_b200_decode_pos_advance(int* pos, void* stream);
 
+/* ---- a 16-bit decode history (DecodeCache(history_dtype=torch.float16 / torch.bfloat16), DESIGN.md section 4.16) -------
+ * Each hyena_b200_decode_*_h16 entry point is the fp32 entry point of the same name with a history dtype code in front
+ * and h (void*) holding HYENA_B200_HIST_F16 (IEEE binary16) or HYENA_B200_HIST_BF16 (bfloat16) elements; any other code
+ * fails.  Only h changes type: k, fbias, tail, s_t, part, win, f, parent and every output stay fp32, and all arithmetic is
+ * fp32.  A value is rounded to nearest even once, when it is stored into h (g^ = round(g)); every read widens it exactly,
+ * and a step's own s = t term and bias term use g^ too:  out_o[t] = sum_{s<=t} k_o[t-s] g^_o[s] + fbias_o g^_o[t].  h is
+ * aligned to 4 elements (8 bytes) wherever the fp32 twin asks for 16 bytes, and to 2 bytes where it asks for 4.  In the
+ * combine entry points out (void*) is the next recurrence's history rows (16-bit) for o < order - 2, else y (fp32).  The
+ * guards, launches, profiler kinds and launch counts are those of the fp32 twin.  A value past the type's range stores
+ * as +-inf (fp16 overflows above 65504) and stays in its (b, channel) row, as a non-finite input does. */
+#define HYENA_B200_HIST_F16 1
+#define HYENA_B200_HIST_BF16 2
+HY_API int hyena_b200_decode_hist_h16(int hist_dtype, const float* p, const float* in_bias, const float* sw,
+                                      const float* sb, void* h, float* tail, int B, int cache_B, int D, int order,
+                                      int P, int Lcap, void* stream);
+HY_API int hyena_b200_decode_hist_rows_h16(int hist_dtype, const float* p, const float* in_bias, const float* sw,
+                                           const float* sb, void* h, float* tail, const int* row_start, int B,
+                                           int cache_B, int D, int order, int P, int Lcap, void* stream);
+HY_API int hyena_b200_decode_admit_h16(int hist_dtype, const float* p, const float* in_bias, const float* sw,
+                                       const float* sb, void* h, float* tail, const int* rows, const int* row_start,
+                                       int k, int cache_B, int D, int order, int P, int t, int Lcap, void* stream);
+HY_API int hyena_b200_decode_shift_h16(int hist_dtype, void* h, int B, int D, int order, int t, int shift, int Lcap,
+                                       void* stream);
+HY_API int hyena_b200_decode_step_h16(int hist_dtype, const float* p_t, const float* in_bias, const float* sw,
+                                      const float* sb, const float* k, const float* fbias, void* h, float* tail,
+                                      float* s_t, const float* v_in, float* out, float* part, int B, int cache_B, int D,
+                                      int order, int o, int t, int Lcap, void* stream);
+HY_API int hyena_b200_decode_win_step_h16(int hist_dtype, const float* p_t, const float* in_bias, const float* sw,
+                                          const float* sb, const float* k, const float* fbias, void* h, float* tail,
+                                          float* s_t, const float* v_in, float* out, float* part, const float* win,
+                                          int B, int cache_B, int D, int order, int o, int t, int b, int Wc, int W,
+                                          int Lcap, void* stream);
+HY_API int hyena_b200_decode_extend_hist_h16(int hist_dtype, const float* p, const float* in_bias, const float* sw,
+                                             const float* sb, void* h, float* tail, float* s, int B, int cache_B, int D,
+                                             int order, int t, int n, int Lcap, void* stream);
+HY_API int hyena_b200_decode_extend_dot_h16(int hist_dtype, const void* h, const float* k, float* part, int groups,
+                                            int B, int cache_B, int D, int order, int o, int t, int n, int Lcap,
+                                            void* stream);
+HY_API int hyena_b200_decode_extend_combine_h16(int hist_dtype, const float* part, long long row_stride, int j_stride,
+                                                int groups, const float* fbias, const void* h, const float* s,
+                                                void* out, int B, int cache_B, int D, int order, int o, int t, int n,
+                                                int Lcap, void* stream);
+HY_API int hyena_b200_decode_branch_step_h16(int hist_dtype, const float* p_t, const float* in_bias, const float* sw,
+                                             const float* sb, const float* k, const float* fbias, void* h, float* tail,
+                                             float* s_t, const float* v_in, float* out, float* part, const float* f,
+                                             const int* parent, int R, int D, int order, int o, int t, int b, int Hc,
+                                             int H, int Lcap, void* stream);
+HY_API int hyena_b200_decode_branch_extend_hist_h16(int hist_dtype, const float* p, const float* in_bias,
+                                                    const float* sw, const float* sb, void* h, float* tail, float* s,
+                                                    int R, int D, int order, int t, int n, int b, int Hc, int H,
+                                                    int Lcap, void* stream);
+HY_API int hyena_b200_decode_branch_extend_dot_h16(int hist_dtype, const void* h, const float* k, float* part,
+                                                   int groups, int R, int D, int order, int o, int t, int n, int b,
+                                                   int Hc, int H, int Lcap, void* stream);
+HY_API int hyena_b200_decode_branch_combine_h16(int hist_dtype, const float* part, long long row_stride, int j_stride,
+                                                int groups, const float* fbias, const void* h, const float* s,
+                                                void* out, const float* f, const int* parent, int R, int D, int order,
+                                                int o, int t, int n, int b, int Hc, int H, int Lcap, void* stream);
+HY_API int hyena_b200_decode_step_dev_h16(int hist_dtype, const float* p_t, const float* in_bias, const float* sw,
+                                          const float* sb, const float* k, const float* fbias, void* h, float* tail,
+                                          float* s_t, const float* v_in, float* out, float* part, const int* pos, int B,
+                                          int cache_B, int D, int order, int o, int t_max, int Lcap, void* stream);
+HY_API int hyena_b200_decode_win_step_dev_h16(int hist_dtype, const float* p_t, const float* in_bias, const float* sw,
+                                              const float* sb, const float* k, const float* fbias, void* h, float* tail,
+                                              float* s_t, const float* v_in, float* out, float* part, const float* win,
+                                              const int* pos, int B, int cache_B, int D, int order, int o, int W,
+                                              int Lcap, void* stream);
+HY_API int hyena_b200_decode_branch_step_dev_h16(int hist_dtype, const float* p_t, const float* in_bias,
+                                                 const float* sw, const float* sb, const float* k, const float* fbias,
+                                                 void* h, float* tail, float* s_t, const float* v_in, float* out,
+                                                 float* part, const float* f, const int* parent, const int* pos, int R,
+                                                 int D, int order, int o, int H, int Lcap, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

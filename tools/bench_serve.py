@@ -46,9 +46,9 @@ def pct(xs, q):
     return xs[min(len(xs) - 1, int(math.ceil(q * len(xs))) - 1)]
 
 
-def continuous(m, trace, B, D, lcap, dev):
+def continuous(m, trace, B, D, lcap, dev, hd=torch.float32):
     """(a): -> (seconds, latencies, admit times, compact times, compactions)."""
-    cache = m.allocate_decode_cache(B, lcap)
+    cache = m.allocate_decode_cache(B, lcap, history_dtype=hd)
     queue = list(range(len(trace)))
     left, lat, adm, cmp_ = {}, [], [], []
     t0 = now()
@@ -98,7 +98,7 @@ def continuous(m, trace, B, D, lcap, dev):
     return now() - t0, lat, adm, cmp_
 
 
-def static(m, trace, B, D, dev):
+def static(m, trace, B, D, dev, hd=torch.float32):
     """(b): -> (seconds, latencies, prefill times)."""
     lat, pre = [], []
     t0 = now()
@@ -111,7 +111,7 @@ def static(m, trace, B, D, dev):
             u = torch.zeros(k, P, D, device=dev)
             for j, n in enumerate(lengths):
                 u[j, P - n:] = 0.5 * torch.randn(n, D, device=dev)
-            cache = m.allocate_decode_cache(k, P + G)
+            cache = m.allocate_decode_cache(k, P + G, history_dtype=hd)
             a = now()
             m.prefill(u, cache, lengths=lengths)
             pre.append(now() - a)
@@ -127,15 +127,15 @@ def static(m, trace, B, D, dev):
     return now() - t0, lat, pre
 
 
-def shift_rate(m, B, D, lcap, dev, reps=5):
-    """hyena_b200_decode_shift on one layer's cache at t = lcap - 8, left by 4096 and back, alternated: (ms per shift,
-    GB/s on 8 (O-1) B D t bytes, the read and the write of every history word below t)."""
+def shift_rate(m, B, D, lcap, dev, reps=5, hd=torch.float32):
+    """hyena_b200_decode_shift (or its _h16 twin) on one layer's cache at t = lcap - 8, left by 4096 and back, alternated:
+    (ms per shift, GB/s on 2 e (O-1) B D t bytes, the read and the write of every history word below t, e bytes each)."""
     import hyena_dna_b200 as H
-    c = m.layers[0].mixer.allocate_decode_cache(B, lcap)
-    lib, t, stream = H._lib.lib(), lcap - 8, torch.cuda.current_stream().cuda_stream
+    c = m.layers[0].mixer.allocate_decode_cache(B, lcap, history_dtype=hd)
+    fn, t, stream = H.ops._decode_fn("shift", c.h), lcap - 8, torch.cuda.current_stream().cuda_stream
 
     def shift(pos, by):
-        H._lib.check(lib.hyena_b200_decode_shift(c.h.data_ptr(), B, D, c.order, pos, by, lcap, stream))
+        H._lib.check(fn(c.h.data_ptr(), B, D, c.order, pos, by, lcap, stream))
     s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     shift(t, -4096)
     shift(t - 4096, 4096)
@@ -147,7 +147,7 @@ def shift_rate(m, B, D, lcap, dev, reps=5):
     e.record()
     torch.cuda.synchronize()
     ms = s.elapsed_time(e) / (2 * reps)
-    nbytes = 8 * (c.order - 1) * B * D * t
+    nbytes = 2 * c.h.element_size() * (c.order - 1) * B * D * t
     del c
     return ms, nbytes / ms / 1e6
 
@@ -165,6 +165,9 @@ def main():
     ap.add_argument("--d-model", type=int, default=256)
     ap.add_argument("--n-layer", type=int, default=8)
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--history-dtype", nargs="+", default=["float32"], choices=["float32", "float16", "bfloat16"],
+                    help="the decode caches' history dtype (DESIGN.md section 4.16); several: each in turn, same trace")
+    ap.add_argument("--skip-static", action="store_true", help="run continuous batching (a) only")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "bench_serve needs a CUDA device"
     import hyena_dna_b200 as H
@@ -172,7 +175,8 @@ def main():
     dev = torch.device("cuda:0")
     name, limit = card()
     D = args.d_model
-    for B, max_len in zip(args.batch, args.max_len):
+    for (B, max_len), hname in [(bm, h) for bm in zip(args.batch, args.max_len) for h in args.history_dtype]:
+        hd = getattr(torch, hname)
         rng = random.Random(args.seed)
         trace = [(int(round(math.exp(rng.uniform(math.log(args.min_len), math.log(max_len))))),
                   rng.randint(args.gen_min, args.gen_max)) for _ in range(args.requests * B)]
@@ -184,22 +188,24 @@ def main():
                        mlp_cls=partial(H.Mlp, hidden_features=4 * D), residual_in_fp32=True).to(dev)
         gen = sum(n for _, n in trace)
         rec = {"bench": "serve", "gpu": name, "power_limit": limit, "B": B, "D": D, "n_layer": args.n_layer,
-               "requests": len(trace), "prompt_sum": sum(p for p, _ in trace), "generated": gen, "lcap": lcap}
+               "requests": len(trace), "prompt_sum": sum(p for p, _ in trace), "generated": gen, "lcap": lcap,
+               "history_dtype": hname, "cache_nbytes": args.n_layer * H.DecodeCache.layout_nbytes(B, D, 2, lcap, hd)}
         with torch.no_grad():
             w = min(B, 2)                    # warm-up of the library's set-up at this model's shapes
             m.prefill(0.5 * torch.randn(w, 1024, D, device=dev), m.allocate_decode_cache(w, 2048))
             torch.cuda.empty_cache()
-            sec, lat, adm, cmp_ = continuous(m, trace, B, D, lcap, dev)
+            sec, lat, adm, cmp_ = continuous(m, trace, B, D, lcap, dev, hd)
             rec.update(a_tokens_per_s=gen / sec, a_seconds=sec, a_latency_p50_s=pct(lat, 0.5), a_latency_p99_s=pct(lat, 0.99),
                        a_admits=len(adm), a_admit_ms_mean=1e3 * sum(adm) / len(adm), a_admit_ms_max=1e3 * max(adm),
                        a_compactions=len(cmp_), a_compact_ms_mean=1e3 * sum(cmp_) / len(cmp_) if cmp_ else None,
                        a_compact_ms_max=1e3 * max(cmp_) if cmp_ else None)
             torch.cuda.empty_cache()
-            sec, lat, pre = static(m, trace, B, D, dev)
-            rec.update(b_tokens_per_s=gen / sec, b_seconds=sec, b_latency_p50_s=pct(lat, 0.5), b_latency_p99_s=pct(lat, 0.99),
-                       b_prefills=len(pre), b_prefill_ms_mean=1e3 * sum(pre) / len(pre))
+            if not args.skip_static:
+                sec, lat, pre = static(m, trace, B, D, dev, hd)
+                rec.update(b_tokens_per_s=gen / sec, b_seconds=sec, b_latency_p50_s=pct(lat, 0.5),
+                           b_latency_p99_s=pct(lat, 0.99), b_prefills=len(pre), b_prefill_ms_mean=1e3 * sum(pre) / len(pre))
             torch.cuda.empty_cache()
-            ms, gbs = shift_rate(m, B, D, lcap, dev)
+            ms, gbs = shift_rate(m, B, D, lcap, dev, hd=hd)
             rec.update(shift_ms=ms, shift_t=lcap - 8, shift_gb_per_s=gbs)
         print(json.dumps({k: (round(v, 4) if isinstance(v, float) else v) for k, v in rec.items()}), flush=True)
         del m
