@@ -6,6 +6,7 @@
 #include <cstring>
 #include <map>
 #include <mutex>
+#include <tuple>
 #include <type_traits>
 #include <utility>
 #include <vector>
@@ -326,18 +327,17 @@ HY_API size_t hyena_b200_workspace_bytes(int B, int D, int L, int backward) {
   return hyena_b200_workspace_min_bytes(B, D, L, backward) * (size_t)nch;
 }
 
-// tensor-core filter path: scratch for the tf32 hi/lo weight images (~0.3 MB, grow-only), one per (device, stream): two
-// operators driven from different streams never share it (the prep kernel of one would overwrite the images the other's
-// wgmma kernel is still reading)
-static int get_wimg(int D, cudaStream_t stream, float** out) {
+// tensor-core filter path: scratch, grow-only, one per (device, stream, use): two operators driven from different streams
+// never share it (the prep kernel of one would overwrite the images the other's wgmma kernel is still reading).
+// Uses: 0 = the tf32 hi/lo weight images (~0.3 MB), 1 = stage 2's [zT; 1] and partial sums (~40 MB at L = 2^20)
+static int get_filter_buf(int use, size_t need, cudaStream_t stream, float** out) {
   int dev = -1;
   HY_CUDA(cudaGetDevice(&dev));
   HY_CHECK(dev >= 0 && dev < 64, "unsupported device ordinal %d", dev);
   std::lock_guard<std::mutex> lk(g_mu);
   struct Buf { float* p = nullptr; size_t n = 0; };
-  static std::map<std::pair<int, cudaStream_t>, Buf> bufs;
-  Buf& b = bufs[std::make_pair(dev, stream)];
-  const size_t need = filter_tc_wimg_bytes(D);
+  static std::map<std::tuple<int, cudaStream_t, int>, Buf> bufs;
+  Buf& b = bufs[std::make_tuple(dev, stream, use)];
   if (b.n < need) {
     if (b.p) { HY_CUDA(cudaStreamSynchronize(stream)); HY_CUDA(cudaFree(b.p)); b.p = nullptr; b.n = 0; }
     HY_CUDA(cudaMalloc(&b.p, need));
@@ -346,6 +346,7 @@ static int get_wimg(int D, cudaStream_t stream, float** out) {
   *out = b.p;
   return 0;
 }
+static int get_wimg(int D, cudaStream_t stream, float** out) { return get_filter_buf(0, filter_tc_wimg_bytes(D), stream, out); }
 
 static int fill_filter_params(FilterParams* P, const float* z, int z_stride, const float* t, const float* W0,
                               const float* b0, const float* W1, const float* b1, const float* W2, const float* b2,
@@ -416,8 +417,10 @@ HY_API int hyena_b200_filter_bwd_stage2(const float* dh, const float* scratch, c
   HY_CHECK(D >= 1 && D <= 256 && E >= 1 && E <= 8 && L >= 1, "fused filter reduction handles D <= 256, E <= 8 (got D=%d E=%d)", D, E);
   HY_CHECK((reinterpret_cast<uintptr_t>(dh) & 15u) == 0 && (reinterpret_cast<uintptr_t>(scratch) & 15u) == 0 &&
                (reinterpret_cast<uintptr_t>(zT) & 15u) == 0, "misaligned pointer");
+  float* work = nullptr;
+  if (get_filter_buf(1, filter_red_work_bytes(L, D, E), (cudaStream_t)stream, &work)) return 1;
   RedLaunch r{dh, scratch, zT, dW0, db0, dW1, db1, dW2, db2, dW3, dfreq, L, D, E};
-  HY_CUDA(launch_filter_red_tc(r, (cudaStream_t)stream));
+  HY_CUDA(launch_filter_stage2(r, work, (cudaStream_t)stream));
   return 0;
 }
 

@@ -104,15 +104,19 @@ struct Frag {
 template <int R>
 __device__ __forceinline__ void layer_ss(float (&m)[R], float (&c)[R], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi,
                                          uint32_t b_lo, uint32_t acc0) {
+  // four base descriptors, stepped by K (2 core matrices = 256 B = 16 descriptor units per k8 block): 32 precomputed
+  // 64-bit descriptors would hold 64 registers and push the accumulators of the callers into local memory
+  const uint64_t ah = make_desc_ls(a_hi, kLBO, kSBO), al = make_desc_ls(a_lo, kLBO, kSBO);
+  const uint64_t bh = make_desc_ls(b_hi, kLBO, kSBO), bl = make_desc_ls(b_lo, kLBO, kSBO);
+  constexpr uint64_t kStep = 2 * kLBO >> 4;
   wgmma_fence();
   fence_regs(m); fence_regs(c);
 #pragma unroll
-  for (int ks = 0; ks < 8; ++ks)
-    wgmma_ss(m, make_desc_ls(a_hi + ks * 2 * kLBO, kLBO, kSBO), make_desc_ls(b_hi + ks * 2 * kLBO, kLBO, kSBO), (acc0 | ks) ? 1u : 0u);
+  for (int ks = 0; ks < 8; ++ks) wgmma_ss(m, ah + ks * kStep, bh + ks * kStep, (acc0 | ks) ? 1u : 0u);
 #pragma unroll
   for (int ks = 0; ks < 8; ++ks) {
-    wgmma_ss(c, make_desc_ls(a_lo + ks * 2 * kLBO, kLBO, kSBO), make_desc_ls(b_hi + ks * 2 * kLBO, kLBO, kSBO), (acc0 | ks) ? 1u : 0u);
-    wgmma_ss(c, make_desc_ls(a_hi + ks * 2 * kLBO, kLBO, kSBO), make_desc_ls(b_lo + ks * 2 * kLBO, kLBO, kSBO), 1u);
+    wgmma_ss(c, al + ks * kStep, bh + ks * kStep, (acc0 | ks) ? 1u : 0u);
+    wgmma_ss(c, ah + ks * kStep, bl + ks * kStep, 1u);
   }
   wgmma_commit();
 }
@@ -292,8 +296,7 @@ filter_tc_fwd_kernel(const FilterParams P, const float* __restrict__ wimg, float
 //   recompute pre1..3 / a1..3;  da3 = dh W3 (dh = dk * modulation, K = channels in chunks of 64);
 //   dp3 = da3 f cos(f pre3);  da2 = dp3 W2;  dp2 = ...;  da1 = dp2 W1;  dp1 = ...
 // and writes, feature-major (64, L): a1, a2, a3, dp1, dp2, dp3, X = sum_l da_l cos(f pre_l) pre_l, plus dh (D, L).
-// Stage 2 (host side, hyena-dna_b200/ops.py) turns those into the parameter gradients with GEMMs whose reduction
-// dimension is the sequence: dW3 = dh a3, dW2 = dp3^T a2, dW1 = dp2^T a1, dW0 = dp1^T z, db_l = colsum(dp_l),
+// Stage 2 (below) turns those into the parameter gradients with GEMMs whose reduction dimension is the sequence: dW3 = dh a3, dW2 = dp3^T a2, dW1 = dp2^T a1, dW0 = dp1^T z, db_l = colsum(dp_l),
 // dfreq = colsum(X), dz = dp1 W0.
 //
 // Streamed operand images (global, built by filter_tc_prep_bwd_kernel), item i lives in stream buffer i & 1:
@@ -372,32 +375,48 @@ filter_tc_bwd_kernel(const FilterParams P, const float* __restrict__ wimg, const
   __syncthreads();
   const uint32_t a_hi = a_rows(sbase + kOffAhi, f), a_lo = a_rows(sbase + kOffAlo, f);
   const uint32_t bcol = (uint32_t)f.ch * 4u * kSBO;      // this warpgroup's 32 columns of a 64-row B image
-  float fr[16];                                          // this thread's frequencies
+  // Live across the dk chunk loop are only what the epilogues after it cannot get back cheaply: pre2, pre3, the
+  // accumulators and the next chunk's dk.  The frequencies are read from shared memory at each use and pre1 (five FMAs
+  // per element) is recomputed after the loop, in the same order, so that nothing spills at 128 registers.
+  auto fr = [&](int i) { return frs[f.col(i, 32)]; };
+  // pre1 = W0 z + b0 of fragment element i's row t (z of rows t >= L reads as zero)
+  auto layer0 = [&](int i, const float (&z)[kMaxE]) {
+    const int c = f.col(i, 32);
+    float acc = b0s[c];
 #pragma unroll
-  for (int i = 0; i < 16; ++i) fr[i] = frs[f.col(i, 32)];
+    for (int e = 0; e < kMaxE; ++e) acc = fmaf(W0s[c * 16 + e], z[e], acc);
+    return acc;
+  };
+  auto load_z = [&](int t, float (&z)[kMaxE]) {
+#pragma unroll
+    for (int e = 0; e < kMaxE; ++e) z[e] = (t < P.L && e < P.E) ? __ldg(P.z + (size_t)t * P.z_stride + e) : 0.f;
+  };
+
+  // dk of chunk q is pulled into L2 while chunk q - 1's MMAs run (a register prefetch would spill)
+  auto prefetch_dk = [&](int q, int tb) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const int ch = q * 64 + f.col(i, 32), t = tb + f.row(i);
+      if (ch < P.D && t < P.L) asm volatile("prefetch.global.L2 [%0];" ::"l"(dk + (size_t)ch * L + t));
+    }
+  };
 
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const int tb = tile * kTileM;
+    prefetch_dk(0, tb);                                  // lands during the forward recompute
     stream_item(smem, wimg, 0, tid);
     stream_item(smem, wimg, 1, tid);
 
     // ---- forward recompute
-    float pre1[16], pre2[16], pre3[16], a[16];
+    float pre2[16], pre3[16], a[16];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int t = tb + f.r0 + 8 * h;
       float z[kMaxE];
-#pragma unroll
-      for (int e = 0; e < kMaxE; ++e) z[e] = (t < P.L && e < P.E) ? __ldg(P.z + (size_t)t * P.z_stride + e) : 0.f;
+      load_z(tb + f.r0 + 8 * h, z);
 #pragma unroll
       for (int i = 0; i < 16; ++i) {
         if (((i >> 1) & 1) != h) continue;
-        const int c = f.col(i, 32);
-        float acc = b0s[c];
-#pragma unroll
-        for (int e = 0; e < kMaxE; ++e) acc = fmaf(W0s[c * 16 + e], z[e], acc);
-        pre1[i] = acc;
-        a[i] = sin_acc(fr[i] * acc);
+        a[i] = sin_acc(fr(i) * layer0(i, z));
       }
     }
     store_frag16(smem, f, a);
@@ -410,7 +429,7 @@ filter_tc_bwd_kernel(const FilterParams P, const float* __restrict__ wimg, const
       layer_wait(m, c);
       __syncthreads();
 #pragma unroll
-      for (int i = 0; i < 16; ++i) { pre2[i] = (m[i] + c[i]) + b1s[f.col(i, 32)]; a[i] = sin_acc(fr[i] * pre2[i]); }
+      for (int i = 0; i < 16; ++i) { pre2[i] = (m[i] + c[i]) + b1s[f.col(i, 32)]; a[i] = sin_acc(fr(i) * pre2[i]); }
     }
     store_frag16(smem, f, a);
     store_feat16(scratch + 1 * arr, L, f, tb, a);
@@ -422,7 +441,7 @@ filter_tc_bwd_kernel(const FilterParams P, const float* __restrict__ wimg, const
       layer_wait(m, c);
       __syncthreads();
 #pragma unroll
-      for (int i = 0; i < 16; ++i) { pre3[i] = (m[i] + c[i]) + b2s[f.col(i, 32)]; a[i] = sin_acc(fr[i] * pre3[i]); }
+      for (int i = 0; i < 16; ++i) { pre3[i] = (m[i] + c[i]) + b2s[f.col(i, 32)]; a[i] = sin_acc(fr(i) * pre3[i]); }
     }
     store_feat16(scratch + 2 * arr, L, f, tb, a);
 
@@ -434,18 +453,13 @@ filter_tc_bwd_kernel(const FilterParams P, const float* __restrict__ wimg, const
       tpos[h] = t < P.L ? __ldg(P.t + t) : 0.f;
     }
     float m[16], c[16];
-    float nx[16];                                        // dk of the next chunk, loaded one MMA group ahead
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      const int ch = f.col(i, 32), t = tb + f.row(i);
-      nx[i] = (ch < P.D && t < P.L) ? __ldg(dk + (size_t)ch * L + t) : 0.f;
-    }
     for (int q = 0; q < nq; ++q) {
 #pragma unroll
       for (int i = 0; i < 16; ++i) {
         const int ch = q * 64 + f.col(i, 32), t = tb + f.row(i);
-        float x = nx[i];
+        float x = 0.f;
         if (ch < P.D && t < P.L) {
+          x = __ldg(dk + (size_t)ch * L + t);
           if (P.modulate) x *= (expf(-tpos[(i >> 1) & 1] * fabsf(__ldg(P.deltas + ch))) + P.shift);
           dh[(size_t)ch * L + t] = x;
         }
@@ -457,13 +471,7 @@ filter_tc_bwd_kernel(const FilterParams P, const float* __restrict__ wimg, const
       __syncthreads();
       const uint32_t sb = sbase + kOffW3hi + (q & 1) * 32768;
       layer_ss(m, c, a_hi, a_lo, sb + bcol, sb + 16384u + bcol, q > 0 ? 1u : 0u);
-      if (q + 1 < nq) {
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const int ch = (q + 1) * 64 + f.col(i, 32), t = tb + f.row(i);
-          nx[i] = (ch < P.D && t < P.L) ? __ldg(dk + (size_t)ch * L + t) : 0.f;
-        }
-      }
+      if (q + 1 < nq) prefetch_dk(q + 1, tb);
       layer_wait(m, c);
       __syncthreads();
       stream_item(smem, wimg, q + 2, tid);               // refill the buffer this group just released
@@ -473,10 +481,10 @@ filter_tc_bwd_kernel(const FilterParams P, const float* __restrict__ wimg, const
     float X[16];
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
-      const float cs = cos_acc(fr[i] * pre3[i]);
+      const float cs = cos_acc(fr(i) * pre3[i]);
       const float g = (m[i] + c[i]) * cs;
       X[i] = g * pre3[i];
-      a[i] = g * fr[i];
+      a[i] = g * fr(i);
     }
     store_feat16(scratch + 5 * arr, L, f, tb, a);
     store_frag16(smem, f, a);
@@ -491,10 +499,10 @@ filter_tc_bwd_kernel(const FilterParams P, const float* __restrict__ wimg, const
     }
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
-      const float cs = cos_acc(fr[i] * pre2[i]);
+      const float cs = cos_acc(fr(i) * pre2[i]);
       const float g = (m[i] + c[i]) * cs;
       X[i] = fmaf(g, pre2[i], X[i]);
-      a[i] = g * fr[i];
+      a[i] = g * fr(i);
     }
     store_feat16(scratch + 4 * arr, L, f, tb, a);
     store_frag16(smem, f, a);
@@ -507,11 +515,18 @@ filter_tc_bwd_kernel(const FilterParams P, const float* __restrict__ wimg, const
       __syncthreads();                                   // A images and stream buffers are free for the next tile
     }
 #pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      const float cs = cos_acc(fr[i] * pre1[i]);
-      const float g = (m[i] + c[i]) * cs;
-      X[i] = fmaf(g, pre1[i], X[i]);
-      a[i] = g * fr[i];
+    for (int h = 0; h < 2; ++h) {
+      float z[kMaxE];
+      load_z(tb + f.r0 + 8 * h, z);
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        if (((i >> 1) & 1) != h) continue;
+        const float pre1 = layer0(i, z);
+        const float cs = cos_acc(fr(i) * pre1);
+        const float g = (m[i] + c[i]) * cs;
+        X[i] = fmaf(g, pre1, X[i]);
+        a[i] = g * fr(i);
+      }
     }
     store_feat16(scratch + 3 * arr, L, f, tb, a);
     store_feat16(scratch + 6 * arr, L, f, tb, X);
@@ -519,228 +534,65 @@ filter_tc_bwd_kernel(const FilterParams P, const float* __restrict__ wimg, const
 }
 
 // ---------------------------------------------------------------------------------------------- backward, stage 2
-// All parameter gradients of the filter are reductions over the sequence.  With the stage-1 arrays stored feature-
-// major every operand is K-major with K = position, so they are three accumulating wgmma GEMM groups whose fp32
-// accumulators stay in registers (persistent CTAs, split over the sequence, an atomic flush every kRedChain K blocks):
-//   G1  dW3[c][j]      = sum_t dh[c][t] a3[j][t]                       M = 128 channels per tile (<= 2 tiles), N = 64
-//   G2  [dp3;dp2] x [a2;a1;1]^T : block(0,0) = dW2, block(1,1) = dW1, column 128 = (db2 ; db1)     M = 128, N = 144
-//   G3  [dp1;X]  x [z;1]^T      : rows 0..63 -> (dW0 | db0), rows 64..127 col 8 -> dfreq             M = 128, N = 16
-// K block = 32 positions (operand images: K-major, SBO 1024 B, LBO 128 B), 3xTF32 like everywhere else.
-constexpr int kRedKB = 32;
-constexpr int kRedThreads = 512;
-constexpr int kRedItems = 12;                // ceil(8 * roundup8(256 + 7*64 + emb_dim) / 512)
-constexpr uint32_t kRedSBO = 1024;
-__host__ __device__ constexpr uint32_t red_off(int r, int k) {
-  return (uint32_t)((r >> 3) * 1024 + (k >> 2) * 128 + (r & 7) * 16 + (k & 3) * 4);
-}
-constexpr uint32_t kRedImg128 = 128 * kRedKB * 4;      // bytes of a 128-row image (16 KB)
-// shared memory map (bytes); every operand has a hi image followed by a lo image
-constexpr uint32_t kRedOffDh = 0;                                  // 2 tiles x (hi 16K + lo 16K) = 64 KB
-constexpr uint32_t kRedOffAs = 65536;                              // [dp3;dp2]   32 KB
-constexpr uint32_t kRedOffAx = kRedOffAs + 32768;                  // [dp1;X]     32 KB
-constexpr uint32_t kRedOffB3 = kRedOffAx + 32768;                  // a3 (64 rows): hi 8K + lo 8K
-constexpr uint32_t kRedOffBs = kRedOffB3 + 16384;                  // [a2;a1;ones16] 144 rows: hi 18K + lo 18K
-constexpr uint32_t kRedOffBz = kRedOffBs + 36864;                  // [z pad 8; ones 8] 16 rows: hi 2K + lo 2K
-constexpr uint32_t kRedOffMisc = kRedOffBz + 4096;
-constexpr size_t kRedSmemBytes = kRedOffMisc + 64;
-
-// D (+)= A * B^T over one K block of 32 positions as 3xTF32, all products into one accumulator (restarted every
-// kRedChain blocks, see below)
-template <int R>
-__device__ __forceinline__ void issue_red(float (&d)[R], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo, uint32_t first_acc) {
-  uint32_t acc = first_acc;
-#pragma unroll
-  for (int pass = 0; pass < 3; ++pass) {
-    const uint32_t a = (pass == 1) ? a_lo : a_hi;
-    const uint32_t b = (pass == 2) ? b_lo : b_hi;
-#pragma unroll
-    for (int ks = 0; ks < kRedKB / 8; ++ks) {
-      wgmma_ss(d, make_desc_ls(a + ks * 2 * kLBO, kLBO, kRedSBO), make_desc_ls(b + ks * 2 * kLBO, kLBO, kRedSBO), acc);
-      acc = 1;
-    }
-  }
+// All parameter gradients of the filter are reductions over the sequence of the stage-1 arrays.  They run as three
+// channel-major weight-gradient GEMMs (proj_gemm.cuh wgrad_ych_kernel: dW^T = sum_pos Y[n][pos] X[m][pos], 3xTF32,
+// running sums in registers, fixed-order split-K partials), on operands the scratch order a1 a2 a3 dp1 dp2 dp3 X
+// makes contiguous:
+//   P1  X = dh (D rows),               Y = a3:          dW3[c][j] = T[j][c]
+//   P2  X = [dp2; dp3] (128 rows),     Y = [a1; a2]:    dW1 = block (0, 0), dW2 = block (1, 1) (the off-diagonal blocks
+//                                                        are not needed)
+//   P3  X = [dp1; dp2; dp3; X],        Y = [zT; 1]:     dW0[j][e] = T[e][j], db0 / db1 / db2 / dfreq = T[E][64 l + j]
+// then filter_red_finish_kernel sums each call's partials in split order and adds them into the gradients.
+// [zT; 1] (E + 1, L) is built next to the partials by filter_red_ones_kernel.
+__global__ void filter_red_ones_kernel(const float* __restrict__ zT, int E, int L, float* __restrict__ zt1) {
+  const size_t nz = (size_t)E * L, total = nz + (size_t)L;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x)
+    zt1[i] = i < nz ? __ldg(zT + i) : 1.f;
 }
 
-// four consecutive positions of a feature row (zero beyond L); vector load when rows are 16-byte aligned
-__device__ __forceinline__ float4 load4_row(const float* __restrict__ src, size_t t, size_t L, bool v4) {
-  float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (v4 && t + 3 < L) return __ldg(reinterpret_cast<const float4*>(src + t));
-  if (t < L) x.x = __ldg(src + t);
-  if (t + 1 < L) x.y = __ldg(src + t + 1);
-  if (t + 2 < L) x.z = __ldg(src + t + 2);
-  if (t + 3 < L) x.w = __ldg(src + t + 3);
-  return x;
-}
-
-struct RedArgs {
-  const float* dh;        // (D, L)
-  const float* scratch;   // (7, 64, L): a1 a2 a3 dp1 dp2 dp3 X
-  const float* zT;        // (E, L)
+struct RedFinish {
+  const float* p1; const float* p2; const float* p3;   // (s1, 64, D), (s2, 128, 128), (s3, E + 1, 256) partials
+  int s1, s2, s3;
   float* dW0; float* db0; float* dW1; float* db1; float* dW2; float* db2; float* dW3; float* dfreq;
-  int L, D, E;
+  int D, E;
 };
 
-// Work items: (row, 4-position piece) pairs, 8 pieces per row; item w = tid + kRedThreads*it, so every item of a thread
-// has the same piece index (tid >> 3) & 7.  Inside every group of 64 items the ROW runs fastest (row = 8 (w >> 6) + (w & 7),
-// piece = (w >> 3) & 7), so the eight lanes of a quarter warp write the eight 16-byte rows of ONE core matrix = 128
-// contiguous bytes (conflict free), and a warp reads 64 contiguous bytes of each of eight rows.
-struct RedItem { const float* src; uint32_t off; uint32_t lo_off; };
-__device__ __forceinline__ RedItem red_item(const RedArgs& R, int it, int tid) {
-  const size_t L = (size_t)R.L;
-  const int nrow = R.D + 7 * 64 + R.E;                   // dh rows, six (64,L) arrays + X, z rows
-  const int pc = (tid >> 3) & 7;
-  const int row = (((tid + kRedThreads * it) >> 6) << 3) + (tid & 7);
-  RedItem m{nullptr, 0u, 0u};
-  uint32_t img = 0, lo = 0;
-  int r = 0;
-  if (row < R.D) {
-    m.src = R.dh + (size_t)row * L; img = kRedOffDh + (row >> 7) * 32768; lo = 16384; r = row & 127;
-  } else if (row < nrow) {
-    const int q = row - R.D;
-    if (q < 7 * 64) {
-      const int arr = q >> 6, f = q & 63;                // scratch order: a1 a2 a3 dp1 dp2 dp3 X
-      m.src = R.scratch + ((size_t)arr * 64 + f) * L;
-      switch (arr) {
-        case 0: img = kRedOffBs; lo = 18432; r = 64 + f; break;     // a1  -> B_s rows 64..127
-        case 1: img = kRedOffBs; lo = 18432; r = f; break;          // a2  -> B_s rows 0..63
-        case 2: img = kRedOffB3; lo = 8192; r = f; break;           // a3
-        case 3: img = kRedOffAx; lo = 16384; r = f; break;          // dp1 -> A_x rows 0..63
-        case 4: img = kRedOffAs; lo = 16384; r = 64 + f; break;     // dp2 -> A_s rows 64..127
-        case 5: img = kRedOffAs; lo = 16384; r = f; break;          // dp3 -> A_s rows 0..63
-        default: img = kRedOffAx; lo = 16384; r = 64 + f; break;    // X   -> A_x rows 64..127
-      }
-    } else {
-      const int e = q - 7 * 64;                          // z feature e -> B_z row e
-      m.src = R.zT + (size_t)e * L; img = kRedOffBz; lo = 2048; r = e;
-    }
-  }
-  m.off = img + red_off(r, 4 * pc);
-  m.lo_off = lo;
-  return m;
+__device__ __forceinline__ float sum_splits(const float* p, size_t stride, int splits) {
+  float s = 0.f;
+  for (int k = 0; k < splits; ++k) s += __ldg(p + (size_t)k * stride);
+  return s;
 }
 
-// K blocks per accumulator chain.  The tensor core truncates every add into its accumulator, so a chain of n MMAs biases
-// the sum towards zero by ~n 2^-24 of its magnitude: one chain through a CTA's whole slice of a 2^20-position sequence
-// (~250 blocks x 12 MMAs) put same-sign sums 8.5e-5 (relative) off, 100x the error of an fp32 library GEMM.  So every
-// kRedChain blocks the accumulators are flushed into the gradients with round-to-nearest atomic adds and restarted.
-// Shorter chains trade the bias for more atomic adds per gradient element (their own rounding) and time: on an H100
-// (400 W) at L = 2^20, D = 256 the kernel took 5.4 ms with one chain, 5.65 ms with 8 blocks, 6.0 ms with 4, 7.3 ms with 2.
-constexpr int kRedChain = 8;
-
-// accumulators -> gradients (fragment element i: row f.row(i) of the group, column f.col(i, n_half))
-__device__ __forceinline__ void red_flush(const RedArgs& R, const Frag& f, int nmt, const float (&g1)[2][16],
-                                          const float (&g2)[36], const float (&g3)[4]) {
-  for (int mt = 0; mt < nmt; ++mt) {                       // G1: dW3 rows c = 128 mt + row, 64 columns
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      const int c = mt * 128 + f.row(i);
-      if (c < R.D) atomicAdd(R.dW3 + (size_t)c * 64 + f.col(i, 32), g1[mt][i]);
+// one thread per gradient element: dW3 (D x 64), dW1, dW2 (64 x 64), dW0 (64 x E), db0, db1, db2, dfreq (64 each),
+// numbered so that consecutive threads read consecutive partials
+__global__ void filter_red_finish_kernel(const RedFinish r) {
+  const int n3 = r.D * 64, n12 = 64 * 64, n0 = 64 * r.E;
+  const int total = n3 + 2 * n12 + n0 + 4 * 64;
+  const size_t st1 = (size_t)64 * r.D, st2 = 128 * 128, st3 = (size_t)(r.E + 1) * 256;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+    int q = i;
+    if (q < n3) {
+      const int j = q / r.D, c = q % r.D;
+      r.dW3[c * 64 + j] += sum_splits(r.p1 + q, st1, r.s1);
+      continue;
     }
-  }
-  // G2: rows < 64: cols 0..63 -> dW2[row][j]; rows >= 64: cols 64..127 -> dW1[row-64][j]; col 128 -> db2 / db1
-#pragma unroll
-  for (int i = 0; i < 36; ++i) {
-    const int r = f.row(i), n = f.col(i, 72);
-    if (n == 128) atomicAdd(((r < 64) ? R.db2 : R.db1) + (r & 63), g2[i]);
-    else if (r < 64 && n < 64) atomicAdd(R.dW2 + r * 64 + n, g2[i]);
-    else if (r >= 64 && n >= 64 && n < 128) atomicAdd(R.dW1 + (r - 64) * 64 + (n - 64), g2[i]);
-  }
-  // G3: rows < 64: cols 0..E-1 -> dW0[row][e], col 8 -> db0[row]; rows >= 64: col 8 -> dfreq[row-64]
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int r = f.row(i), n = f.col(i, 8);
-    if (r < 64) {
-      if (n < R.E) atomicAdd(R.dW0 + r * R.E + n, g3[i]);
-      else if (n == 8) atomicAdd(R.db0 + r, g3[i]);
-    } else if (n == 8) {
-      atomicAdd(R.dfreq + (r - 64), g3[i]);
+    q -= n3;
+    if (q < 2 * n12) {
+      const int l = q / n12, k = (q % n12) / 64, j = q % 64;     // l = 0: dW1 = dp2 a1^T, l = 1: dW2 = dp3 a2^T
+      (l ? r.dW2 : r.dW1)[j * 64 + k] += sum_splits(r.p2 + (size_t)(64 * l + k) * 128 + 64 * l + j, st2, r.s2);
+      continue;
     }
-  }
-}
-
-__global__ void __launch_bounds__(kRedThreads, 1) filter_tc_red_kernel(const RedArgs R, int nblocks) {
-  extern __shared__ __align__(1024) unsigned char smem[];
-  const int tid = threadIdx.x;
-  const Frag f(tid);
-  const uint32_t sbase = smem_u32(smem);
-  const int nmt = (R.D + 127) / 128;                       // channel tiles (host guarantees <= 2)
-  const size_t L = (size_t)R.L;
-  const bool v4 = (R.L & 3) == 0;
-  const int pc = (tid >> 3) & 7;
-
-  // zero every image once (rows that are never loaded -- channel padding, z padding -- stay zero), then the ones rows
-  for (uint32_t i = tid; i < kRedOffMisc / 16; i += kRedThreads) reinterpret_cast<float4*>(smem)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  __syncthreads();
-  for (int i = tid; i < 16 * kRedKB; i += kRedThreads) {   // [a2;a1;ones16]: rows 128..143 hi = 1
-    const int r = 128 + i / kRedKB, k = i % kRedKB;
-    *reinterpret_cast<float*>(smem + kRedOffBs + red_off(r, k)) = 1.f;
-  }
-  for (int i = tid; i < 8 * kRedKB; i += kRedThreads) {    // [z;ones8]: rows 8..15 hi = 1
-    const int r = 8 + i / kRedKB, k = i % kRedKB;
-    *reinterpret_cast<float*>(smem + kRedOffBz + red_off(r, k)) = 1.f;
-  }
-  __syncthreads();
-
-  // accumulators of this warpgroup: rows 64 rh .. of every group, column half ch
-  float g1[2][16], g2[36], g3[4];
-  const uint32_t arow = (uint32_t)f.rh * 8u * kRedSBO;
-  bool first = true;                                       // no MMA issued yet
-  int chain = 0;                                           // K blocks in the accumulators since their last flush
-  for (int blk = blockIdx.x; blk < nblocks; blk += gridDim.x) {
-    const size_t t = (size_t)blk * kRedKB + 4 * pc;
-    if (!first) {                                          // previous MMAs have read the images
-      wgmma_wait<0>();
-      fence_regs(g1[0]); fence_regs(g1[1]); fence_regs(g2); fence_regs(g3);
-      __syncthreads();
+    q -= 2 * n12;
+    if (q < n0) {
+      const int e = q / 64, j = q % 64;
+      r.dW0[j * r.E + e] += sum_splits(r.p3 + (size_t)e * 256 + j, st3, r.s3);
+      continue;
     }
-#pragma unroll
-    for (int half = 0; half < 2; ++half) {
-      constexpr int kH = kRedItems / 2;
-      float4 x[kH];
-      RedItem m[kH];
-#pragma unroll
-      for (int j = 0; j < kH; ++j) {                       // all loads of this half block in flight at once
-        m[j] = red_item(R, half * kH + j, tid);
-        x[j] = m[j].src ? load4_row(m[j].src, t, L, v4) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-#pragma unroll
-      for (int j = 0; j < kH; ++j) {
-        if (m[j].src) {
-          float4 hi, lo;
-          split_tf32(x[j].x, hi.x, lo.x); split_tf32(x[j].y, hi.y, lo.y);
-          split_tf32(x[j].z, hi.z, lo.z); split_tf32(x[j].w, hi.w, lo.w);
-          *reinterpret_cast<float4*>(smem + m[j].off) = hi;
-          *reinterpret_cast<float4*>(smem + m[j].off + m[j].lo_off) = lo;
-        }
-      }
-    }
-    fence_async_smem();
-    __syncthreads();
-    const uint32_t acc0 = chain ? 1u : 0u;
-    wgmma_fence();
-    fence_regs(g1[0]); fence_regs(g1[1]); fence_regs(g2); fence_regs(g3);
-#pragma unroll
-    for (int mt = 0; mt < 2; ++mt)
-      if (mt < nmt)
-        issue_red(g1[mt], sbase + kRedOffDh + mt * 32768 + arow, sbase + kRedOffDh + mt * 32768 + 16384 + arow,
-                  sbase + kRedOffB3 + f.ch * 4 * kRedSBO, sbase + kRedOffB3 + 8192 + f.ch * 4 * kRedSBO, acc0);
-    issue_red(g2, sbase + kRedOffAs + arow, sbase + kRedOffAs + 16384 + arow, sbase + kRedOffBs + f.ch * 9 * kRedSBO,
-              sbase + kRedOffBs + 18432 + f.ch * 9 * kRedSBO, acc0);
-    issue_red(g3, sbase + kRedOffAx + arow, sbase + kRedOffAx + 16384 + arow, sbase + kRedOffBz + f.ch * kRedSBO,
-              sbase + kRedOffBz + 2048 + f.ch * kRedSBO, acc0);
-    wgmma_commit();
-    first = false;
-    if (++chain == kRedChain) {                            // the images stay untouched until the barrier at the loop top
-      wgmma_wait<0>();
-      fence_regs(g1[0]); fence_regs(g1[1]); fence_regs(g2); fence_regs(g3);
-      red_flush(R, f, nmt, g1, g2, g3);
-      chain = 0;
-    }
+    q -= n0;
+    const int l = q / 64, j = q % 64;
+    float* dst = l == 0 ? r.db0 : l == 1 ? r.db1 : l == 2 ? r.db2 : r.dfreq;
+    dst[j] += sum_splits(r.p3 + (size_t)r.E * 256 + q, st3, r.s3);
   }
-  if (chain == 0) return;
-  wgmma_wait<0>();
-  fence_regs(g1[0]); fence_regs(g1[1]); fence_regs(g2); fence_regs(g3);
-  red_flush(R, f, nmt, g1, g2, g3);
 }
 
 }  // namespace tc

@@ -146,8 +146,20 @@ size_t proj_wgrad_scratch_bytes(int M, int N) {
   return (size_t)sp * M * N * sizeof(float);
 }
 
-cudaError_t launch_proj_wgrad(const float* X, const float* Y, const float* fir, float* dW, int transposed_out, float beta,
-                              int B, int L, int M, int N, float* part, cudaStream_t s, int fn) {
+template <int FN, bool YCH>
+static cudaError_t wgrad_go(const wg::Args& a, const CUtensorMap& tmx, const CUtensorMap& tmy, int kind, cudaStream_t s) {
+  auto kern = YCH ? wg::wgrad_ych_kernel : wg::wgrad_kernel<FN>;
+  const size_t smem = wg::Lay<YCH>::Smem;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  prof_begin(kind, s);
+  kern<<<a.mtiles * a.ntiles * a.splits, wg::kThreads, smem, s>>>(a, tmx, tmy);
+  prof_end(kind, s);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_wgrad_part(const float* X, const float* Y, int y_ch, const float* fir, int B, int L, int M, int N,
+                              float* part, cudaStream_t s, int fn, int kind, int* splits) {
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
@@ -157,31 +169,40 @@ cudaError_t launch_proj_wgrad(const float* X, const float* Y, const float* fir, 
   proj_wgrad_plan(M, N, sms, &a.mtiles, &a.ntiles, &a.splits);
   const long long total_chunks = (long long)B * a.chunks_per_b;
   if (a.splits > total_chunks) a.splits = (int)total_chunks;
-  a.vec = (L % 4 == 0) && (N % 4 == 0) && ((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(Y)) & 15u) == 0;
+  *splits = a.splits;
+  // a row-major Y needs 16-byte aligned rows of N floats, a channel-major one rows of L floats (as X)
+  a.vec = (L % 4 == 0) && (y_ch || N % 4 == 0) &&
+          ((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(Y)) & 15u) == 0;
   CUtensorMap tmx, tmy;
   memset(&tmx, 0, sizeof(tmx)); memset(&tmy, 0, sizeof(tmy));
   if (a.vec) {
-    // X (B, M, L): box 36 positions x 128 rows;  Y (B, L, N): box 128 columns x 32 positions
+    // X (B, M, L): box 36 positions x 128 rows;  Y (B, L, N): box 128 columns x 32 positions, (B, N, L): as X
     const bool ok = make_tmap3(&tmx, X, (unsigned long long)L, (unsigned long long)M, (unsigned long long)B, 36, 128) &&
-                    make_tmap3(&tmy, Y, (unsigned long long)N, (unsigned long long)L, (unsigned long long)B, 128, 32);
+                    (y_ch ? make_tmap3(&tmy, Y, (unsigned long long)L, (unsigned long long)N, (unsigned long long)B, 36, 128)
+                          : make_tmap3(&tmy, Y, (unsigned long long)N, (unsigned long long)L, (unsigned long long)B, 128, 32));
     if (!ok) a.vec = 0;                  // no driver entry point / unencodable shape: the producer warp stages by hand
   }
-  auto kern = fn == FN_GELU_TANH ? wg::wgrad_kernel<FN_GELU_TANH>
-            : fn == FN_GELU_ERF  ? wg::wgrad_kernel<FN_GELU_ERF> : wg::wgrad_kernel<FN_NONE>;
+  if (y_ch) return (fn == FN_NONE && !fir) ? wgrad_go<FN_NONE, true>(a, tmx, tmy, kind, s) : cudaErrorInvalidValue;
   if (fn != FN_NONE && (fir || (fn != FN_GELU_TANH && fn != FN_GELU_ERF))) return cudaErrorInvalidValue;
+  if (fn == FN_GELU_TANH) return wgrad_go<FN_GELU_TANH, false>(a, tmx, tmy, kind, s);
+  if (fn == FN_GELU_ERF) return wgrad_go<FN_GELU_ERF, false>(a, tmx, tmy, kind, s);
+  return wgrad_go<FN_NONE, false>(a, tmx, tmy, kind, s);
+}
+
+cudaError_t launch_proj_wgrad(const float* X, const float* Y, const float* fir, float* dW, int transposed_out, float beta,
+                              int B, int L, int M, int N, float* part, cudaStream_t s, int fn) {
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int kind = fn == FN_NONE ? K_PROJ_WGRAD : K_PROJ_WGRAD_GELU;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wg::kSmem);
-  if (e != cudaSuccess) return e;
-  prof_begin(kind, s);
-  kern<<<a.mtiles * a.ntiles * a.splits, wg::kThreads, wg::kSmem, s>>>(a, tmx, tmy);
-  prof_end(kind, s);
-  e = cudaGetLastError();
+  int splits = 1;
+  cudaError_t e = launch_wgrad_part(X, Y, 0, fir, B, L, M, N, part, s, fn, kind, &splits);
   if (e != cudaSuccess) return e;
   const size_t total = (size_t)M * N;
   int blocks = (int)((total + 255) / 256);
   if (blocks > 2 * sms) blocks = 2 * sms;
   prof_begin(kind, s);
-  wg::wgrad_reduce_kernel<<<blocks, 256, 0, s>>>(part, dW, a.splits, M, N, transposed_out, beta);
+  wg::wgrad_reduce_kernel<<<blocks, 256, 0, s>>>(part, dW, splits, M, N, transposed_out, beta);
   prof_end(kind, s);
   return cudaGetLastError();
 }

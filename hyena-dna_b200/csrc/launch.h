@@ -38,7 +38,8 @@ size_t filter_tc_wimg_bytes(int D);
 cudaError_t launch_filter_bwd_tc(const FilterParams& P, float* wimg, const float* dk, float* dh, float* scratch, cudaStream_t s);
 struct RedLaunch { const float* dh; const float* scratch; const float* zT; float* dW0; float* db0; float* dW1; float* db1;
                    float* dW2; float* db2; float* dW3; float* dfreq; int L, D, E; };
-cudaError_t launch_filter_red_tc(const RedLaunch& r, cudaStream_t s);   // k_filter_tc.cu
+size_t filter_red_work_bytes(int L, int D, int E);                       // k_filter_tc.cu
+cudaError_t launch_filter_stage2(const RedLaunch& r, float* work, cudaStream_t s);
 cudaError_t launch_filter_bwd(const FilterParams& P, const float* dk, const FilterGrads& G, cudaStream_t s);
 cudaError_t launch_short_bwd(const ShortBwdArgs& a, int B, cudaStream_t s);
 cudaError_t launch_twiddle_init(float2* tw1024, float2* twlo, cudaStream_t s);
@@ -50,6 +51,10 @@ cudaError_t launch_proj_gemm(const float* act, int act_layout, const float* W, i
 size_t proj_wgrad_scratch_bytes(int M, int N);
 cudaError_t launch_proj_wgrad(const float* X, const float* Y, const float* fir, float* dW, int transposed_out, float beta,
                               int B, int L, int M, int N, float* part, cudaStream_t s, int fn = 0);
+// wgrad_kernel alone: X (B, M, L) times Y (B, L, N), or (B, N, L) when y_ch; writes the partials (splits, N, M) of the
+// transposed product (proj_wgrad_scratch_bytes(M, N) bytes) and returns the split count in *splits
+cudaError_t launch_wgrad_part(const float* X, const float* Y, int y_ch, const float* fir, int B, int L, int M, int N,
+                              float* part, cudaStream_t s, int fn, int kind, int* splits);
 // k_filter.cu: filter_extra.cuh
 cudaError_t launch_filter_ddelta(const float* dk, const float* k, const float* t, const float* deltas, float shift, int D,
                                  int L, float* ddelta, cudaStream_t s);

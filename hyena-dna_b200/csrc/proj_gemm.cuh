@@ -391,6 +391,9 @@ __global__ void __launch_bounds__(kThreads, 1) proj_gemm_kernel(const Args a, co
 //   registers acc 64 + sum 64 + A fragments 32 + next chunk's Y 16 per consumer thread: whole warpgroups, and moves
 //             registers from the converter and producer warpgroups to the consumers (setmaxnreg).
 //   overlap   the next chunk's Y values are loaded while this chunk's MMAs run; the converters fill the other image pair.
+//   YCH       Y channel-major (B, N, L) instead of (B, L, N) (the implicit filter's feature-major backward arrays): the Y
+//             tile is staged like the X tile, 128 rows n x 36 positions (the 144-byte pitch keeps the A-fragment loads of
+//             a warp -- 8 rows x 4 positions -- bank-conflict free; the 4 look-ahead positions are not used)
 namespace wg {
 
 constexpr int kThreads = 512;             // warpgroups: 0, 1 consumers; 2 X -> B images; 3 TMA producer (one warp)
@@ -403,17 +406,21 @@ constexpr uint32_t kYStage = 32 * kYPitch;            // 32 positions
 constexpr uint32_t kXPitch = 36 * 4;      // staged X row: 32 positions + one look-ahead quad (fused FIR)
 constexpr uint32_t kXStage = 128 * kXPitch;           // 128 rows
 constexpr uint32_t kImg = 128 * 32 * 4;               // one 128 x 32 operand image (16 KB)
-constexpr uint32_t kOffY = 0, kOffX = kOffY + kStg * kYStage;
-constexpr uint32_t kOffImg = (kOffX + kStg * kXStage + 1023u) & ~1023u;                       // images: [2][hi | lo]
-constexpr uint32_t kOffBar = kOffImg + 2 * 2 * kImg;
-constexpr size_t kSmem = kOffBar + 256;
-static_assert(kOffImg % 1024 == 0, "operand images must start on a core-matrix group boundary");
 static_assert(kYStage % 128 == 0 && kXStage % 128 == 0, "TMA destinations are 128-byte aligned");
-static_assert(kSmem <= 227 * 1024, "shared memory budget");
+// shared memory map: Y ring, X ring, images [2][hi | lo], barriers; a channel-major Y is staged at the X pitch
+template <bool YCH> struct Lay {
+  static constexpr uint32_t YStage = YCH ? kXStage : kYStage;
+  static constexpr uint32_t OffY = 0, OffX = OffY + kStg * YStage;
+  static constexpr uint32_t OffImg = (OffX + kStg * kXStage + 1023u) & ~1023u;
+  static constexpr uint32_t OffBar = OffImg + 2 * 2 * kImg;
+  static constexpr size_t Smem = OffBar + 256;
+  static_assert(OffImg % 1024 == 0, "operand images must start on a core-matrix group boundary");
+  static_assert(Smem <= 227 * 1024, "shared memory budget");
+};
 
 struct Args {
   const float* X;       // (B, M, L)
-  const float* Y;       // (B, L, N)
+  const float* Y;       // (B, L, N), or (B, N, L) for YCH
   const float* fir;     // (M, 3) or null
   float* part;          // (splits, N, M) partial sums of the TRANSPOSED product
   int B, L, M, N;
@@ -428,11 +435,14 @@ struct Args {
 // the fused FIR), completion on an mbarrier per stage.  Out-of-range rows / columns / positions are zero-filled by the
 // copy engine (tails of M, N and L; the 3-D maps keep a tile from running into the next batch).
 // FN != FN_NONE: the product is taken with gelu(X) (fir must be null), applied by the converter warps.
-template <int FN = FN_NONE>
-__global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const Args a, const __grid_constant__ CUtensorMap tmapX,
-                                                            const __grid_constant__ CUtensorMap tmapY) {
+// YCH: Y is (B, N, L); its tile is one copy of box 36 pos x 128 n of the (L, N, B) tensor, like X's.
+// The body of wgrad_kernel (row-major Y) and wgrad_ych_kernel (channel-major Y), which pass their tensor maps.
+template <int FN, bool YCH>
+__device__ __forceinline__ void wgrad_body(const Args& a, const CUtensorMap* tmapX, const CUtensorMap* tmapY) {
+  static_assert(!YCH || FN == FN_NONE, "the channel-major Y variant has no fused activation");
+  using Ly = Lay<YCH>;
   extern __shared__ __align__(1024) unsigned char smem[];
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBar);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Ly::OffBar);
   // barriers: b_full[2] b_empty[2] s_full[4] y_empty[4] x_empty[4]
   const uint32_t sbase = tc::smem_u32(smem), bar0 = tc::smem_u32(bars);
   auto B_FULL = [&](int s) { return bar0 + 8u * s; };
@@ -471,14 +481,15 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const Args a, const 
     auto load_y = [&](long long q) {
       const int ss = (int)(q % kStg);
       tc::mbar_wait_u(S_FULL(ss), (uint32_t)(q / kStg) & 1u);            // the producer's copies of this chunk have landed
-      const unsigned char* st = smem + kOffY + (size_t)ss * kYStage;
+      const unsigned char* st = smem + Ly::OffY + (size_t)ss * Ly::YStage;
       uint32_t dep = 0;
 #pragma unroll
       for (int ks = 0; ks < 4; ++ks) {
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
           const int nl = nl0 + ((e & 1) ? 8 : 0), k = 8 * ks + t + ((e & 2) ? 4 : 0);
-          yv[ks][e] = *reinterpret_cast<const float*>(st + k * kYPitch + nl * 4);
+          if constexpr (YCH) yv[ks][e] = *reinterpret_cast<const float*>(st + nl * kXPitch + k * 4);
+          else yv[ks][e] = *reinterpret_cast<const float*>(st + k * kYPitch + nl * 4);
           dep |= __float_as_uint(yv[ks][e]);
         }
       }
@@ -499,7 +510,7 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const Args a, const 
       const uint32_t it = (uint32_t)q;
       const int s = it & 1;
       tc::mbar_wait_u(B_FULL(s), (it >> 1) & 1);
-      const uint32_t bhi = sbase + kOffImg + s * 2 * kImg, blo = bhi + kImg;
+      const uint32_t bhi = sbase + Ly::OffImg + s * 2 * kImg, blo = bhi + kImg;
       const uint32_t cont = (it % kSeg) != 0;                           // 0: this chunk starts a segment
       tc::wgmma_fence();
       tc::fence_regs(acc);
@@ -558,11 +569,11 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const Args a, const 
     for (long long q = 0; q < nchunks; ++q) {
       const int ss = (int)(q % kStg);
       tc::mbar_wait_u(S_FULL(ss), (uint32_t)(q / kStg) & 1u);
-      const unsigned char* st = smem + kOffX + (size_t)ss * kXStage;
+      const unsigned char* st = smem + Ly::OffX + (size_t)ss * kXStage;
       const uint32_t it = (uint32_t)q;
       const int s = it & 1;
       tc::mbar_wait_u(B_EMPTY(s), ((it >> 1) & 1) ^ 1);                 // the MMAs that read this image pair are done
-      unsigned char* hi_img = smem + kOffImg + (size_t)s * 2 * kImg;
+      unsigned char* hi_img = smem + Ly::OffImg + (size_t)s * 2 * kImg;
       unsigned char* lo_img = hi_img + kImg;
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
@@ -597,7 +608,7 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const Args a, const 
     // ---------------------------------------------------------------- producer: Y and X tiles of every chunk (TMA)
     tc::setmaxnreg_dec<kRegProducer>();
     if (warp != 12) return;
-    if (lane == 0 && a.vec) { tc::tma_prefetch_desc(&tmapX); tc::tma_prefetch_desc(&tmapY); }
+    if (lane == 0 && a.vec) { tc::tma_prefetch_desc(tmapX); tc::tma_prefetch_desc(tmapY); }
     int sb_ = (int)(c_begin / a.chunks_per_b), sl_ = (int)(c_begin - (long long)sb_ * a.chunks_per_b) * 32;
     for (long long q = 0; q < nchunks; ++q) {
       const int ss = (int)(q % kStg);
@@ -609,18 +620,26 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const Args a, const 
       tc::mbar_wait_u(X_EMPTY(ss), par);
       if (a.vec) {
         if (lane == 0) {
-          tc::mbar_arrive_expect_tx(S_FULL(ss), kYStage + kXStage);
-          tc::tma_load_3d(sbase + kOffY + ss * kYStage, &tmapY, n0, l0, b, S_FULL(ss));
-          tc::tma_load_3d(sbase + kOffX + ss * kXStage, &tmapX, l0, m0, b, S_FULL(ss));
+          tc::mbar_arrive_expect_tx(S_FULL(ss), Ly::YStage + kXStage);
+          if constexpr (YCH) tc::tma_load_3d(sbase + Ly::OffY + ss * Ly::YStage, tmapY, l0, n0, b, S_FULL(ss));
+          else tc::tma_load_3d(sbase + Ly::OffY + ss * Ly::YStage, tmapY, n0, l0, b, S_FULL(ss));
+          tc::tma_load_3d(sbase + Ly::OffX + ss * kXStage, tmapX, l0, m0, b, S_FULL(ss));
         }
       } else {
         // rows that do not qualify for TMA: the 32 lanes stage the tiles with plain loads (zero fill outside the tensors)
-        float* ys = reinterpret_cast<float*>(smem + kOffY + (size_t)ss * kYStage);
-        for (int i = lane; i < 32 * 128; i += 32) {
-          const int k = i >> 7, n = i & 127, l = l0 + k;
-          ys[i] = (l < a.L && n0 + n < a.N) ? __ldg(a.Y + ((size_t)b * a.L + l) * a.N + n0 + n) : 0.f;
+        float* ys = reinterpret_cast<float*>(smem + Ly::OffY + (size_t)ss * Ly::YStage);
+        if constexpr (YCH) {
+          for (int i = lane; i < 128 * 36; i += 32) {
+            const int n = i / 36, e = i - n * 36, l = l0 + e;
+            ys[i] = (n0 + n < a.N && l < a.L) ? __ldg(a.Y + ((size_t)b * a.N + n0 + n) * a.L + l) : 0.f;
+          }
+        } else {
+          for (int i = lane; i < 32 * 128; i += 32) {
+            const int k = i >> 7, n = i & 127, l = l0 + k;
+            ys[i] = (l < a.L && n0 + n < a.N) ? __ldg(a.Y + ((size_t)b * a.L + l) * a.N + n0 + n) : 0.f;
+          }
         }
-        float* xs = reinterpret_cast<float*>(smem + kOffX + (size_t)ss * kXStage);
+        float* xs = reinterpret_cast<float*>(smem + Ly::OffX + (size_t)ss * kXStage);
         for (int i = lane; i < 128 * 36; i += 32) {
           const int r = i / 36, e = i - r * 36, l = l0 + e;
           xs[i] = (m0 + r < a.M && l < a.L) ? __ldg(a.X + ((size_t)b * a.M + m0 + r) * a.L + l) : 0.f;
@@ -630,6 +649,16 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const Args a, const 
       }
     }
   }
+}
+
+template <int FN = FN_NONE>
+__global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const Args a, const __grid_constant__ CUtensorMap tmapX,
+                                                            const __grid_constant__ CUtensorMap tmapY) {
+  wgrad_body<FN, false>(a, &tmapX, &tmapY);
+}
+__global__ void __launch_bounds__(kThreads, 1) wgrad_ych_kernel(const Args a, const __grid_constant__ CUtensorMap tmapX,
+                                                                const __grid_constant__ CUtensorMap tmapY) {
+  wgrad_body<FN_NONE, true>(a, &tmapX, &tmapY);
 }
 
 // dW = sum over splits of part^T (fixed order: deterministic).  part is (splits, N, M); dW is (M, N), or (N, M) when

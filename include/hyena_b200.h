@@ -88,8 +88,8 @@ HY_API int hyena_b200_filter_bwd(const float* z, int z_stride, const float* t,
 /* Tensor-core (wgmma, 3xTF32) backward in two stages.  Stage 1: per position, recompute the activations and back-
  * propagate through the MLP, writing dh = dk * modulation (D,L) and seven feature-major (64,L) arrays into `scratch`
  * (7*64*L floats, 16-byte aligned): a1, a2, a3, dp1, dp2, dp3, X.  Stage 2: the parameter gradients are reductions
- * over the sequence, done as accumulating wgmma GEMMs with K = position (all outputs (+=); zT is z transposed,
- * (E,L)); D <= 256, E <= 8:
+ * over the sequence, done as wgmma GEMMs with K = position and fixed-order split-K, so two calls give the same bits
+ * (all outputs (+=); zT is z transposed, (E,L)); D <= 256, E <= 8:
  *   dW3 = dh a3^T, dW2 = dp3 a2^T, dW1 = dp2 a1^T, dW0 = dp1 z, db_l = rowsum(dp_{l+1}), dfreq = rowsum(X) */
 HY_API int hyena_b200_filter_bwd_stage1(const float* z, int z_stride, const float* t,
                                  const float* W0, const float* b0, const float* W1, const float* b1,
