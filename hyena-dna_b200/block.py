@@ -58,11 +58,17 @@ class Block(nn.Module):
         return ops.add_layer_norm(x, r, norm.weight.to(torch.float32), norm.bias.to(torch.float32) if norm.bias is not None
                                   else None, norm.eps)
 
-    def forward(self, hidden_states, residual=None, mixer_subset=None, mixer_kwargs=None, lengths=None):
+    def forward(self, hidden_states, residual=None, mixer_subset=None, mixer_kwargs=None, lengths=None, mask=None):
         """(hidden_states, residual) -> (mlp(LN2(.)) or mixer output, new residual); block.py:111-180, prenorm branch.
-        ``lengths``: left-padded rows, passed to the mixer (HyenaOperator.forward); LayerNorm and the MLP act per position."""
+        ``lengths``: left-padded rows, passed to the mixer (HyenaOperator.forward); LayerNorm and the MLP act per position.
+        ``mask``: the (B, L) attention mask of a left-padded batch, passed to the mixer, differentiable
+        (HyenaOperator.forward); with the loss on real positions only, every gradient at the pads is 0."""
         if mixer_subset is not None:
             raise HyenaB200Error("Block: mixer_subset is not supported")
+        if mask is not None:
+            kw = dict(mixer_kwargs or {})
+            pad = self._check_mask(hidden_states, mask, kw.get("inference_params"), lengths)
+            return self._run(hidden_states, residual, lambda y: self.mixer(y, mask=pad, **kw))
         if lengths is not None:
             self._check_lengths(hidden_states, lengths, None, "forward")
             kw = dict(mixer_kwargs or {}, lengths=lengths)
@@ -73,6 +79,11 @@ class Block(nn.Module):
         if not hasattr(self.mixer, "check_lengths"):
             raise HyenaB200Error(f"Block: the mixer {type(self.mixer).__name__} takes no lengths")
         self.mixer.check_lengths(hidden_states, lengths, cache, how)
+
+    def _check_mask(self, hidden_states, mask, cache=None, lengths=None):
+        if not hasattr(self.mixer, "check_mask"):
+            raise HyenaB200Error(f"Block: the mixer {type(self.mixer).__name__} takes no mask")
+        return self.mixer.check_mask(hidden_states, mask, cache, lengths)
 
     def prefill(self, hidden_states, residual, cache, lengths=None):
         """forward over the first positions, filling the mixer's DecodeCache (HyenaOperator.prefill); ``lengths``:
@@ -142,14 +153,16 @@ class Backbone(nn.Module):
                   prenorm=True, residual_in_fp32=residual_in_fp32) for _ in range(n_layer)])
         self.ln_f = nn.LayerNorm(d_model, eps=layer_norm_epsilon)
 
-    def forward(self, hidden_states, lengths=None):
-        """``lengths``: left-padded rows (HyenaOperator.forward), inference only."""
+    def forward(self, hidden_states, lengths=None, mask=None):
+        """``lengths``: left-padded rows (HyenaOperator.forward), inference only.  ``mask``: the (B, L) attention mask of a
+        left-padded batch (the reference datamodules' ``mask`` batch kwarg), differentiable (HyenaOperator.forward)."""
+        if mask is not None:                  # validated once: the layers get the LeftPadding
+            mask = self.layers[0]._check_mask(hidden_states, mask, None, lengths)
         if lengths is not None:
             self.layers[0]._check_lengths(hidden_states, lengths, None, "forward")
         residual = None
         for layer in self.layers:
-            hidden_states, residual = layer(hidden_states, residual) if lengths is None else \
-                layer(hidden_states, residual, lengths=lengths)
+            hidden_states, residual = layer(hidden_states, residual, lengths=lengths, mask=mask)
         y, _ = Block._add_norm(hidden_states, residual, self.ln_f)
         return y.to(hidden_states.dtype)
 

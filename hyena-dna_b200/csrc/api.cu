@@ -573,13 +573,11 @@ HY_API int hyena_b200_core_fwd_rows(const float* p, const float* in_bias, const 
                       workspace_bytes, stream);
 }
 
-HY_API int hyena_b200_core_bwd(const float* dy_pre, const float* p, const float* in_bias, const float* sw, const float* sb,
-                        const float* kspec, const float* fbias, const float* c_saved, const float* gspec_saved,
-                        float* dp, float* dk, float* dsw, float* dsb, float* dfbias, float* d_in_bias,
-                        float* ds_scratch, int B, int D, int L, void* workspace, size_t workspace_bytes, void* stream) {
-  if (check_shape(B, D, L)) return 1;
-  HY_CHECK(dy_pre && p && sw && sb && kspec && fbias && c_saved && dk && dsw && dsb && dfbias && ds_scratch,
-           "null pointer");
+// the backward passes of core_bwd; row_start non-null: the left-padded modes (core_bwd_rows), the same launch sequence
+static int core_bwd_run(const float* dy_pre, const float* p, const float* in_bias, const float* sw, const float* sb,
+                        const float* kspec, const float* fbias, const float* c_saved, const float* gspec_saved, float* dp,
+                        float* dk, float* dsw, float* dsb, float* dfbias, float* d_in_bias, float* ds_scratch,
+                        const int* row_start, int B, int D, int L, void* workspace, size_t workspace_bytes, void* stream) {
   cudaStream_t s = (cudaStream_t)stream;
   Twiddles T;
   if (get_twiddles(s, &T)) return 1;
@@ -588,6 +586,9 @@ HY_API int hyena_b200_core_bwd(const float* dy_pre, const float* p, const float*
   PassArgs a = base_args(B, D, L, T);
   a.kspec = reinterpret_cast<const float2*>(kspec);
   a.p = p; a.in_bias = in_bias; a.sw = sw; a.sb = sb; a.fbias = fbias;
+  a.row_start = row_start;
+  const int dc_mode = row_start ? COL_DC_ROWS : COL_DC, gate_mode = row_start ? COL_GATE_ROWS : COL_GATE,
+            dg_mode = row_start ? INV_BWD_DG_ROWS : INV_BWD_DG;
   a.vec = ((L & 1) == 0) && aligned8(p) && aligned8(dy_pre) && aligned8(c_saved) && aligned8(dk) &&
           aligned8(ds_scratch);
   a.stage = ((L & 3) == 0) && aligned16(p) && aligned16(dy_pre) && aligned16(c_saved) && !getenv("HYENA_B200_NO_STAGE");
@@ -610,18 +611,18 @@ HY_API int hyena_b200_core_bwd(const float* dy_pre, const float* p, const float*
     a.c0 = c0; a.B = B;
     a.A2 = c.A2; a.A3 = c.A3;
     a.A = c.A; a.src = dy_pre;
-    HY_CUDA(launch_col_fwd(COL_DC, a, n * B, s));        // A  <- columns of dc = dy_pre * x0
+    HY_CUDA(launch_col_fwd(dc_mode, a, n * B, s));       // A  <- columns of dc = dy_pre * x0
     a.gspec = const_cast<float2*>(reinterpret_cast<const float2*>(gspec_saved));
     if (!gspec_saved) {
       a.A = c.A2;
-      HY_CUDA(launch_col_fwd(COL_GATE, a, n * B, s));    // A2 <- columns of g = v * x1 (recomputed)
+      HY_CUDA(launch_col_fwd(gate_mode, a, n * B, s));   // A2 <- columns of g = v * x1 (recomputed)
     }
     a.A = c.A;
     static const bool bwd1 = !(getenv("HYENA_B200_ROW_BWD1") && !strcmp(getenv("HYENA_B200_ROW_BWD1"), "0"));
     // (the 128-thread batch-1 kernel exists for 1024-point rows only)
     HY_CUDA(launch_row_pass((B == 1 && gspec_saved && bwd1 && a.logM2 == 10) ? ROW_CONV_BWD1 : ROW_CONV_BWD, a, n, s));   // A <- rows of dg, A3 <- rows of dk
     a.src = dy_pre; a.src2 = c_saved; a.out2 = ds_scratch; a.red = dfbias; a.dsw = dsw; a.dsb = dsb;
-    HY_CUDA(launch_col_inv(INV_BWD_DG, a, n * B, s));
+    HY_CUDA(launch_col_inv(dg_mode, a, n * B, s));
     a.B = 1; a.out = dk;
     HY_CUDA(launch_col_inv(INV_DK, a, n, s));
   }
@@ -630,10 +631,40 @@ HY_API int hyena_b200_core_bwd(const float* dy_pre, const float* p, const float*
   // dp == NULL: the caller consumes ds directly (hyena_b200_proj_gemm / proj_wgrad apply the transposed short filter on
   // the fly and d in_proj.bias follows from dsb and two edge samples), so dp never exists in HBM.
   if (dp) {
-    ShortBwdArgs sa{ds_scratch, nullptr, in_bias, sw, dp, dsw, dsb, d_in_bias, L, 3 * D, a.vec && aligned8(dp)};
+    ShortBwdArgs sa{ds_scratch, nullptr, in_bias, sw, dp, dsw, dsb, d_in_bias, L, 3 * D, a.vec && aligned8(dp), row_start};
     HY_CUDA(launch_short_bwd(sa, B, s));
   }
   return 0;
+}
+
+HY_API int hyena_b200_core_bwd(const float* dy_pre, const float* p, const float* in_bias, const float* sw, const float* sb,
+                        const float* kspec, const float* fbias, const float* c_saved, const float* gspec_saved,
+                        float* dp, float* dk, float* dsw, float* dsb, float* dfbias, float* d_in_bias,
+                        float* ds_scratch, int B, int D, int L, void* workspace, size_t workspace_bytes, void* stream) {
+  if (check_shape(B, D, L)) return 1;
+  HY_CHECK(dy_pre && p && sw && sb && kspec && fbias && c_saved && dk && dsw && dsb && dfbias && ds_scratch,
+           "null pointer");
+  return core_bwd_run(dy_pre, p, in_bias, sw, sb, kspec, fbias, c_saved, gspec_saved, dp, dk, dsw, dsb, dfbias, d_in_bias,
+                      ds_scratch, nullptr, B, D, L, workspace, workspace_bytes, stream);
+}
+
+HY_API int hyena_b200_core_bwd_rows(const float* dy_pre, const float* p, const float* in_bias, const float* sw,
+                                    const float* sb, const float* kspec, const float* fbias, const float* c_saved,
+                                    const float* gspec_saved, float* dp, float* dk, float* dsw, float* dsb, float* dfbias,
+                                    float* d_in_bias, float* ds_scratch, const int* row_start, int B, int D, int L,
+                                    void* workspace, size_t workspace_bytes, void* stream) {
+  if (check_shape(B, D, L)) return 1;
+  HY_CHECK(dy_pre && p && sw && sb && kspec && fbias && c_saved && dk && dsw && dsb && dfbias && ds_scratch && row_start,
+           "null pointer");
+  HY_CHECK(aligned4(dy_pre) && aligned4(p) && aligned4(sw) && aligned4(sb) && aligned4(fbias) && aligned4(c_saved) &&
+               aligned4(dk) && aligned4(dsw) && aligned4(dsb) && aligned4(dfbias) && aligned4(ds_scratch) &&
+               aligned4(row_start) && (!in_bias || aligned4(in_bias)) && (!dp || aligned4(dp)) &&
+               (!d_in_bias || aligned4(d_in_bias)),
+           "misaligned pointer: every float operand and row_start must be 4-byte aligned");
+  HY_CHECK(aligned8(kspec) && (!gspec_saved || aligned8(gspec_saved)), "misaligned pointer: kspec and gspec_saved must be "
+           "8-byte aligned");
+  return core_bwd_run(dy_pre, p, in_bias, sw, sb, kspec, fbias, c_saved, gspec_saved, dp, dk, dsw, dsb, dfbias, d_in_bias,
+                      ds_scratch, row_start, B, D, L, workspace, workspace_bytes, stream);
 }
 
 /* OUT[pos][n] = sum_k ACT[pos][k] W'[n][k] (+ bias[n]) on wgmma, fp32 accuracy (3xTF32); see include/hyena_b200.h */

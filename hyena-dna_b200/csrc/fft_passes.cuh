@@ -126,7 +126,7 @@ __device__ __forceinline__ float2 staged_pair(const float* st, int rr, int col) 
   return *reinterpret_cast<const float2*>(st + rr * (2 * C) + 2 * col);
 }
 
-// Left-padded rows (COL_GATE_ROWS / INV_CONV_FWD_ROWS): positions t < rs of the row are padding and read as the short
+// Left-padded rows (the *_ROWS modes): positions t < rs of the row are padding and read as the short
 // filter's padding before t = 0 (value 0, no in_proj bias).  Applied per element after the window is loaded or staged, so
 // a window straddling rs is masked however it was fetched.
 __device__ __forceinline__ void mask_window(float (&P)[4], int t0, int rs) {
@@ -140,12 +140,20 @@ __device__ __forceinline__ float2 mask_pair(float2 v, int t0, int rs) {
 // ------------------------------------------------------------------------------------------------
 // argument blocks
 // ------------------------------------------------------------------------------------------------
-// *_ROWS: the forward modes on left-padded rows; row b's samples t < row_start[b] are padding (g, y_pre and c_save are 0
-// there, and the short filters see zeros).  Their launches count under the kind of the plain mode (col_kind / inv_kind).
-enum ColMode { COL_FILTER = 0, COL_GATE = 1, COL_DC = 2, COL_PLAIN = 3, COL_GATE_ROWS = 4 };
-enum InvMode { INV_CONV_FWD = 0, INV_BWD_DG = 1, INV_DK = 2, INV_PLAIN_FWD = 3, INV_PLAIN_BWD = 4, INV_CONV_FWD_ROWS = 5 };
-__host__ __device__ constexpr int col_kind(int mode) { return mode == COL_GATE_ROWS ? COL_GATE : mode; }
-__host__ __device__ constexpr int inv_kind(int mode) { return mode == INV_CONV_FWD_ROWS ? INV_CONV_FWD : mode; }
+// *_ROWS: the core modes on left-padded rows; row b's samples t < row_start[b] are padding (g, y_pre and c_save are 0
+// there, and the short filters see zeros; backward: dc, dg and the three ds are 0 there).  Their launches count under the
+// kind of the plain mode (col_kind / inv_kind).
+enum ColMode { COL_FILTER = 0, COL_GATE = 1, COL_DC = 2, COL_PLAIN = 3, COL_GATE_ROWS = 4, COL_DC_ROWS = 5 };
+enum InvMode { INV_CONV_FWD = 0, INV_BWD_DG = 1, INV_DK = 2, INV_PLAIN_FWD = 3, INV_PLAIN_BWD = 4, INV_CONV_FWD_ROWS = 5,
+               INV_BWD_DG_ROWS = 6 };
+__host__ __device__ constexpr int col_kind(int mode) {
+  return mode == COL_GATE_ROWS ? COL_GATE : mode == COL_DC_ROWS ? COL_DC : mode;
+}
+__host__ __device__ constexpr int inv_kind(int mode) {
+  return mode == INV_CONV_FWD_ROWS ? INV_CONV_FWD : mode == INV_BWD_DG_ROWS ? INV_BWD_DG : mode;
+}
+// the backward pass-3 epilogue (plain or on left-padded rows)
+__host__ __device__ constexpr bool inv_bwd_dg(int mode) { return mode == INV_BWD_DG || mode == INV_BWD_DG_ROWS; }
 enum RowMode { ROW_FILTER = 0, ROW_CONV_FWD = 1, ROW_CONV_BWD = 2, ROW_CONV_BWD1 = 3 };
 
 // Rows of one launch are numbered r = ci*B + b (all batches of a channel adjacent), channel c = c0 + ci.
@@ -179,7 +187,7 @@ struct PassArgs {
   float* red;            // INV_BWD_DG: dfbias (D); INV_PLAIN_BWD: dD (H)   (atomicAdd)
   float* dsw;            // INV_BWD_DG: d short_filter.weight (3D,3) (atomicAdd)
   float* dsb;            // INV_BWD_DG: d short_filter.bias (3D)     (atomicAdd)
-  const int* row_start;  // COL_GATE_ROWS / INV_CONV_FWD_ROWS: (B) first real position of each batch row
+  const int* row_start;  // *_ROWS modes: (B) first real position of each batch row
 };
 
 __device__ __forceinline__ size_t row_off(int b, int ch, int nch, int L) { return ((size_t)b * nch + ch) * (size_t)L; }
@@ -216,11 +224,11 @@ struct ColGeo {
   // Shared memory per mode: the forward kernel keeps its smaller footprint.
   template <int MODE>
   static constexpr size_t stage_inv() {
-    return TWO ? 2 * (MODE == INV_BWD_DG ? BATCH_BWD_FLOATS : BATCH_FWD_FLOATS) * sizeof(float) : 0;
+    return TWO ? 2 * (inv_bwd_dg(MODE) ? BATCH_BWD_FLOATS : BATCH_FWD_FLOATS) * sizeof(float) : 0;
   }
   template <int MODE>
   static constexpr size_t smem_inv() {
-    return (MODE == INV_BWD_DG || MODE == INV_CONV_FWD || MODE == INV_CONV_FWD_ROWS) && stage_inv<MODE>() > EXCH
+    return (inv_bwd_dg(MODE) || MODE == INV_CONV_FWD || MODE == INV_CONV_FWD_ROWS) && stage_inv<MODE>() > EXCH
                ? stage_inv<MODE>() : EXCH;
   }
   static constexpr size_t SMEM_FWD = EXCH > STAGE_FWD ? EXCH : STAGE_FWD;
@@ -244,6 +252,13 @@ __device__ __forceinline__ float2 col_input(const PassArgs& a, int b, int c, int
     mask_window(P, t0, rs);
     const float2 v = conv_window(P, t0, a.L, kb);
     return mask_pair(make_float2(x1.x * v.x, x1.y * v.y), t0, rs);
+  } else if constexpr (MODE == COL_DC_ROWS) {    // COL_DC on a left-padded row: dc is 0 at t < rs
+    float P[4];
+    load_window(a.p + row_off(b, c, 3 * a.D, a.L), t0, a.L, vec, ka.ib, P);
+    mask_window(P, t0, rs);
+    const float2 x0 = conv_window(P, t0, a.L, ka);
+    const float2 dy = load_pair(a.src + row_off(b, c, a.D, a.L), t0, a.L, vec);
+    return mask_pair(make_float2(x0.x * dy.x, x0.y * dy.y), t0, rs);
   } else if constexpr (MODE == COL_FILTER) {
     return load_pair(a.src + (size_t)c * a.L, t0, a.L, vec);
   } else if constexpr (MODE == COL_PLAIN) {
@@ -289,6 +304,9 @@ __device__ __forceinline__ void col_fwd_body(const PassArgs& a, const int bx, co
     if constexpr (MODE == COL_GATE_ROWS) rs = __ldg(a.row_start + b);
   } else if constexpr (MODE == COL_DC) {
     ka = load_taps(a.sw, a.sb, a.in_bias, c);
+  } else if constexpr (MODE == COL_DC_ROWS) {
+    ka = load_taps(a.sw, a.sb, a.in_bias, c);
+    rs = __ldg(a.row_start + b);
   }
 
   float2 v[32];
@@ -296,7 +314,7 @@ __device__ __forceinline__ void col_fwd_body(const PassArgs& a, const int bx, co
     const int col = threadIdx.x % CG::C, q = threadIdx.x / CG::C;
     const int m2 = colbase + col;
     // slots n1 >= 16 (m1 >= M1/2) are the zero padding: never loaded
-    if ((MODE == COL_GATE || MODE == COL_DC || MODE == COL_GATE_ROWS) && a.stage) {
+    if ((MODE == COL_GATE || MODE == COL_DC || MODE == COL_GATE_ROWS || MODE == COL_DC_ROWS) && a.stage) {
       float* st0 = reinterpret_cast<float*>(smem_raw);
       float* st1 = st0 + CG::DATA_ROWS * CG::WP;
       if constexpr (MODE == COL_GATE || MODE == COL_GATE_ROWS) {
@@ -316,7 +334,7 @@ __device__ __forceinline__ void col_fwd_body(const PassArgs& a, const int bx, co
         if (t0 < L) {
           float P[4];
           staged_window<CG::C>(st0, m1, col, t0, ka.ib, P);
-          if constexpr (MODE == COL_GATE_ROWS) mask_window(P, t0, rs);
+          if constexpr (MODE == COL_GATE_ROWS || MODE == COL_DC_ROWS) mask_window(P, t0, rs);
           const float2 x = conv_window(P, t0, L, ka);
           if constexpr (MODE == COL_GATE || MODE == COL_GATE_ROWS) {
             staged_window<CG::C>(st1, m1, col, t0, kb.ib, P);
@@ -327,6 +345,7 @@ __device__ __forceinline__ void col_fwd_body(const PassArgs& a, const int bx, co
           } else {
             const float2 dy = staged_pair<CG::C>(st1, m1, col);
             g = make_float2(x.x * dy.x, x.y * dy.y);
+            if constexpr (MODE == COL_DC_ROWS) g = mask_pair(g, t0, rs);
           }
         }
         v[n1] = g;
@@ -395,7 +414,7 @@ struct InvCtx {
   float red;           // per-thread partial of the reduction this mode produces
   float rw[3][3];      // INV_BWD_DG: partials of d short_filter.weight for the x0 / x1 / v channels
   float rb[3];         //             and of d short_filter.bias
-  int rs;              // INV_CONV_FWD_ROWS: first real position of the row
+  int rs;              // INV_CONV_FWD_ROWS / INV_BWD_DG_ROWS: first real position of the row
 };
 
 // dw_j += ds[t0] P(t0-2+j) + ds[t0+1] P(t0-1+j);  db += ds[t0] + ds[t0+1]     (P = window of the filter input)
@@ -423,7 +442,7 @@ __device__ __forceinline__ void inv_load(const PassArgs& a, const InvCtx& cx, in
     in.b = load_pair(a.src + row_off(b, c, D, L), t0, L, vec);
   } else if constexpr (MODE == INV_CONV_FWD || MODE == INV_CONV_FWD_ROWS) {
     load_window(a.p + row_off(b, c, 3 * D, L), t0, L, vec, cx.k0.ib, in.P0);     // x0 only: c = y already holds bias * g
-  } else if constexpr (MODE == INV_BWD_DG) {
+  } else if constexpr (inv_bwd_dg(MODE)) {
     load_window(a.p + row_off(b, c, 3 * D, L), t0, L, vec, cx.k0.ib, in.P0);
     load_window(a.p + row_off(b, D + c, 3 * D, L), t0, L, vec, cx.k1.ib, in.P1);
     load_window(a.p + row_off(b, 2 * D + c, 3 * D, L), t0, L, vec, cx.k2.ib, in.P2);
@@ -455,6 +474,27 @@ __device__ __forceinline__ void inv_finish(const PassArgs& a, InvCtx& cx, int b,
     const float2 cm = mask_pair(y, t0, cx.rs);
     if (a.out2) store_pair(a.out2 + row_off(b, c, D, L), t0, L, vec, cm);
     store_pair(a.out + row_off(b, c, D, L), t0, L, vec, mask_pair(pmul(y, x0), t0, cx.rs));
+  } else if constexpr (MODE == INV_BWD_DG_ROWS) {     // INV_BWD_DG on a left-padded row: the windows are masked as the
+    float P0[4], P1[4], P2[4];                        // forward masked them, dc, dg and the three ds are 0 at t < rs, so
+#pragma unroll                                        // dbias and the tap gradients see real positions only
+    for (int j = 0; j < 4; ++j) { P0[j] = in.P0[j]; P1[j] = in.P1[j]; P2[j] = in.P2[j]; }
+    mask_window(P0, t0, cx.rs);
+    mask_window(P1, t0, cx.rs);
+    mask_window(P2, t0, cx.rs);
+    const float2 x0 = conv_window(P0, t0, L, cx.k0), x1 = conv_window(P1, t0, L, cx.k1), vv = conv_window(P2, t0, L, cx.k2);
+    const float2 dy = in.a, cs = in.b;
+    const float2 dc = mask_pair(pmul(dy, x0), t0, cx.rs);
+    const float2 dg = mask_pair(y, t0, cx.rs);
+    cx.red = fmaf(dc.x, x1.x * vv.x, fmaf(dc.y, x1.y * vv.y, cx.red));
+    const float2 d0 = mask_pair(pmul(dy, cs), t0, cx.rs);
+    const float2 d1 = mask_pair(pmul(dg, vv), t0, cx.rs);
+    const float2 d2 = mask_pair(pmul(dg, x1), t0, cx.rs);
+    store_pair(a.out2 + row_off(b, c, 3 * D, L), t0, L, vec, d0);
+    store_pair(a.out2 + row_off(b, D + c, 3 * D, L), t0, L, vec, d1);
+    store_pair(a.out2 + row_off(b, 2 * D + c, 3 * D, L), t0, L, vec, d2);
+    tap_grads(cx.rw[0], cx.rb[0], d0, P0);
+    tap_grads(cx.rw[1], cx.rb[1], d1, P1);
+    tap_grads(cx.rw[2], cx.rb[2], d2, P2);
   } else {                                            // INV_BWD_DG
     const float2 x0 = conv_window(in.P0, t0, L, cx.k0), x1 = conv_window(in.P1, t0, L, cx.k1),
                  vv = conv_window(in.P2, t0, L, cx.k2);
@@ -499,11 +539,11 @@ __device__ __forceinline__ void col_inv_body(const PassArgs& a, const int bx, co
   InvCtx cx{};
   cx.red = 0.f;
   if constexpr (MODE == INV_CONV_FWD || MODE == INV_BWD_DG) cx.k0 = load_taps(a.sw, a.sb, a.in_bias, c);
-  if constexpr (MODE == INV_CONV_FWD_ROWS) {
+  if constexpr (MODE == INV_CONV_FWD_ROWS || MODE == INV_BWD_DG_ROWS) {
     cx.k0 = load_taps(a.sw, a.sb, a.in_bias, c);
     cx.rs = __ldg(a.row_start + b);
   }
-  if constexpr (MODE == INV_BWD_DG) {
+  if constexpr (inv_bwd_dg(MODE)) {
     cx.k1 = load_taps(a.sw, a.sb, a.in_bias, a.D + c);
     cx.k2 = load_taps(a.sw, a.sb, a.in_bias, 2 * a.D + c);
   }
@@ -518,14 +558,14 @@ __device__ __forceinline__ void col_inv_body(const PassArgs& a, const int bx, co
     });
     block_fft<CG::TWO ? LOGM1 : 5, true, false>(v, smem + col * CG::PITCH, q, a.T.tw1024, CtaSync{});
     // only m1 < M1/2 (slots s < 16) can hold samples t < L
-    if ((MODE == INV_CONV_FWD || MODE == INV_BWD_DG || MODE == INV_CONV_FWD_ROWS) && a.stage) {
+    if ((MODE == INV_CONV_FWD || inv_bwd_dg(MODE) || MODE == INV_CONV_FWD_ROWS) && a.stage) {
       // epilogue operands staged through shared memory, SB slots (SB*R2 consecutive rows) per batch; forward:
       // double buffered, the cp.async group of batch k+1 is in flight while batch k is consumed
       constexpr bool DBL = true;
-      constexpr int SB = (MODE == INV_BWD_DG) ? CG::SB_BWD : CG::SB_FWD;
+      constexpr int SB = inv_bwd_dg(MODE) ? CG::SB_BWD : CG::SB_FWD;
       constexpr int NBATCH = 16 / SB;
       constexpr int BROWS = SB * CG::R2;
-      constexpr size_t BFLOATS = (MODE == INV_BWD_DG) ? CG::BATCH_BWD_FLOATS : CG::BATCH_FWD_FLOATS;
+      constexpr size_t BFLOATS = inv_bwd_dg(MODE) ? CG::BATCH_BWD_FLOATS : CG::BATCH_FWD_FLOATS;
       float* st = reinterpret_cast<float*>(smem_raw);
       const float* p0 = a.p + row_off(b, c, 3 * a.D, L);
       const float* p1 = a.p + row_off(b, a.D + c, 3 * a.D, L);
@@ -536,7 +576,7 @@ __device__ __forceinline__ void col_inv_body(const PassArgs& a, const int bx, co
         float* w2 = w1 + BROWS * CG::WP;
         const int row0 = BROWS * k;
         stage_windows<CG::C, kM2>(w0, p0, row0, BROWS, colbase, L);
-        if constexpr (MODE == INV_BWD_DG) {
+        if constexpr (inv_bwd_dg(MODE)) {
           stage_windows<CG::C, kM2>(w1, p1, row0, BROWS, colbase, L);
           stage_windows<CG::C, kM2>(w2, p2, row0, BROWS, colbase, L);
           float* x0 = w2 + BROWS * CG::WP;
@@ -571,7 +611,7 @@ __device__ __forceinline__ void col_inv_body(const PassArgs& a, const int bx, co
             InvIn in;
             const int rr = m1 - BROWS * k;
             staged_window<CG::C>(w0, rr, col, t0, cx.k0.ib, in.P0);
-            if constexpr (MODE == INV_BWD_DG) {
+            if constexpr (inv_bwd_dg(MODE)) {
               staged_window<CG::C>(w1, rr, col, t0, cx.k1.ib, in.P1);
               staged_window<CG::C>(w2, rr, col, t0, cx.k2.ib, in.P2);
               in.a = staged_pair<CG::C>(x0, rr, col);
@@ -624,12 +664,12 @@ __device__ __forceinline__ void col_inv_body(const PassArgs& a, const int bx, co
     });
   }
 
-  if constexpr (MODE == INV_BWD_DG || MODE == INV_PLAIN_BWD) {
-    constexpr int NR = (MODE == INV_BWD_DG) ? 13 : 1;
+  if constexpr (inv_bwd_dg(MODE) || MODE == INV_PLAIN_BWD) {
+    constexpr int NR = inv_bwd_dg(MODE) ? 13 : 1;
     __shared__ float red_all[8][NR];
     float vals[NR];
     vals[0] = cx.red;
-    if constexpr (MODE == INV_BWD_DG) {
+    if constexpr (inv_bwd_dg(MODE)) {
 #pragma unroll
       for (int ch = 0; ch < 3; ++ch) {
 #pragma unroll

@@ -8,6 +8,7 @@ cudaError_t launch_col_fwd(int mode, const PassArgs& a, int rows, cudaStream_t s
     case COL_DC: return launch_col_fwd_mode<COL_DC>(a, rows, s);
     case COL_PLAIN: return launch_col_fwd_mode<COL_PLAIN>(a, rows, s);
     case COL_GATE_ROWS: return launch_col_fwd_mode<COL_GATE_ROWS>(a, rows, s);
+    case COL_DC_ROWS: return launch_col_fwd_mode<COL_DC_ROWS>(a, rows, s);
   }
   return cudaErrorInvalidValue;
 }

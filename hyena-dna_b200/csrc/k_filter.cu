@@ -50,7 +50,8 @@ cudaError_t launch_filter_bwd(const FilterParams& P, const float* dk, const Filt
 cudaError_t launch_short_bwd(const ShortBwdArgs& a, int B, cudaStream_t s) {
   dim3 grid((a.L + kScSpan - 1) / kScSpan, a.C3, B);
   prof_begin(K_SHORT_BWD, s);
-  short_conv_bwd_kernel<<<grid, 256, 0, s>>>(a);
+  if (a.row_start) short_conv_bwd_rows_kernel<<<grid, 256, 0, s>>>(a);
+  else short_conv_bwd_kernel<<<grid, 256, 0, s>>>(a);
   prof_end(K_SHORT_BWD, s);
   return cudaGetLastError();
 }

@@ -5,6 +5,9 @@
 // Backward, given ds = d loss / d s  (B,3D,L):
 //   dp[t]  = w2 ds[t] + w1 ds[t+1] + w0 ds[t+2]          (ds[t>=L] = 0)
 //   dw_j   = sum_{b,t} ds[t] P(t-2+j),  db = sum ds,  d in_bias = sum dp
+// Left-padded rows (row_start non-null, short_conv_bwd_rows_kernel): positions t < row_start[b] are padding that the forward
+// zeroed before the filter, so dp is 0 there (the transposed filter would carry ds[rs], ds[rs+1] into rs-1, rs-2) and they
+// stay out of d in_bias; a pad sample of a window reads 0.
 #pragma once
 #include "fft_passes.cuh"
 
@@ -22,10 +25,12 @@ struct ShortBwdArgs {
   float* dsb;           // (3D)    atomicAdd
   float* dib;           // (3D)    atomicAdd (d in_proj.bias) or null
   int L, C3, vec;
+  const int* row_start; // (B) first real position of each row, or null (plain kernel)
 };
 
 #ifdef HY_FILTER_KERNEL_TU
-__global__ void __launch_bounds__(256) short_conv_bwd_kernel(const ShortBwdArgs a) {
+template <bool ROWS>
+__device__ __forceinline__ void short_conv_bwd_body(const ShortBwdArgs& a) {
   const int ch = blockIdx.y, b = blockIdx.z;
   const int L = a.L;
   const bool vec = a.vec;
@@ -34,6 +39,8 @@ __global__ void __launch_bounds__(256) short_conv_bwd_kernel(const ShortBwdArgs 
   float* dp = a.dp + row_off(b, ch, a.C3, L);
   const float w0 = __ldg(a.sw + 3 * ch), w1 = __ldg(a.sw + 3 * ch + 1), w2 = __ldg(a.sw + 3 * ch + 2);
   const float ib = a.in_bias ? __ldg(a.in_bias + ch) : 0.f;
+  [[maybe_unused]] int rs = 0;
+  if constexpr (ROWS) rs = __ldg(a.row_start + b);
   float r[5] = {0.f, 0.f, 0.f, 0.f, 0.f};      // dw0, dw1, dw2, db, dib
   const int tbeg = blockIdx.x * kScSpan;
   const int tend = min(L, tbeg + kScSpan);
@@ -43,10 +50,12 @@ __global__ void __launch_bounds__(256) short_conv_bwd_kernel(const ShortBwdArgs 
     float2 o;
     o.x = fmaf(w2, d0.x, fmaf(w1, d0.y, w0 * d1.x));
     o.y = fmaf(w2, d0.y, fmaf(w1, d1.x, w0 * d1.y));
+    if constexpr (ROWS) o = mask_pair(o, t0, rs);
     store_pair(dp, t0, L, vec, o);
     if (a.p) {
       float P[4];
       load_window(p, t0, L, vec, ib, P);
+      if constexpr (ROWS) mask_window(P, t0, rs);
       r[0] = fmaf(d0.x, P[0], fmaf(d0.y, P[1], r[0]));
       r[1] = fmaf(d0.x, P[1], fmaf(d0.y, P[2], r[1]));
       r[2] = fmaf(d0.x, P[2], fmaf(d0.y, P[3], r[2]));
@@ -71,6 +80,9 @@ __global__ void __launch_bounds__(256) short_conv_bwd_kernel(const ShortBwdArgs 
     else if (a.dib) atomicAdd(a.dib + ch, s);
   }
 }
+
+__global__ void __launch_bounds__(256) short_conv_bwd_kernel(const ShortBwdArgs a) { short_conv_bwd_body<false>(a); }
+__global__ void __launch_bounds__(256) short_conv_bwd_rows_kernel(const ShortBwdArgs a) { short_conv_bwd_body<true>(a); }
 
 #endif  // HY_FILTER_KERNEL_TU
 

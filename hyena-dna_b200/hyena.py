@@ -297,6 +297,53 @@ class _OutProj(torch.autograd.Function):
         return d_pre, dW, db
 
 
+class LeftPadding:
+    """A validated left-padding mask (HyenaOperator.check_mask): the rows' first real positions on the host (``starts``)
+    and on the mask's device or u's device (``row_start``, (B,) int32).  Block and Backbone pass it on to their mixers so
+    that a mask is validated, and copied, once per call."""
+
+    def __init__(self, starts, row_start, positions):
+        self.starts, self.row_start, self.positions = starts, row_start, positions
+
+
+def host_mask_starts(mask, batch, positions, device):
+    """mask (batch, positions), bool or integer 0/1, on the CPU or on ``device`` -> LeftPadding, checked with one
+    device-to-host copy of per-row results for a device mask.  Row b must be zeros followed by at least one one (the
+    attention mask of a left-padded batch); its real tokens are its last mask[b].sum() positions."""
+    if isinstance(mask, LeftPadding):
+        if len(mask.starts) != batch or mask.positions != positions or mask.row_start.device != device:
+            raise HyenaB200Error("this LeftPadding was validated for another input shape or device")
+        return mask
+    if not torch.is_tensor(mask):
+        raise HyenaB200Error(f"mask must be a ({batch}, {positions}) bool or integer tensor; got {type(mask).__name__}")
+    if mask.dtype.is_floating_point or mask.dtype.is_complex:
+        raise HyenaB200Error(f"mask must be bool or integer 0/1; got {mask.dtype}")
+    if tuple(mask.shape) != (batch, positions):
+        raise HyenaB200Error(f"mask must be ({batch}, {positions}) like the input's (B, L); got {tuple(mask.shape)}")
+    if mask.device.type != "cpu" and mask.device != device:
+        raise HyenaB200Error(f"mask must be on the CPU or on the input's device {device}; got {mask.device}")
+    m = mask.detach()
+    badval = ((m != 0) & (m != 1)).any(1) if m.dtype != torch.bool else torch.zeros_like(m[:, 0])
+    m = m != 0
+    n = m.sum(1)
+    unordered = (m[:, :-1] & ~m[:, 1:]).any(1)                 # a one followed by a zero
+    info = torch.stack([n, badval.to(n.dtype), unordered.to(n.dtype)]).cpu().tolist()
+    for b in range(batch):
+        if info[1][b]:
+            raise HyenaB200Error(f"mask values must be 0 or 1 (row {b})")
+    for b in range(batch):
+        if info[0][b] == 0:
+            raise HyenaB200Error(f"mask row {b} is empty: every row needs at least one real token")
+        if info[2][b]:
+            raise HyenaB200Error(f"mask row {b} is not left-padded: a row must be zeros (pads) followed by ones "
+                                 "(real tokens)")
+    starts = [positions - k for k in info[0]]
+    row_start = (positions - n).to(torch.int32)
+    if row_start.device != device and device.type == "cuda":
+        row_start = row_start.pin_memory().to(device, non_blocking=True)
+    return LeftPadding(starts, row_start, positions)
+
+
 class HyenaOperator(nn.Module):
     """Hyena operator (hyena.py:270-448): order 2 as one fused pass on sm_90a, order >= 3 as a chain of its kernels.
 
@@ -334,12 +381,21 @@ class HyenaOperator(nn.Module):
         self.filter_fn = HyenaFilter(self.head_dim * inner_factor * (order - 1), order=filter_order, seq_len=l_max,
                                      channels=1, dropout=filter_dropout, **filter_args)
 
-    def forward(self, u, *args, lengths=None, **kwargs):
+    def forward(self, u, *args, lengths=None, mask=None, **kwargs):
         """``lengths`` (B integers in [1, L]): u is left-padded, row b's real tokens are its last lengths[b] positions.  Its
         outputs there do not depend on the padding: they are the outputs of the unpadded row (DESIGN.md section 4.14); at a
-        pad position the output is out_proj(0) = out_proj.bias.  Inference only: with grad required it raises (train on
-        right-padded batches, where a causal operator is exact as it stands)."""
+        pad position the output is out_proj(0) = out_proj.bias.  Inference only: with grad required it raises (use
+        ``mask``, or train on right-padded batches, where a causal operator is exact as it stands).
+
+        ``mask`` ((B, L) bool or integer 0/1, the attention mask of a left-padded batch, on the CPU or on u's device): the
+        same masked operator, differentiable (DESIGN.md section 4.17).  Outputs and every gradient at real positions are
+        the unpadded rows', parameter gradients are the sums over rows of the unpadded rows', du is 0 at the pads and the
+        pad contents (NaN and inf included) change nothing.  Under torch.no_grad() it gives the bits of
+        ``forward(u, lengths=mask.sum(-1))``.  Not with ``lengths`` or a DecodeCache (decoding takes ``lengths``)."""
         cache = kwargs.get("inference_params")
+        if mask is not None:
+            y = self._forward_masked(u, self.check_mask(u, mask, cache, lengths))
+            return (y, None) if self.return_state else y
         if isinstance(cache, DecodeCache):
             # incremental decoding driven by the caller's model (LMBackbone passes inference_params to every mixer,
             # long_conv_lm.py:375-376); any other inference_params object is ignored, as the reference does
@@ -391,16 +447,34 @@ class HyenaOperator(nn.Module):
             return y, None
         return y
 
-    def _ragged_checks(self, u, lengths):
-        """Host validation of a left-padded input before any device work -> the rows' first real positions."""
+    def _padded_checks(self, u, what):
+        """Host validation of a left-padded input's filter and shape -> (B, P)."""
         if self.filter_fn.bidirectional:
-            raise HyenaB200Error("lengths needs a causal filter; this HyenaFilter is bidirectional")
+            raise HyenaB200Error(f"{what} needs a causal filter; this HyenaFilter is bidirectional")
         if u.dim() != 3 or u.shape[-1] != self.d_model:
             raise HyenaB200Error(f"left-padded input must be (B, L, {self.d_model}); got {tuple(u.shape)}")
         B, P = u.shape[0], u.shape[1]
         if P > self.l_max:
             raise HyenaB200Error(f"left-padded input of {P} positions exceeds l_max = {self.l_max}")
+        return B, P
+
+    def _ragged_checks(self, u, lengths):
+        """Host validation of a left-padded input before any device work -> the rows' first real positions."""
+        B, P = self._padded_checks(u, "lengths")
         return [P - n for n in host_lengths(lengths, B, P)]
+
+    def check_mask(self, u, mask, cache=None, lengths=None):
+        """Every host check of ``forward(u, mask=mask)`` without device work (Block and Backbone run it before their first
+        kernel) -> LeftPadding (``mask`` may be one already)."""
+        if lengths is not None:
+            raise HyenaB200Error("pass mask or lengths, not both: they describe the same left padding")
+        if isinstance(cache, DecodeCache):
+            raise HyenaB200Error("mask does not combine with a DecodeCache: decoding takes lengths= (a left-padded prefill)")
+        B, P = self._padded_checks(u, "mask")
+        pad = host_mask_starts(mask, B, P, u.device)
+        if not u.is_cuda:
+            raise HyenaB200Error("HyenaOperator (hyena_b200) runs on CUDA sm_90a only; there is no CPU fallback")
+        return pad
 
     def check_lengths(self, u, lengths, cache=None, how="forward"):
         """Every host check of ``how``(u, [cache,] lengths=lengths) -- "forward", "prefill", "extend" or "step" -- without
@@ -410,8 +484,8 @@ class HyenaOperator(nn.Module):
         if how == "forward":
             if torch.is_grad_enabled() and (u.requires_grad or any(p.requires_grad for p in self.parameters())):
                 raise HyenaB200Error("forward(u, lengths=...) is inference only (run under torch.no_grad()); to train on "
-                                     "sequences of different lengths pad them on the right: the causal operator is exact "
-                                     "there")
+                                     "left-padded sequences pass their attention mask as forward(u, mask=...), or pad "
+                                     "them on the right: the causal operator is exact there")
             starts = self._ragged_checks(u, lengths)
             if not u.is_cuda:
                 raise HyenaB200Error("HyenaOperator (hyena_b200) runs on CUDA sm_90a only; there is no CPU fallback")
@@ -453,6 +527,28 @@ class HyenaOperator(nn.Module):
             p, gs = cap["p"], cap["g"]
         y = _OutProj.apply(y_pre, self.out_proj.weight, self.out_proj.bias).to(in_dtype)
         return y, p, gs
+
+    def _forward_masked(self, u, pad):
+        """forward(u, mask=...) under autograd: u (B, P, D) left-padded as ``pad`` (LeftPadding) says.  The in_proj input is
+        zeroed at the pads (torch.where), so p is 0 there, du is 0 there and the pads stay out of d in_proj.weight whatever
+        they hold.  Order 2 takes plain training's route choice with the masked core (hyena_b200_core_fwd_rows /
+        core_bwd_rows); order >= 3 is the chained route with the pads masked, differentiable as it stands."""
+        in_dtype, P = u.dtype, u.shape[1]
+        row_start = pad.row_start
+        keep = torch.arange(P, device=u.device)[None, :] >= row_start.to(torch.long)[:, None]          # (B, P)
+        u32 = torch.where(keep[:, :, None], u.to(torch.float32), 0.0)
+        k = self.filter_fn.filter_channel_major(P)
+        fb = self.filter_fn.bias if self.filter_fn.use_bias else 0 * self.filter_fn.bias
+        if self.order > 2:
+            y_pre = self._forward_chained(u32, k, fb, P, keep=keep[:, None, :])
+        elif ops.proj_mode() == "tc" and ops.fuse_fir():
+            y_pre = ops.HyenaInCoreFn.apply(u32, self.in_proj.weight, self.in_proj.bias, self.short_filter.weight,
+                                            self.short_filter.bias, k, fb, None, row_start)
+        else:
+            p = _InProj.apply(u32, self.in_proj.weight)
+            y_pre = ops.HyenaCoreFn.apply(p, self.in_proj.bias, self.short_filter.weight, self.short_filter.bias, k, fb,
+                                          None, row_start)
+        return _OutProj.apply(y_pre, self.out_proj.weight, self.out_proj.bias).to(in_dtype)
 
     def _forward_chained(self, u, k, fb, l_filter, capture=None, keep=None):
         """order >= 3 (the shipped HyenaDNA layer default is 3, configs/model/layer/hyena_dna.yaml:3): the recurrence of

@@ -268,6 +268,12 @@ def _save_spectrum():
     return os.environ.get("HYENA_B200_SAVE_SPECTRUM", "1") != "0"
 
 
+def _check_row_start(row_start, B, dev, what):
+    if row_start is not None and (row_start.dtype != torch.int32 or row_start.device != dev
+                                  or tuple(row_start.shape) != (B,) or not row_start.is_contiguous()):
+        raise _lib.HyenaB200Error(f"{what}: row_start must be a contiguous ({B},) int32 tensor on {dev}")
+
+
 def core_forward(p, in_bias, sw, sb, kspec, fbias, save_c, row_start=None):
     """y_pre (B, D, L) of the fused order-2 core, and c / the g spectrum when save_c.  row_start ((B,) int32 on p's device):
     row b is left-padded, its positions t < row_start[b] are padding (hyena_b200_core_fwd_rows)."""
@@ -284,9 +290,7 @@ def core_forward(p, in_bias, sw, sb, kspec, fbias, save_c, row_start=None):
     # spectrum of the gated input, rows ordered (c, b): saves a column pass + a row FFT per row in backward
     gs = (torch.empty(D * B, kspec.shape[-1], dtype=torch.complex64, device=p.device)
           if (save_c and _save_spectrum()) else None)
-    if row_start is not None and (row_start.dtype != torch.int32 or row_start.device != p.device
-                                  or tuple(row_start.shape) != (B,) or not row_start.is_contiguous()):
-        raise _lib.HyenaB200Error(f"core_forward: row_start must be a contiguous ({B},) int32 tensor on {p.device}")
+    _check_row_start(row_start, B, p.device, "core_forward")
     ws = workspace(B, D, L, False, p.device)
     with torch.cuda.device(p.device):
         if row_start is None:
@@ -300,7 +304,9 @@ def core_forward(p, in_bias, sw, sb, kspec, fbias, save_c, row_start=None):
     return y, c, gs
 
 
-def core_backward(dy_pre, p, in_bias, sw, sb, kspec, fbias, c_saved, gspec=None, return_ds=False):
+def core_backward(dy_pre, p, in_bias, sw, sb, kspec, fbias, c_saved, gspec=None, return_ds=False, row_start=None):
+    """Backward of core_forward.  row_start: the rows were left-padded (core_forward(..., row_start), whose c and g
+    spectrum must be passed here); gradients then cover the real positions only (hyena_b200_core_bwd_rows)."""
     _need_cuda(dy_pre, p, in_bias, sw, sb, fbias, c_saved)
     B, C3, L = p.shape
     D = C3 // 3
@@ -308,6 +314,7 @@ def core_backward(dy_pre, p, in_bias, sw, sb, kspec, fbias, c_saved, gspec=None,
     _check_spectrum(kspec, D, L, "core_backward")
     if tuple(dy_pre.shape) != (B, D, L) or tuple(c_saved.shape) != (B, D, L):
         raise _lib.HyenaB200Error("core_backward: dy_pre / c_saved must be (B, D, L)")
+    _check_row_start(row_start, B, dev, "core_backward")
     dy_pre = dy_pre.contiguous()
     dp = None if return_ds else torch.empty_like(p)
     ds = torch.empty_like(p)
@@ -318,26 +325,50 @@ def core_backward(dy_pre, p, in_bias, sw, sb, kspec, fbias, c_saved, gspec=None,
     dib = torch.zeros(C3, dtype=torch.float32, device=dev) if in_bias is not None else None
     ws = workspace(B, D, L, True, dev)
     with torch.cuda.device(dev):
-        _lib.check(_lib.lib().hyena_b200_core_bwd(
-            _ptr(dy_pre), _ptr(p), _ptr(in_bias), _ptr(sw), _ptr(sb), _ptr(kspec), _ptr(fbias), _ptr(c_saved),
-            _ptr(gspec), _ptr(dp), _ptr(dk), _ptr(dsw), _ptr(dsb), _ptr(dfb), _ptr(dib), _ptr(ds),
-            B, D, L, _ptr(ws), ws.numel(), _stream()))
+        if row_start is None:
+            _lib.check(_lib.lib().hyena_b200_core_bwd(
+                _ptr(dy_pre), _ptr(p), _ptr(in_bias), _ptr(sw), _ptr(sb), _ptr(kspec), _ptr(fbias), _ptr(c_saved),
+                _ptr(gspec), _ptr(dp), _ptr(dk), _ptr(dsw), _ptr(dsb), _ptr(dfb), _ptr(dib), _ptr(ds),
+                B, D, L, _ptr(ws), ws.numel(), _stream()))
+        else:
+            _lib.check(_lib.lib().hyena_b200_core_bwd_rows(
+                _ptr(dy_pre), _ptr(p), _ptr(in_bias), _ptr(sw), _ptr(sb), _ptr(kspec), _ptr(fbias), _ptr(c_saved),
+                _ptr(gspec), _ptr(dp), _ptr(dk), _ptr(dsw), _ptr(dsb), _ptr(dfb), _ptr(dib), _ptr(ds), _ptr(row_start),
+                B, D, L, _ptr(ws), ws.numel(), _stream()))
     if return_ds:
         # d in_proj.bias = sum_t dp[t] = (w0 + w1 + w2) sum_t ds[t] - w1 ds[0] - w0 (ds[0] + ds[1])   (conv padding edge)
         if in_bias is not None:
-            e0 = ds[:, :, 0].sum(0)
-            e1 = ds[:, :, 1].sum(0) if L > 1 else torch.zeros_like(e0)
-            dib = sw.sum(1) * dsb - sw[:, 1] * e0 - sw[:, 0] * (e0 + e1)
+            if row_start is None:
+                e0 = ds[:, :, 0].sum(0)
+                e1 = ds[:, :, 1].sum(0) if L > 1 else torch.zeros_like(e0)
+                dib = sw.sum(1) * dsb - sw[:, 1] * e0 - sw[:, 0] * (e0 + e1)
+            else:
+                dib = rows_in_bias_grad(ds, sw, dsb, row_start)
         return ds, dk, dsw, dsb, dfb, dib
     del ds
     return dp, dk, dsw, dsb, dfb, dib
 
 
+def rows_in_bias_grad(ds, sw, dsb, row_start):
+    """d in_proj.bias of left-padded rows from ds (B, 3D, L), zero at the pads: the edge formula of core_backward at each
+    row's first real position s_b, sum_t dp[t >= s_b] = (w0 + w1 + w2) sum_t ds[t] - w1 ds[s_b] - w0 (ds[s_b] + ds[s_b+1]),
+    summed over the rows (ds[s_b + 1] = 0 past the end, for a row of length 1).  dsb = sum_{b,t} ds."""
+    B, C3, L = ds.shape
+    s0 = row_start.to(torch.long)
+    s1 = s0 + 1
+    e0 = ds.gather(2, s0[:, None, None].expand(B, C3, 1))[..., 0]
+    e1 = ds.gather(2, s1.clamp(max=L - 1)[:, None, None].expand(B, C3, 1))[..., 0]
+    e1 = torch.where((s1 < L)[:, None], e1, 0.0)
+    e0, e1 = e0.sum(0), e1.sum(0)
+    return sw.sum(1) * dsb - sw[:, 1] * e0 - sw[:, 0] * (e0 + e1)
+
+
 class HyenaCoreFn(torch.autograd.Function):
-    """(p, in_bias, short filter, k, filter bias) -> y_pre (B, D, L); hyena.py:394-432 for order 2."""
+    """(p, in_bias, short filter, k, filter bias) -> y_pre (B, D, L); hyena.py:394-432 for order 2.  row_start ((B,) int32
+    on the device): left-padded rows, the masked forward and backward (core_forward / core_backward with row_start)."""
 
     @staticmethod
-    def forward(ctx, p, in_bias, sw, sb, k, fbias, kspec=None):
+    def forward(ctx, p, in_bias, sw, sb, k, fbias, kspec=None, row_start=None):
         p = p.contiguous()
         sw2 = sw.reshape(sw.shape[0], -1).contiguous()
         sb = sb.contiguous(); fbias = fbias.contiguous()
@@ -345,16 +376,16 @@ class HyenaCoreFn(torch.autograd.Function):
         if kspec is None:
             kspec = filter_spectrum(k)
         need = any(ctx.needs_input_grad)
-        y, c, gs = core_forward(p, ib, sw2, sb, kspec, fbias, need)
-        ctx.save_for_backward(p, ib, sw2, sb, kspec, fbias, c, gs)
+        y, c, gs = core_forward(p, ib, sw2, sb, kspec, fbias, need, row_start)
+        ctx.save_for_backward(p, ib, sw2, sb, kspec, fbias, c, gs, row_start)
         ctx.sw_shape = sw.shape
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        p, ib, sw2, sb, kspec, fbias, c, gs = ctx.saved_tensors
-        dp, dk, dsw, dsb, dfb, dib = core_backward(dy, p, ib, sw2, sb, kspec, fbias, c, gs)
-        return dp, dib, dsw.reshape(ctx.sw_shape), dsb, dk, dfb, None
+        p, ib, sw2, sb, kspec, fbias, c, gs, row_start = ctx.saved_tensors
+        dp, dk, dsw, dsb, dfb, dib = core_backward(dy, p, ib, sw2, sb, kspec, fbias, c, gs, row_start=row_start)
+        return dp, dib, dsw.reshape(ctx.sw_shape), dsb, dk, dfb, None, None
 
 
 class HyenaInCoreFn(torch.autograd.Function):
@@ -362,10 +393,14 @@ class HyenaInCoreFn(torch.autograd.Function):
 
     Forward: p = W u^T channel-major (proj_gemm), then the fused core.  Backward: the core returns ds (gradient w.r.t. the
     short-filter outputs) and the two projection-backward GEMMs apply the transposed 3-tap filter to it on the fly, so
-    neither dp nor a separate short-filter backward pass exists (hyena.py:391-432 and its autograd)."""
+    neither dp nor a separate short-filter backward pass exists (hyena.py:391-432 and its autograd).
+
+    row_start ((B,) int32 on the device): left-padded rows.  u must then be zero at the pads: the transposed short filter
+    carries ds into the two positions before each row's start, and a zero u keeps them out of dW (the caller zeroes du
+    there, see HyenaOperator._forward_masked); d in_proj.bias follows per row (rows_in_bias_grad)."""
 
     @staticmethod
-    def forward(ctx, u, W, in_bias, sw, sb, k, fbias, kspec=None):
+    def forward(ctx, u, W, in_bias, sw, sb, k, fbias, kspec=None, row_start=None):
         u = u.contiguous(); W = W.contiguous()
         sw2 = sw.reshape(sw.shape[0], -1).contiguous()
         sb = sb.contiguous(); fbias = fbias.contiguous()
@@ -374,18 +409,19 @@ class HyenaInCoreFn(torch.autograd.Function):
         if kspec is None:
             kspec = filter_spectrum(k)
         need = any(ctx.needs_input_grad)
-        y, c, gs = core_forward(p, ib, sw2, sb, kspec, fbias, need)
-        ctx.save_for_backward(u, W, p, ib, sw2, sb, kspec, fbias, c, gs)
+        y, c, gs = core_forward(p, ib, sw2, sb, kspec, fbias, need, row_start)
+        ctx.save_for_backward(u, W, p, ib, sw2, sb, kspec, fbias, c, gs, row_start)
         ctx.sw_shape = sw.shape
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        u, W, p, ib, sw2, sb, kspec, fbias, c, gs = ctx.saved_tensors
-        ds, dk, dsw, dsb, dfb, dib = core_backward(dy, p, ib, sw2, sb, kspec, fbias, c, gs, return_ds=True)
+        u, W, p, ib, sw2, sb, kspec, fbias, c, gs, row_start = ctx.saved_tensors
+        ds, dk, dsw, dsb, dfb, dib = core_backward(dy, p, ib, sw2, sb, kspec, fbias, c, gs, return_ds=True,
+                                                   row_start=row_start)
         du = proj_gemm(ds, 1, W, True, 1, fir=sw2) if ctx.needs_input_grad[0] else None
         dW = proj_wgrad(ds, u, fir=sw2) if ctx.needs_input_grad[1] else None
-        return du, dW, dib, dsw.reshape(ctx.sw_shape), dsb, dk, dfb, None
+        return du, dW, dib, dsw.reshape(ctx.sw_shape), dsb, dk, dfb, None, None
 
 
 # ------------------------------------------------------------------------------------------ plain fftconv

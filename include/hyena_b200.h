@@ -144,6 +144,22 @@ HY_API int hyena_b200_core_bwd(const float* dy_pre, const float* p, const float*
                         float* ds_scratch, int B, int D, int L,
                         void* workspace, size_t workspace_bytes, void* stream);
 
+/* core_bwd on left-padded rows (training on left-padded batches): the backward of core_fwd_rows with the same row_start
+ * (B) int32 on the device; c_saved and gspec_saved must come from core_fwd_rows.  The windows of x0, x1 and v are masked
+ * as the forward masked them, dc, dg and the three ds outputs are 0 at t < row_start[b], and so dfbias, dsw and dsb sum
+ * over real positions only; dk is the sum over rows of the unpadded rows' dk (time invariance).  With dp non-NULL, dp is 0
+ * at t < row_start[b] and d_in_bias sums dp over real positions only.  With dp == NULL, ds is 0 at the pads but the
+ * transposed short filter applied to it (hyena_b200_proj_gemm / proj_wgrad with fir) reaches t = row_start[b] - 1 and - 2:
+ * the caller zeroes the in_proj input there, which excludes those positions from dW, and zeroes the input gradient there.
+ * The values are not checked (<= 0 masks nothing, >= L masks the whole row).  Pointers 4-byte aligned (kspec, gspec_saved
+ * 8); the same launches as core_bwd, counted under its kinds (and under HYENA_B200_PIPE pipelined the same way); no
+ * allocation, no synchronisation. */
+HY_API int hyena_b200_core_bwd_rows(const float* dy_pre, const float* p, const float* in_bias, const float* sw,
+                                    const float* sb, const float* kspec, const float* fbias, const float* c_saved,
+                                    const float* gspec_saved, float* dp, float* dk, float* dsw, float* dsb, float* dfbias,
+                                    float* d_in_bias, float* ds_scratch, const int* row_start, int B, int D, int L,
+                                    void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- plain long convolution (the reference extension's own surface) ---------------------------
  * fftconv_fwd replaces csrc/fftconv/fftconv.cpp:53-132 for fp32, gelu=false, no dropout mask, no q/v,
  * head_dim=1:  out[b,h,:] = causal_conv(u[b,h,:], k[h,:]) + u[b,h,:] * Dvec[h]     (fftconv_ref,
