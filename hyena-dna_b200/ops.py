@@ -352,9 +352,10 @@ def core_backward(dy_pre, p, in_bias, sw, sb, kspec, fbias, c_saved, gspec=None,
 def rows_in_bias_grad(ds, sw, dsb, row_start):
     """d in_proj.bias of left-padded rows from ds (B, 3D, L), zero at the pads: the edge formula of core_backward at each
     row's first real position s_b, sum_t dp[t >= s_b] = (w0 + w1 + w2) sum_t ds[t] - w1 ds[s_b] - w0 (ds[s_b] + ds[s_b+1]),
-    summed over the rows (ds[s_b + 1] = 0 past the end, for a row of length 1).  dsb = sum_{b,t} ds."""
+    summed over the rows (ds[s_b + 1] = 0 past the end, for a row of length 1).  dsb = sum_{b,t} ds.  A start <= 0 masks
+    nothing (the edge formula at t = 0); a start >= L masks the whole row, whose ds[L - 1] the kernel has zeroed."""
     B, C3, L = ds.shape
-    s0 = row_start.to(torch.long)
+    s0 = row_start.to(torch.long).clamp(0, L - 1)
     s1 = s0 + 1
     e0 = ds.gather(2, s0[:, None, None].expand(B, C3, 1))[..., 0]
     e1 = ds.gather(2, s1.clamp(max=L - 1)[:, None, None].expand(B, C3, 1))[..., 0]

@@ -37,12 +37,14 @@ def _mask(lengths, P):
     return torch.stack([torch.arange(P) >= P - n for n in lengths])
 
 
-def _dy(u, lengths, seed=6):
-    """Upstream gradient on the real positions only (the loss of a padded batch), zero at the pads."""
+def _dy(u, lengths, seed=6, pads="zero"):
+    """Upstream gradient: random on the real positions; at the pads zero (the loss of a padded batch) or, pads="random",
+    random values of a loss that also reads the pad outputs."""
     B, P, D = u.shape
     dy = torch.randn(B, P, D, generator=torch.Generator().manual_seed(seed))
-    for b, n in enumerate(lengths):
-        dy[b, :P - n] = 0.0
+    if pads == "zero":
+        for b, n in enumerate(lengths):
+            dy[b, :P - n] = 0.0
     return dy
 
 
@@ -59,11 +61,16 @@ def _train(model, u, dy, mask, **kw):
 
 
 def _check_truth(res, u, dy, lengths, Pp, op, tag):
-    """Real positions against the per-row truth, all 15 parameter gradients against its sums, the pads exactly."""
+    """Real positions against the per-row truth, all 15 parameter gradients against its sums, the pads exactly.  The
+    outputs at the pads are out_proj.bias, so d out_proj.bias is the truth's plus the sum of dy over the pads; dy at the
+    pads reaches no other gradient."""
     y, du, grads = res
     P = u.shape[1]
     ys32, dus32, s32 = row_truth(u, dy, lengths, Pp, torch.float32)
     ys64, dus64, s64 = row_truth(u, dy, lengths, Pp, torch.float64)
+    pad_dy = sum(dy[b, :P - n].double().sum(0) for b, n in enumerate(lengths))
+    s32["out_proj.bias"] = s32["out_proj.bias"] + pad_dy.float()
+    s64["out_proj.bias"] = s64["out_proj.bias"] + pad_dy
     bias = op.out_proj.bias.detach().cpu()
     for b, n in enumerate(lengths):
         s = P - n
@@ -83,21 +90,34 @@ def _lengths(P):
 
 
 # ---------------------------------------------------------------------------------------------- 1. operator, per-row truth
-@pytest.mark.parametrize("order,D,P", [
+OPERATOR_CASES = [
     (2, 1, 1023), (2, 3, 1026), (2, 100, 1024), (2, 256, 1024), (2, 256, 1023),      # odd: vec = 0; 1026: unstaged
     (3, 3, 1023), (3, 100, 1026), (3, 256, 1024),
-])
-def test_operator_against_per_row_truth(order, D, P):
+]
+
+
+def _with_dy_pads(cases):
+    """Each case with dy zero at the pads (its plain id) and with dy random there (id suffix "dy_pads")."""
+    ids = lambda c: "-".join(map(str, c if isinstance(c, tuple) else (c,)))
+    out = []
+    for c in cases:
+        t = c if isinstance(c, tuple) else (c,)
+        out += [pytest.param(*t, "zero", id=ids(c)), pytest.param(*t, "random", id=ids(c) + "-dy_pads")]
+    return out
+
+
+@pytest.mark.parametrize("order,D,P,dy_pads", _with_dy_pads(OPERATOR_CASES))
+def test_operator_against_per_row_truth(order, D, P, dy_pads):
     lengths = _lengths(P)
     op, Pp = _make(D, P, order)
     u = _padded(len(lengths), P, D, lengths)
-    dy = _dy(u, lengths)
+    dy = _dy(u, lengths, pads=dy_pads)
     _check_truth(_train(op, u, dy, _mask(lengths, P)), u, dy, lengths, Pp, op, f"order {order} D={D} P={P}")
 
 
 # ---------------------------------------------------------------------------------------------- 2. routes
-@pytest.mark.parametrize("route", ["fused", "fir0", "library", "recompute", "batch1", "groups"])
-def test_routes_against_per_row_truth(monkeypatch, route):
+@pytest.mark.parametrize("route,dy_pads", _with_dy_pads(["fused", "fir0", "library", "recompute", "batch1", "groups"]))
+def test_routes_against_per_row_truth(monkeypatch, route, dy_pads):
     H = _H()
     D, P = 8, 2048
     lengths = [2048, 1, 1027, 2, 514]
@@ -115,7 +135,7 @@ def test_routes_against_per_row_truth(monkeypatch, route):
         monkeypatch.setattr(H.ops, "workspace", _exact_workspace(H, 3))
     op, Pp = _make(D, P)
     u = _padded(len(lengths), P, D, lengths)
-    dy = _dy(u, lengths)
+    dy = _dy(u, lengths, pads=dy_pads)
     H._lib.profile_begin()
     res = _train(op, u, dy, _mask(lengths, P))
     prof = {k: v[1] for k, v in H._lib.profile_end().items()}

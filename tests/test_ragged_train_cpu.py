@@ -160,10 +160,12 @@ def test_block_and_backbone_validate_before_the_first_kernel(no_device):
 
 
 # ---------------------------------------------------------------------------------------------- d in_proj.bias per row
-@pytest.mark.parametrize("lengths,L", [([12, 1, 2, 7], 12), ([1, 1], 5), ([2, 9, 3], 9), ([1], 1), ([2, 1], 2)])
+@pytest.mark.parametrize("lengths,L", [([12, 1, 2, 7], 12), ([1, 1], 5), ([2, 9, 3], 9), ([1], 1), ([2, 1], 2),
+                                       ([15, 12, 0, 3], 12), ([9, -5, 2, 10], 9), ([2, 0], 1), ([3, -1], 2)])
 def test_rows_in_bias_grad_matches_autograd(lengths, L):
     """d in_proj.bias = d/d bias of sum_t ds[t] * short(where(t >= s_b, p + bias, 0))[t] in fp64 autograd, against the
-    per-row edge formula of ops.rows_in_bias_grad (ds zero at the pads, as core_bwd_rows leaves it)."""
+    per-row edge formula of ops.rows_in_bias_grad (ds zero at the pads, as core_bwd_rows leaves it).  A length > L is a
+    start < 0, which masks nothing; a length <= 0 is a start >= L, which masks the whole row."""
     H = _H()
     g = torch.Generator().manual_seed(len(lengths) * 100 + L)
     B, C = len(lengths), 6
