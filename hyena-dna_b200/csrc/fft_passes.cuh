@@ -982,7 +982,8 @@ __device__ __forceinline__ void row_pass_body(const PassArgs& a, const int bx, c
 // (issued before the forward row FFT / before the first inverse FFT, so the 2 x 64 dependent __ldg's per thread of the
 // two pointwise phases -- `long_scoreboard`, the top stall of the kernel -- become shared-memory reads).  One 8 KB
 // buffer per row, reused for k then g; the partner row's buffer supplies the mirrored bins.  Shared memory per CTA:
-// rows * (EX + 2 * M2) complex = 99 KB for four rows, two CTAs per SM.  Default for batch 1; HYENA_B200_ROW_BWD1_STAGE=0 selects the register-load form.
+// rows * (EX + 2 * M2) complex = 99 KB for four rows, two CTAs per SM.  Taken for batch 1 when kspec and gspec are 16-byte
+// aligned; otherwise row_pass_kernel<ROW_CONV_BWD1> loads them into registers.
 template <int LOGM2>
 __host__ __device__ constexpr size_t row_bwd1_staged_smem_elems(int rows) {
   return (size_t)rows * (RowGeo<LOGM2>::EX + 2 * RowGeo<LOGM2>::M2);
@@ -1064,8 +1065,8 @@ __device__ __forceinline__ void row_bwd1_staged_body(const PassArgs& a, const in
 // ------------------------------------------------------------------------------------------------
 // Forward row pass with the filter spectrum row staged by cp.async under the forward row FFT (the register form issues 64
 // __ldg per thread right in front of the pointwise product: long_scoreboard is its top stall).  128-thread CTAs of four
-// rows, shared memory rows * (EX + M2) complex = 66.6 KB: three CTAs per SM.  Default;
-// HYENA_B200_ROW_FWD_STAGE=0 selects the register-load form.
+// rows, shared memory rows * (EX + M2) complex = 66.6 KB: three CTAs per SM.  Taken when kspec is 16-byte aligned and
+// M1 >= 4; otherwise row_pass_kernel<ROW_CONV_FWD> loads the filter spectrum into registers.
 // ------------------------------------------------------------------------------------------------
 template <int LOGM2>
 __host__ __device__ constexpr size_t row_fwd_staged_smem_elems(int rows) {
@@ -1125,8 +1126,10 @@ __device__ __forceinline__ void row_fwd_staged_body(const PassArgs& a, const int
   row_ifft_store<LOGM2>(v, ex, Arow, q, id.k1, logM, a.T, rsync);
 }
 
+// ROW_CONV_BWD1 (batch 1) runs 128-thread CTAs at two per SM: up to 255 registers, no spills (three CTAs per SM would cap
+// it at 170 registers with ~80 spilled)
 template <int MODE, int LOGM2>
-__global__ void __launch_bounds__(MODE == ROW_CONV_BWD1 ? 128 : 256, MODE == ROW_CONV_BWD ? 1 : (MODE == ROW_CONV_BWD1 ? 3 : 2))
+__global__ void __launch_bounds__(MODE == ROW_CONV_BWD1 ? 128 : 256, MODE == ROW_CONV_BWD ? 1 : 2)
 row_pass_kernel(const PassArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   row_pass_body<MODE, LOGM2>(a, blockIdx.x, blockIdx.y, smem_raw);

@@ -1,7 +1,7 @@
 // Implicit filter (forward and backward) on the Hopper tensor cores (wgmma), sm_90a.
 //
-// Same math as filter_fwd_kernel (filter_mlp.cuh; reference src/models/sequence/hyena.py:96-155,199-238),
-// but the three GEMM-shaped layers run as wgmma.mma_async ... .tf32 with fp32 accumulators in registers:
+// The filter MLP of filter_params.h (reference src/models/sequence/hyena.py:96-155,199-238), with the three
+// GEMM-shaped layers run as wgmma.mma_async ... .tf32 with fp32 accumulators in registers:
 //
 //   tile = 128 positions; 512 threads = four warpgroups, warpgroup w owns rows 64 (w & 1) .. of the tile and column
 //          half (w >> 1) of every layer (wgmma M = 64)
@@ -18,7 +18,7 @@
 // i.e. 8-row x 16-byte core matrices, LBO (K direction) = 128 B, SBO (M/N direction) = 2048 B.
 #pragma once
 #include "fft_passes.cuh"
-#include "filter_mlp.cuh"
+#include "filter_params.h"
 #include "tc_prims.cuh"
 
 namespace hy {

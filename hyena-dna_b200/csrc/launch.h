@@ -1,7 +1,7 @@
 // Host-side launch entry points implemented in the k_*.cu translation units.
 #pragma once
 #include "fft_passes.cuh"
-#include "filter_mlp.cuh"
+#include "filter_params.h"
 #include "short_conv.cuh"
 #include "layernorm_args.h"
 #include "decode_args.h"
@@ -13,16 +13,15 @@ enum Kind {
   K_COL_FWD = 0,      // + ColMode  (0..3)
   K_COL_INV = 4,      // + InvMode  (4..8)
   K_ROW = 9,          // + RowMode  (9..11)
-  K_FILTER_FWD = 12, K_FILTER_BWD = 13, K_SHORT_BWD = 14, K_TWIDDLE = 15, K_FILTER_TC_PREP = 16, K_FILTER_TC_FWD = 17,
-  K_FILTER_TC_BWD = 18, K_FILTER_TC_RED = 19, K_FUSED_FWD = 20, K_CONVERT = 21, K_PROJ_PREP = 22, K_PROJ_GEMM = 23, K_PROJ_WGRAD = 24,
-  K_PIPE_FWD = 25, K_PIPE_BWD = 26, K_PIPE_FILTER = 27,   // whole pipelined calls (api.cu PipeRun): kernels of different groups overlap
-  K_ADD_LN = 28,            // residual add + LayerNorm (block glue, layernorm.cuh)
-  K_FILTER_EXTRA = 29,      // deltas gradient / channel L1 normalisation (filter_extra.cuh; non-default filter options)
-  K_PROJ_GEMM_GELU = 30, K_PROJ_GEMM_DGELU = 31, K_PROJ_WGRAD_GELU = 32,   // block MLP: projection GEMMs with fused GELU
-  K_DECODE_HIST = 33, K_DECODE_STEP = 34,   // incremental decoding (decode.cuh): history fill, one-position step
-  K_DECODE_EXT_HIST = 35, K_DECODE_EXT_DOT = 36, K_DECODE_EXT_COMBINE = 37,   // extending by n positions (decode_extend.cuh)
-  K_DECODE_WIN_STEP = 38,   // a step inside an open window (decode.cuh): its dot product and combine kernel
-  K_COUNT = 39
+  K_SHORT_BWD = 12, K_TWIDDLE = 13, K_FILTER_TC_PREP = 14, K_FILTER_TC_FWD = 15, K_FILTER_TC_BWD = 16, K_FILTER_TC_RED = 17,
+  K_CONVERT = 18, K_PROJ_PREP = 19, K_PROJ_GEMM = 20, K_PROJ_WGRAD = 21,
+  K_ADD_LN = 22,            // residual add + LayerNorm (block glue, layernorm.cuh)
+  K_FILTER_EXTRA = 23,      // deltas gradient / channel L1 normalisation (filter_extra.cuh; non-default filter options)
+  K_PROJ_GEMM_GELU = 24, K_PROJ_GEMM_DGELU = 25, K_PROJ_WGRAD_GELU = 26,   // block MLP: projection GEMMs with fused GELU
+  K_DECODE_HIST = 27, K_DECODE_STEP = 28,   // incremental decoding (decode.cuh): history fill, one-position step
+  K_DECODE_EXT_HIST = 29, K_DECODE_EXT_DOT = 30, K_DECODE_EXT_COMBINE = 31,   // extending by n positions (decode_extend.cuh)
+  K_DECODE_WIN_STEP = 32,   // a step inside an open window (decode.cuh): its dot product and combine kernel
+  K_COUNT = 33
 };
 void prof_begin(int kind, cudaStream_t s);     // api.cu: records an event when profiling is on
 void prof_end(int kind, cudaStream_t s);       // api.cu: records an event when profiling is on; counts the launch
@@ -32,7 +31,6 @@ cudaError_t launch_col_inv(int mode, const PassArgs& a, int rows, cudaStream_t s
 cudaError_t launch_row_pass(int mode, const PassArgs& a, int rows, cudaStream_t s);
 template <int MODE> cudaError_t launch_col_fwd_mode(const PassArgs& a, int rows, cudaStream_t s);   // k_col_fwd_m*.cu
 template <int MODE> cudaError_t launch_col_inv_mode(const PassArgs& a, int rows, cudaStream_t s);   // k_col_inv_m*.cu
-cudaError_t launch_filter_fwd(const FilterParams& P, float* kout, cudaStream_t s);
 cudaError_t launch_filter_fwd_tc(const FilterParams& P, float* wimg, float* kout, cudaStream_t s);   // k_filter_tc.cu
 size_t filter_tc_wimg_bytes(int D);
 cudaError_t launch_filter_bwd_tc(const FilterParams& P, float* wimg, const float* dk, float* dh, float* scratch, cudaStream_t s);
@@ -40,7 +38,6 @@ struct RedLaunch { const float* dh; const float* scratch; const float* zT; float
                    float* dW2; float* db2; float* dW3; float* dfreq; int L, D, E; };
 size_t filter_red_work_bytes(int L, int D, int E);                       // k_filter_tc.cu
 cudaError_t launch_filter_stage2(const RedLaunch& r, float* work, cudaStream_t s);
-cudaError_t launch_filter_bwd(const FilterParams& P, const float* dk, const FilterGrads& G, cudaStream_t s);
 cudaError_t launch_short_bwd(const ShortBwdArgs& a, int B, cudaStream_t s);
 cudaError_t launch_twiddle_init(float2* tw1024, float2* twlo, cudaStream_t s);
 // k_proj.cu: projection GEMMs on wgmma (3xTF32)

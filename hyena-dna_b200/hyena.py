@@ -213,22 +213,15 @@ class _InProj(torch.autograd.Function):
             dW = torch.bmm(dp, u).sum(0) if ctx.needs_input_grad[1] else None
             return du, dW
         du = dW = None
-        main = torch.cuda.current_stream(u.device)
-        side = ops.side_stream(u.device) if (ctx.needs_input_grad[0] and ctx.needs_input_grad[1]) else None
         if ctx.needs_input_grad[1]:
             dW = torch.empty_like(W)
-            if side is not None:
-                side.wait_stream(main)
-            with torch.cuda.stream(side if side is not None else main):
-                # dW^T (D x 3D, ld D) = sum_b U_b^T (D x L, stored, op N) dP_b^T (L x 3D, stored ld L, op N)
-                for b in range(B):
-                    ops.gemm(0, 0, D, C3, L, u[b], D, 0, dp[b], L, 0, dW, D, 0, batch=1, beta=0.0 if b == 0 else 1.0)
+            # dW^T (D x 3D, ld D) = sum_b U_b^T (D x L, stored, op N) dP_b^T (L x 3D, stored ld L, op N)
+            for b in range(B):
+                ops.gemm(0, 0, D, C3, L, u[b], D, 0, dp[b], L, 0, dW, D, 0, batch=1, beta=0.0 if b == 0 else 1.0)
         if ctx.needs_input_grad[0]:
             du = torch.empty_like(u)
             # dU^T (D x L, ld D) = W^T (D x 3D, stored ld D, op N) dP (3D x L; stored (L x 3D, ld L) -> op T)
             ops.gemm(0, 1, D, L, C3, W, D, 0, dp, L, C3 * L, du, D, L * D, batch=B)
-        if side is not None:
-            main.wait_stream(side)
         return du, dW
 
 
@@ -274,26 +267,17 @@ class _OutProj(torch.autograd.Function):
             db = dy.sum((0, 1)) if (ctx.has_bias and ctx.needs_input_grad[2]) else None
             return d_pre, dW, db
         d_pre = dW = db = None
-        main = torch.cuda.current_stream(dy.device)
-        side = ops.side_stream(dy.device) if (ctx.needs_input_grad[0] and ctx.needs_input_grad[1]) else None
         if ctx.needs_input_grad[1]:
             dW = torch.empty_like(W)
-            if side is not None:
-                side.wait_stream(main)
-            with torch.cuda.stream(side if side is not None else main):
-                # dW^T (C x Do, ld C) = sum_b Ypre_b (C x L; stored (L x C, ld L) -> op T) dY_b (L x Do; stored (Do x L) -> op T)
-                for b in range(B):
-                    ops.gemm(1, 1, C, Do, L, y_pre[b], L, 0, dy[b], Do, 0, dW, C, 0, batch=1, beta=0.0 if b == 0 else 1.0)
-        # db on the caller's stream: a tensor allocated inside the side-stream context and consumed by autograd on the main
-        # stream could be handed back to side-stream work by the caching allocator while main-stream readers are pending
+            # dW^T (C x Do, ld C) = sum_b Ypre_b (C x L; stored (L x C, ld L) -> op T) dY_b (L x Do; stored (Do x L) -> op T)
+            for b in range(B):
+                ops.gemm(1, 1, C, Do, L, y_pre[b], L, 0, dy[b], Do, 0, dW, C, 0, batch=1, beta=0.0 if b == 0 else 1.0)
         if ctx.has_bias and ctx.needs_input_grad[2]:
             db = dy.sum((0, 1))
         if ctx.needs_input_grad[0]:
             d_pre = torch.empty_like(y_pre)
             # dYpre^T (L x C, ld L) = dY (L x Do; stored (Do x L, ld Do) -> op T) W (Do x C; stored (C x Do, ld C) -> op T)
             ops.gemm(1, 1, L, C, Do, dy, Do, L * Do, W, C, 0, d_pre, L, C * L, batch=B)
-        if side is not None:
-            main.wait_stream(side)
         return d_pre, dW, db
 
 
@@ -432,7 +416,7 @@ class HyenaOperator(nn.Module):
                 self._kspec_cache = (kkey, kspec)
         if self.order > 2 or self.filter_fn.bidirectional:
             y_pre = self._forward_chained(u, k, fb, l_filter)
-        elif ops.proj_mode() == "tc" and l_filter == l and ops.fuse_fir():
+        elif ops.proj_mode() == "tc" and l_filter == l:
             # one autograd node: in_proj GEMM + fused core; backward feeds ds straight into the projection GEMMs
             y_pre = ops.HyenaInCoreFn.apply(u, self.in_proj.weight, self.in_proj.bias, self.short_filter.weight,
                                             self.short_filter.bias, k, fb, kspec)
@@ -541,7 +525,7 @@ class HyenaOperator(nn.Module):
         fb = self.filter_fn.bias if self.filter_fn.use_bias else 0 * self.filter_fn.bias
         if self.order > 2:
             y_pre = self._forward_chained(u32, k, fb, P, keep=keep[:, None, :])
-        elif ops.proj_mode() == "tc" and ops.fuse_fir():
+        elif ops.proj_mode() == "tc":
             y_pre = ops.HyenaInCoreFn.apply(u32, self.in_proj.weight, self.in_proj.bias, self.short_filter.weight,
                                             self.short_filter.bias, k, fb, None, row_start)
         else:

@@ -80,8 +80,9 @@ def filter_forward(z, t, W0, b0, W1, b1, W2, b2, W3, freq, deltas, shift, modula
     return k
 
 
-def _filter_backward_tc(z, t, W0, b0, W1, b1, W2, b2, W3, freq, deltas, shift, modulate, L, dk, need_dz):
+def filter_backward(z, t, W0, b0, W1, b1, W2, b2, W3, freq, deltas, shift, modulate, L, dk, need_dz):
     """Tensor-core backward: stage 1 on wgmma (csrc/filter_tc.cuh), stage 2 = sequence-length reductions."""
+    _need_cuda(z, t, W0, b0, W1, b1, W2, b2, W3, freq, deltas, dk)
     zz, tt, E, N, D = _filter_args(z, t, W0, b0, W1, b1, W2, b2, W3, freq, deltas, shift, modulate, L)
     ws = [x.contiguous() for x in (W0, b0, W1, b1, W2, b2, W3)]
     fr = freq.reshape(-1).contiguous()
@@ -107,27 +108,6 @@ def _filter_backward_tc(z, t, W0, b0, W1, b1, W2, b2, W3, freq, deltas, shift, m
         grads = [dp1 @ zz, sums[0], dp2 @ a1.t(), sums[1], dp3 @ a2.t(), sums[2], dh @ a3.t()]
         dfreq = sums[3]
     dz = (dp1.t() @ ws[0]) if need_dz else None
-    return grads, dfreq, dz
-
-
-def filter_backward(z, t, W0, b0, W1, b1, W2, b2, W3, freq, deltas, shift, modulate, L, dk, need_dz):
-    _need_cuda(z, t, W0, b0, W1, b1, W2, b2, W3, freq, deltas, dk)
-    import os
-    if os.environ.get("HYENA_B200_FILTER", "tc") != "simt":
-        return _filter_backward_tc(z, t, W0, b0, W1, b1, W2, b2, W3, freq, deltas, shift, modulate, L, dk, need_dz)
-    zz, tt, E, N, D = _filter_args(z, t, W0, b0, W1, b1, W2, b2, W3, freq, deltas, shift, modulate, L)
-    ws = [x.contiguous() for x in (W0, b0, W1, b1, W2, b2, W3)]
-    fr = freq.reshape(-1).contiguous()
-    dl = deltas.reshape(-1).contiguous()
-    dk = dk.contiguous()
-    grads = [torch.zeros_like(w) for w in ws]
-    dfreq = torch.zeros_like(fr)
-    dz = torch.zeros(L, E, dtype=torch.float32, device=z.device) if need_dz else None
-    with torch.cuda.device(z.device):
-        _lib.check(_lib.lib().hyena_b200_filter_bwd(
-            _ptr(zz), zz.stride(0), _ptr(tt), *[_ptr(w) for w in ws], _ptr(fr), _ptr(dl),
-            float(shift), int(bool(modulate)), int(L), E, N, D, _ptr(dk),
-            *[_ptr(g) for g in grads], _ptr(dfreq), _ptr(dz), E, _stream()))
     return grads, dfreq, dz
 
 
@@ -617,13 +597,6 @@ def proj_gemm(act, act_layout, W, w_transposed, out_layout, bias=None, fir=None,
 _wgrad_cache = {}
 
 
-def fuse_fir():
-    """Transposed short filter fused into the projection-backward GEMMs (default on; HYENA_B200_FUSE_FIR=0 keeps the
-    separate short_conv_bwd pass for A/B runs)."""
-    import os
-    return os.environ.get("HYENA_B200_FUSE_FIR", "1") != "0"
-
-
 def proj_wgrad(X, Y, fir=None, transposed_out=False, gelu=None):
     """dW (M, N) [(N, M) if transposed_out] = sum_{b,pos} X[b][m][pos] Y[b][pos][n]; X (B, M, L), Y (B, L, N)
     (csrc/proj_gemm.cuh wgrad_kernel: wgmma 3xTF32, split-K, deterministic).  gelu ('tanh' | 'none'): the product is
@@ -694,24 +667,6 @@ class MlpFn(torch.autograd.Function):
             dW1 = proj_wgrad(da, x) if need_w1 else None                                # (H, D) = sum da x
             db1 = da.sum((0, 2)) if (ctx.has_b1 and need_b1) else None
         return dx, dW1, db1, dW2, db2, None
-
-
-_side_streams = {}
-
-
-def side_stream(device):
-    """A second stream per device for work that is independent of the main chain (weight-gradient GEMMs run there
-    while the input-gradient GEMM runs on the caller's stream: one op's cuBLASLt input scan overlaps the other's
-    tensor-core phase).  Both GEMMs want the whole chip, so it is OFF unless HYENA_B200_SIDE_STREAM=1."""
-    import os
-    if os.environ.get("HYENA_B200_SIDE_STREAM", "0") != "1":
-        return None
-    key = device.index if device.index is not None else torch.cuda.current_device()
-    s = _side_streams.get(key)
-    if s is None:
-        s = torch.cuda.Stream(device=device)
-        _side_streams[key] = s
-    return s
 
 
 # ------------------------------------------------------------------------------------------ block glue: add + LayerNorm

@@ -35,8 +35,9 @@
 extern "C" {
 #endif
 
-/* 2: hyena_b200_proj_debug_buffer removed (the wgmma projection kernels keep no per-role counters) */
-#define HYENA_B200_ABI_VERSION 2
+/* 2: hyena_b200_proj_debug_buffer removed (the wgmma projection kernels keep no per-role counters)
+ * 3: hyena_b200_filter_bwd removed (the filter backward is hyena_b200_filter_bwd_stage1 + _stage2) */
+#define HYENA_B200_ABI_VERSION 3
 #if defined(__GNUC__)
 #define HY_API __attribute__((visibility("default")))
 #else
@@ -75,17 +76,8 @@ HY_API int hyena_b200_filter_fwd(const float* z, int z_stride, const float* t,
                           const float* freq, const float* deltas, float shift, int modulate,
                           int L, int E, int N, int D, float* k_out, void* stream);
 
-/* autograd of the above (the reference relies on torch autograd; closed form restated in DESIGN.md).
- * dk (D,L) -> parameter grads, all (+=) so callers zero them; dz (L,E; row stride dz_stride) may be NULL. */
-HY_API int hyena_b200_filter_bwd(const float* z, int z_stride, const float* t,
-                          const float* W0, const float* b0, const float* W1, const float* b1,
-                          const float* W2, const float* b2, const float* W3,
-                          const float* freq, const float* deltas, float shift, int modulate,
-                          int L, int E, int N, int D, const float* dk,
-                          float* dW0, float* db0, float* dW1, float* db1, float* dW2, float* db2,
-                          float* dW3, float* dfreq, float* dz, int dz_stride, void* stream);
-
-/* Tensor-core (wgmma, 3xTF32) backward in two stages.  Stage 1: per position, recompute the activations and back-
+/* Backward of the above (the reference relies on torch autograd; closed form restated in DESIGN.md), on the tensor
+ * cores (wgmma, 3xTF32) in two stages.  Stage 1: per position, recompute the activations and back-
  * propagate through the MLP, writing dh = dk * modulation (D,L) and seven feature-major (64,L) arrays into `scratch`
  * (7*64*L floats, 16-byte aligned): a1, a2, a3, dp1, dp2, dp3, X.  Stage 2: the parameter gradients are reductions
  * over the sequence, done as wgmma GEMMs with K = position and fixed-order split-K, so two calls give the same bits
@@ -124,8 +116,8 @@ HY_API int hyena_b200_core_fwd(const float* p, const float* in_bias, const float
  * t = 0 (value 0, no in_proj bias), so g = 0 there, and y_pre and c_save are 0 there.  By time invariance, y_pre of row b
  * at row_start[b] + j is the unpadded row's at j, whatever the pad values of p are.  The values are not checked (<= 0 masks
  * nothing, >= L masks the whole row).  Pointers 4-byte aligned (kspec, gspec_save 8); the same three launches as core_fwd,
- * counted under col_fwd<gate>, row_pass<conv_fwd> and col_inv<conv_fwd> (and under HYENA_B200_PIPE pipelined the same way);
- * no allocation, no synchronisation. */
+ * counted under col_fwd<gate>, row_pass<conv_fwd> and col_inv<conv_fwd>; no
+ * allocation, no synchronisation. */
 HY_API int hyena_b200_core_fwd_rows(const float* p, const float* in_bias, const float* sw, const float* sb,
                                     const float* kspec, const float* fbias, float* y_pre, float* c_save, float* gspec_save,
                                     const int* row_start, int B, int D, int L, void* workspace, size_t workspace_bytes,
@@ -152,8 +144,7 @@ HY_API int hyena_b200_core_bwd(const float* dy_pre, const float* p, const float*
  * transposed short filter applied to it (hyena_b200_proj_gemm / proj_wgrad with fir) reaches t = row_start[b] - 1 and - 2:
  * the caller zeroes the in_proj input there, which excludes those positions from dW, and zeroes the input gradient there.
  * The values are not checked (<= 0 masks nothing, >= L masks the whole row).  Pointers 4-byte aligned (kspec, gspec_saved
- * 8); the same launches as core_bwd, counted under its kinds (and under HYENA_B200_PIPE pipelined the same way); no
- * allocation, no synchronisation. */
+ * 8); the same launches as core_bwd, counted under its kinds; no allocation, no synchronisation. */
 HY_API int hyena_b200_core_bwd_rows(const float* dy_pre, const float* p, const float* in_bias, const float* sw,
                                     const float* sb, const float* kspec, const float* fbias, const float* c_saved,
                                     const float* gspec_saved, float* dp, float* dk, float* dsw, float* dsb, float* dfbias,

@@ -34,7 +34,7 @@ def test_abi_present_and_no_new_kinds():
         header = f.read()
     for name in ("hyena_b200_decode_admit", "hyena_b200_decode_shift"):
         assert name in _lib.SIGNATURES and hasattr(L, name) and name + "(" in header
-    assert L.hyena_b200_abi_version() == 2 and L.hyena_b200_kind_count() == 39
+    assert L.hyena_b200_abi_version() == 3 and L.hyena_b200_kind_count() == 33
 
 
 def _admit(p=PTR, h=PTR, tail=PTR, rows=PTR, rs=None, ib=None, k=2, cache_B=4, order=2, Pn=16, t=32, Lcap=64):

@@ -48,7 +48,7 @@ def test_profiler_kinds_include_decoding():
     L = _lib.lib()
     names = [L.hyena_b200_kind_name(i).decode() for i in range(L.hyena_b200_kind_count())]
     assert "decode_hist" in names and "decode_step" in names
-    assert L.hyena_b200_abi_version() == 2
+    assert L.hyena_b200_abi_version() == 3
 
 
 def _op(**kw):

@@ -28,7 +28,7 @@ def test_extend_abi_present():
         header = f.read()
     for name in NAMES:
         assert name + "(" in header
-    assert L.hyena_b200_abi_version() == 2
+    assert L.hyena_b200_abi_version() == 3
     names = [L.hyena_b200_kind_name(i).decode() for i in range(L.hyena_b200_kind_count())]
     assert {"decode_extend_hist", "decode_extend_dot", "decode_extend_combine"} <= set(names)
 

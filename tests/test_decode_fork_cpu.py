@@ -25,9 +25,9 @@ def test_branch_abi_present():
         header = f.read()
     for name in NAMES:
         assert name in _lib.SIGNATURES and hasattr(L, name) and name + "(" in header
-    assert L.hyena_b200_abi_version() == 2
+    assert L.hyena_b200_abi_version() == 3
     names = [L.hyena_b200_kind_name(i).decode() for i in range(L.hyena_b200_kind_count())]
-    assert names[-1] == "decode_win_step" and len(names) == 39          # branch launches count under existing kinds
+    assert names[-1] == "decode_win_step" and len(names) == 33          # branch launches count under existing kinds
 
 
 def _step(p_t=P, h=P, k=P, f=P, parent=P, v_in=None, o=0, order=2, t=21, b=16, Hc=8, H=8, Lcap=64, R=1):

@@ -22,7 +22,7 @@ def test_win_step_abi_present():
     assert name in _lib.SIGNATURES and hasattr(L, name)
     with open(_lib.os.path.join(_lib._HERE, "..", "include", "hyena_b200.h")) as f:
         assert name + "(" in f.read()
-    assert L.hyena_b200_abi_version() == 2
+    assert L.hyena_b200_abi_version() == 3
     names = [L.hyena_b200_kind_name(i).decode() for i in range(L.hyena_b200_kind_count())]
     assert names[-1] == "decode_win_step" and names.count("decode_win_step") == 1
     assert names[-4:-1] == ["decode_extend_hist", "decode_extend_dot", "decode_extend_combine"]

@@ -113,7 +113,7 @@ def test_c_abi_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(L, name), f"{name} declared in include/hyena_b200.h but not exported"
     assert declared == set(_lib.SIGNATURES), (declared ^ set(_lib.SIGNATURES))
-    assert L.hyena_b200_abi_version() == 2
+    assert L.hyena_b200_abi_version() == 3
     assert L.hyena_b200_max_seqlen() == 1 << 20
     assert L.hyena_b200_spectrum_elems(1000) == 1024 and L.hyena_b200_spectrum_elems(160000) == 262144
 

@@ -8,22 +8,18 @@ every output with an fp64 restatement of the same operation (``core_ref``), thro
 |------------------------------------------------------------|-----------------------------------|----------------------------------------|
 | transform template LOGM1 = 0..10, TWO / G-column geometry  | L                                 | test_fused_core_sweep, test_unfused_core |
 | staged row pass vs row_pass_kernel<ROW_CONV_FWD>           | L (LOGM1 >= 2), kspec alignment   | test_fused_core_sweep, test_operand_addresses[kspec8] |
-| batch-1 backward: staged / 2-CTA fallback / ROW_CONV_BWD   | B, saved gspec, alignment         | test_fused_core_sweep, test_operand_addresses[kspec8], test_spectrum_recompute |
+| batch-1 backward: staged / unstaged BWD1 / ROW_CONV_BWD    | B, saved gspec, alignment         | test_fused_core_sweep, test_operand_addresses[kspec8], test_spectrum_recompute |
 | cp.async column staging (a.stage) vs direct loads          | L mod 4, 16-byte rows             | test_fused_core_sweep, test_operand_addresses[p8] |
 | float2 accesses (a.vec)                                    | L parity, 8-byte rows             | test_fused_core_sweep, test_operand_addresses[p4] |
 | channel groups (carve, c0 > 0, ragged last group)          | workspace size, D > 65535 / B     | test_channel_groups_bitwise, test_operator_batch_300_groups, test_core_full_length_groups |
-| un-fused core: core_bwd with dp, short_conv_bwd            | L > l_max, proj mode, FUSE_FIR=0  | test_unfused_core, test_operator_longer_than_l_max, test_operator_unfused_routes |
+| un-fused core: core_bwd with dp, short_conv_bwd            | L > l_max, proj mode              | test_unfused_core, test_operator_longer_than_l_max, test_operator_unfused_routes |
 | spectrum recompute (gspec == NULL)                         | HYENA_B200_SAVE_SPECTRUM=0        | test_spectrum_recompute                |
-| pipelined row groups (PipeRun, per-slot carving)           | HYENA_B200_PIPE="S,G"             | test_pipelined_row_groups              |
 
 Activations are held to 1e-3 rel with the absolute term scaled by max|ref|, parameter gradients with ``param_grad=True``;
 the fp32 twin of the reference (``ref32``) and its fp64 truth (``ref64``) are both passed, so the S8(c) hatch can apply
 and is book-kept.  The tests marked ``gpu`` need an H100; the reference self-checks at the top run on the CPU.
 """
 import math
-import os
-import subprocess
-import sys
 
 import pytest
 import torch
@@ -33,8 +29,6 @@ from oracle import hyena_oracle as O
 from tests import parity_util as PU
 
 gpu = pytest.mark.gpu
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 # ------------------------------------------------------------------------------------------ fp64 reference of the core
@@ -75,7 +69,7 @@ def decaying_filter(D, L, g):
 
 
 def core_inputs(B, D, L, seed, with_u=False):
-    """Seeded host inputs of one core call (the pipelined child process regenerates the same ones)."""
+    """Seeded host inputs of one core call."""
     g = torch.Generator().manual_seed(seed)
     t = dict(p=torch.randn(B, 3 * D, L, generator=g), ib=torch.randn(3 * D, generator=g) * 0.5,
              sw=(torch.rand(3 * D, 3, generator=g) * 2 - 1) / math.sqrt(3), sb=(torch.rand(3 * D, generator=g) * 2 - 1) / math.sqrt(3),
@@ -234,7 +228,7 @@ def _at_offset(t, nbytes):
 def test_operand_addresses(where, L, B):
     """core_forward / core_backward with operands at a storage offset.  p4: p, dy_pre and c_saved 4 bytes off (no float2
     accesses, vec = 0); p8: 8 bytes off (vec = 1, no cp.async column staging); kspec8: the filter spectrum one complex64
-    element off, which selects the unstaged row_pass_kernel<ROW_CONV_FWD> and, at B = 1, row_pass_bwd1_2cta_kernel."""
+    element off, which selects the unstaged row_pass_kernel<ROW_CONV_FWD> and, at B = 1, <ROW_CONV_BWD1>."""
     H = _H()
     dev = _dev()
     D = 4
@@ -430,16 +424,12 @@ def test_operator_longer_than_l_max(l_max, L):
 
 
 @gpu
-@pytest.mark.parametrize("route", ["fuse_fir_off", "proj_lt"])
+@pytest.mark.parametrize("route", ["proj_lt"])
 def test_operator_unfused_routes(monkeypatch, route):
-    """L == l_max through HyenaCoreFn: with the transposed short filter not fused into the projections
-    (HYENA_B200_FUSE_FIR=0), and with the library projection GEMMs."""
+    """L == l_max through HyenaCoreFn and a separate short_conv_bwd pass, with the library projection GEMMs."""
     H = _H()
     dev = _dev()
-    if route == "fuse_fir_off":
-        monkeypatch.setenv("HYENA_B200_FUSE_FIR", "0")
-    else:
-        monkeypatch.setattr(H.ops, "_proj_mode", "lt" if H.ops.gemm_mode() == "bf16x9" else "torch")
+    monkeypatch.setattr(H.ops, "_proj_mode", "lt" if H.ops.gemm_mode() == "bf16x9" else "torch")
     B, L, D = 2, 2999, 8
     g = torch.Generator().manual_seed(2999)
     P = O.init_params(D, L, emb_dim=5, w=1.0, generator=g)
@@ -477,63 +467,3 @@ def test_spectrum_recompute(monkeypatch, L, B):
     got = dict(dW=W.grad, dib=ib.grad, dsw=sw.grad, dsb=sb.grad, dk=k.grad, dfb=fb.grad)
     _check_core_grads(got, r32, r64, tag, ("dW", "dib", "dsw", "dsb", "dk", "dfb"))
 
-
-# ------------------------------------------------------------------------------------------ 7. pipelined row groups
-PIPE_SEED = 23
-
-
-def _pipe_run(H, B, D, L, dev):
-    t = core_inputs(B, D, L, seed=PIPE_SEED * L + B)
-    ib, sw, sb, k, fb, p, dy = (t[n].to(dev) for n in ("ib", "sw", "sb", "k", "fb", "p", "dy"))
-    o = {}
-    o["kspec"] = H.ops.filter_spectrum(k)
-    o["y"], o["c"], o["gspec"] = H.ops.core_forward(p, ib, sw, sb, o["kspec"], fb, True)
-    o["dp"], o["dk"], o["dsw"], o["dsb"], o["dfb"], o["dib"] = H.ops.core_backward(dy, p, ib, sw, sb, o["kspec"], fb,
-                                                                                   o["c"], o["gspec"])
-    torch.cuda.synchronize()
-    return t, o
-
-
-def pipe_child(path, B, D, L):
-    """Entry point of the child process (HYENA_B200_PIPE is read once per process): writes its outputs and the profiled
-    kernel kinds to ``path``."""
-    import numpy as np
-    H = _H()
-    dev = _dev()
-    H._lib.profile_begin()
-    _, o = _pipe_run(H, B, D, L, dev)
-    prof = H._lib.profile_end()
-    arrs = {n: v.cpu().numpy() for n, v in o.items()}
-    arrs["kinds"] = np.array(sorted(prof))
-    np.savez(path, **arrs)
-
-
-@gpu
-@pytest.mark.parametrize("B", [1, 3])
-@pytest.mark.parametrize("L", [4096, 40000])
-def test_pipelined_row_groups(tmp_path, L, B):
-    """HYENA_B200_PIPE="2,3" (two streams, groups of 3 channels: 3 + 3 + 2 at D = 8) in a child process: per-row
-    outputs bit-identical to the non-pipelined run here, the atomic sums within the fp64 tolerance."""
-    import numpy as np
-    H = _H()
-    dev = _dev()
-    D = 8
-    out = tmp_path / "pipe.npz"
-    env = dict(os.environ, HYENA_B200_PIPE="2,3")
-    code = (f"import sys; sys.path.insert(0, {ROOT!r}); from tests.test_gpu_fft_core_paths import pipe_child; "
-            f"pipe_child({str(out)!r}, {B}, {D}, {L})")
-    res = subprocess.run([sys.executable, "-c", code], env=env, cwd=ROOT, capture_output=True, text=True, timeout=600)
-    assert res.returncode == 0, res.stdout[-2000:] + res.stderr[-4000:]
-    z = np.load(out)
-    kinds = set(z["kinds"].tolist())
-    assert {"filter_spectrum<pipelined>", "conv_fwd<pipelined>", "conv_bwd<pipelined>"} <= kinds, kinds
-    assert "col_fwd<gate>" not in kinds, kinds          # every column pass ran inside a pipelined span
-    t, o = _pipe_run(H, B, D, L, dev)
-    for n in ("kspec", "y", "c", "gspec", "dp", "dk"):
-        assert np.array_equal(z[n], o[n].cpu().numpy()), f"pipelined {n} differs from the non-pipelined run"
-    r32, r64 = core_refs(t["p"], t["ib"], t["sw"], t["sb"], t["k"], t["fb"], t["dy"])
-    tag = f"pipelined B={B} L={L}"
-    _act(o["y"], r32["y"], r64["y"], f"{tag} y_pre")
-    _act(o["dp"], r32["dx"], r64["dx"], f"{tag} dp")
-    got = {n: torch.from_numpy(z[n]) for n in ("dib", "dsw", "dsb", "dk", "dfb")}
-    _check_core_grads(got, r32, r64, tag)

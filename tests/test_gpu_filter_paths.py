@@ -1,8 +1,7 @@
 """The implicit filter's kernels against fp64: every parameter gradient, at the shapes where the kernels branch.
 
 The filter (csrc/filter_tc.cuh: filter_tc_fwd_kernel, filter_tc_bwd_kernel = backward stage 1, filter_tc_red_kernel =
-stage 2; csrc/filter_mlp.cuh behind HYENA_B200_FILTER=simt) picks a code path from L, D, E, the module options and the
-size of its sine arguments.  Each test below drives one family of those decisions on purpose and compares k and every
+stage 2) picks a code path from L, D, E, the module options and the size of its sine arguments.  Each test below drives one family of those decisions on purpose and compares k and every
 gradient (the eight MLP tensors, dz, ddeltas) with ``filter_ref``, the oracle's filter under fp64 autograd:
 
 | decision                                                         | selected by               | test                                  |
@@ -16,7 +15,6 @@ gradient (the eight MLP tensors, dz, ddeltas) with ``filter_ref``, the oracle's 
 | modulation off, shift != 0, trainable deltas, normalized         | module options            | test_module_options                   |
 | z a prefix of a longer embedding (l_max > L), dz                 | lr_pos_emb != 0           | test_z_prefix_of_longer_embedding     |
 | inline Cody-Waite sin/cos vs the |x| > 3e4 library branch        | |freq * pre|              | test_sine_arguments                   |
-| tensor-core vs CUDA-core filter                                  | HYENA_B200_FILTER=simt    | test_cuda_core_filter (child process) |
 | stage 1 on its own (dh and the seven feature-major arrays)       |                           | test_stage1_arrays                    |
 | stage 2 on its own: accumulation over 2^20 positions, flush map  | arrays built by the test  | test_stage2_*                         |
 | per-(device, stream) grow-only weight images                     | D sequence, two streams   | test_weight_images_across_streams     |
@@ -31,9 +29,6 @@ Comparisons go through tests/parity_util.check: activations with the absolute te
 an H100; the reference self-checks at the top run on the CPU.
 """
 import math
-import os
-import subprocess
-import sys
 
 import pytest
 import torch
@@ -42,8 +37,6 @@ from oracle import hyena_oracle as O
 from tests import parity_util as PU
 
 gpu = pytest.mark.gpu
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 MLP = ("implicit_filter.0.weight", "implicit_filter.0.bias", "implicit_filter.2.weight", "implicit_filter.2.bias",
        "implicit_filter.4.weight", "implicit_filter.4.bias", "implicit_filter.6.weight", "implicit_filter.1.freq")
@@ -398,53 +391,7 @@ def test_sine_arguments(w, init_std):
     run_and_check(c, f"sine w={w} init={init_std or 'unit'}")
 
 
-# ------------------------------------------------------------------------------------------ 6. CUDA-core filter
-SIMT_CASES = {
-    "seq": case(256, 4097, dk="tail", seed=11),
-    "channels": case(129, 1000, dk="lastch", seed=12),
-    "wide": case(320, 1500, seed=13),
-    "options": case(256, 40000, shift=0.25, modulation_lr=1e-3, seed=14),
-    "guard": case(64, 4097, guard=True, seed=15),
-}
-
-
-def simt_child(path):
-    """Entry point of the child process (HYENA_B200_FILTER=simt is read once per process by the forward)."""
-    import numpy as np
-    H = _H()
-    dev = _dev()
-    H._lib.profile_begin()
-    arrs = {}
-    for name, c in SIMT_CASES.items():
-        for n, v in run_case(H, c, dev).items():
-            arrs[f"{name}|{n}"] = v.numpy()
-    prof = H._lib.profile_end()
-    arrs["kinds"] = np.array(sorted(prof))
-    np.savez(path, **arrs)
-
-
-@gpu
-def test_cuda_core_filter(tmp_path):
-    """The CUDA-core filter (csrc/filter_mlp.cuh) in a child process with HYENA_B200_FILTER=simt: no tensor-core filter
-    kernel runs, and k and every gradient of the core cases match fp64."""
-    import numpy as np
-    dev = _dev()
-    out = tmp_path / "simt.npz"
-    env = dict(os.environ, HYENA_B200_FILTER="simt")
-    code = f"import sys; sys.path.insert(0, {ROOT!r}); from tests.test_gpu_filter_paths import simt_child; simt_child({str(out)!r})"
-    res = subprocess.run([sys.executable, "-c", code], env=env, cwd=ROOT, capture_output=True, text=True, timeout=900)
-    assert res.returncode == 0, res.stdout[-2000:] + res.stderr[-4000:]
-    z = np.load(out)
-    kinds = set(z["kinds"].tolist())
-    assert {"filter_fwd", "filter_bwd"} <= kinds, kinds
-    assert not any(k.startswith("filter_tc") for k in kinds), kinds
-    for name, c in SIMT_CASES.items():
-        ours = {n: torch.from_numpy(z[f"{name}|{n}"]) for n in ("k",) + expected_grads(c)}
-        r32, r64 = case_refs(c, dev)
-        check_case(f"simt {name}", c, ours, r32, r64)
-
-
-# ------------------------------------------------------------------------------------------ 7. full size
+# ------------------------------------------------------------------------------------------ 6. full size
 @gpu
 @pytest.mark.parametrize("init_std", [0.02, None])
 def test_full_size(init_std):
@@ -457,7 +404,7 @@ def test_full_size(init_std):
         print(f"  {n:28s} {eo:.3e}  {er:.3e}")
 
 
-# ------------------------------------------------------------------------------------------ 8. stage 1 on its own
+# ------------------------------------------------------------------------------------------ 7. stage 1 on its own
 def _mlp_args(f):
     m = f.implicit_filter
     return [a.detach() for a in (f.pos_emb.z, f.pos_emb.t, m[0].weight, m[0].bias, m[2].weight, m[2].bias, m[4].weight,
@@ -499,7 +446,7 @@ def test_stage1_arrays(D, L):
         _act(sc[i], r32[1][i], r64[1][i], f"stage 1 D={D} L={L} {n}")
 
 
-# ------------------------------------------------------------------------------------------ 9. stage 2 on its own
+# ------------------------------------------------------------------------------------------ 8. stage 2 on its own
 # The tensor core adds into its accumulator with truncation.  filter_tc_red_kernel used to chain all MMAs of a CTA's K blocks
 # into one accumulator: on same-sign arrays at L = 2^20 that put dW0 8.5e-5 (relative to max|fp64|) off, 110x the fp32
 # library route.  It now restarts every 8 blocks and flushes with atomic adds, whose own rounding (132 CTAs x ~30 flushes
@@ -592,7 +539,7 @@ def test_stage2_every_emb_dim(E):
     check_stage2("random", 129, E, 4099, seed=10 + E)
 
 
-# ------------------------------------------------------------------------------------------ 10. bar tight enough
+# ------------------------------------------------------------------------------------------ 9. bar tight enough
 @gpu
 def test_parity_bar_rejects_tf32_reference():
     """The fp32 reference with TF32 on (one MMA per product instead of 3xTF32) is rejected at D = 256, L = 40000, for k
@@ -619,7 +566,7 @@ def test_parity_bar_rejects_tf32_reference():
         del PU._records[n0:]
 
 
-# ------------------------------------------------------------------------------------------ 11. streams and determinism
+# ------------------------------------------------------------------------------------------ 10. streams and determinism
 @gpu
 def test_weight_images_across_streams():
     """The weight images are per (device, stream) and only grow.  k, dh and the seven stage-1 arrays are bitwise equal to

@@ -164,19 +164,17 @@ def _exact_workspace(H, G):
 @pytest.mark.parametrize("P,lengths,D,path", [
     (1023, [1023, 1, 2, 3], 16, "staged"),            # odd P: register path, vec = 0
     (1024, [1024, 517, 2, 1], 16, "staged"),
-    (1024, [1024, 517, 2, 1], 16, "register"),
+    (1022, [1022, 517, 2, 1], 16, "register"),        # P % 4 == 2: register path with float2 accesses, LOGM1 of 1024
     (1025, [1025, 1024, 3, 999], 16, "staged"),
     (4096, [4096, 4095, 1, 2], 16, "groups"),         # G = 3 channels per launch: c0 > 0 and a ragged last group
     (65535, [65535, 65535 - 12345, 1, 77], 4, "staged"),
     (65536, [65536, 3, 65535, 40001], 4, "staged"),
-    (65536, [65536, 3, 65535, 40001], 4, "register"),
+    (65534, [65534, 3, 65533, 40001], 4, "register"),  # the same at the LOGM1 of 65536
     (65537, [65537, 2, 65536, 333], 4, "staged"),
 ])
 def test_rows_against_fp64_truth(monkeypatch, P, lengths, D, path):
     H = _H()
     dev = _dev()
-    if path == "register":
-        monkeypatch.setenv("HYENA_B200_NO_STAGE", "1")
     if path == "groups":
         monkeypatch.setattr(H.ops, "workspace", _exact_workspace(H, 3))
     op, Pp = _make(D, P)

@@ -2,9 +2,6 @@
 hyena_b200_core_bwd_rows; DESIGN.md section 4.17).  Truth: the oracle on each row's UNPADDED tokens in fp32 and fp64, the
 parameter gradients summed over the rows (tests/test_ragged_train_cpu.row_truth).  Tolerance policy:
 tests/parity_util.py."""
-import os
-import subprocess
-import sys
 from functools import partial
 
 import pytest
@@ -18,7 +15,6 @@ from tests.test_ragged_train_cpu import row_truth
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SKIP = ("filter_fn.pos_emb.z", "filter_fn.pos_emb.t", "filter_fn.modulation.deltas")
 
 
@@ -116,14 +112,12 @@ def test_operator_against_per_row_truth(order, D, P, dy_pads):
 
 
 # ---------------------------------------------------------------------------------------------- 2. routes
-@pytest.mark.parametrize("route,dy_pads", _with_dy_pads(["fused", "fir0", "library", "recompute", "batch1", "groups"]))
+@pytest.mark.parametrize("route,dy_pads", _with_dy_pads(["fused", "library", "recompute", "batch1", "groups"]))
 def test_routes_against_per_row_truth(monkeypatch, route, dy_pads):
     H = _H()
     D, P = 8, 2048
     lengths = [2048, 1, 1027, 2, 514]
-    if route == "fir0":
-        monkeypatch.setenv("HYENA_B200_FUSE_FIR", "0")
-    elif route == "library":
+    if route == "library":
         H.ops.proj_mode()
         monkeypatch.setattr(H.ops, "_proj_mode", "lt")
         assert H.ops.proj_mode() == "lt"
@@ -141,54 +135,11 @@ def test_routes_against_per_row_truth(monkeypatch, route, dy_pads):
     prof = {k: v[1] for k, v in H._lib.profile_end().items()}
     if route == "recompute":
         assert prof["col_fwd<gate>"] == 2, prof          # forward + the recomputation in the backward
-    if route == "fir0" or route == "library":
+    if route == "library":
         assert prof.get("short_conv_bwd") == 1, prof
     if route == "groups":
         assert prof["col_fwd<dc>"] == 3, prof
     _check_truth(res, u, dy, lengths, Pp, op, f"route {route}")
-
-
-def pipe_child(path):
-    """Entry point of the child process (HYENA_B200_PIPE is read once per process): one masked training step, saved."""
-    import numpy as np
-    H = _H()
-    H._lib.profile_begin()
-    y, du, grads = _pipe_run()
-    prof = H._lib.profile_end()
-    np.savez(path, y=y.numpy(), du=du.numpy(), kinds=np.array(sorted(prof)),
-             **{"g:" + k: v.numpy() for k, v in grads.items()})
-
-
-def _pipe_run():
-    D, P = 8, 4096
-    lengths = [4096, 3, 2001]
-    op, _ = _make(D, P, seed=3)
-    u = _padded(len(lengths), P, D, lengths, seed=3)
-    return _train(op, u, _dy(u, lengths), _mask(lengths, P))
-
-
-def test_pipelined_row_groups(tmp_path):
-    """HYENA_B200_PIPE="2,3" in a child process: y and du bit-identical to the non-pipelined run, every parameter
-    gradient within the fp64 tolerance of the per-row truth (the atomic sums may round differently)."""
-    import numpy as np
-    out = tmp_path / "pipe.npz"
-    env = dict(os.environ, HYENA_B200_PIPE="2,3")
-    code = (f"import sys; sys.path.insert(0, {ROOT!r}); from tests.test_gpu_ragged_train import pipe_child; "
-            f"pipe_child({str(out)!r})")
-    res = subprocess.run([sys.executable, "-c", code], env=env, cwd=ROOT, capture_output=True, text=True, timeout=600)
-    assert res.returncode == 0, res.stdout[-2000:] + res.stderr[-4000:]
-    z = np.load(out)
-    kinds = set(z["kinds"].tolist())
-    assert {"conv_fwd<pipelined>", "conv_bwd<pipelined>"} <= kinds, kinds
-    assert "col_fwd<dc>" not in kinds, kinds
-    y, du, grads = _pipe_run()
-    assert np.array_equal(z["y"], y.numpy()) and np.array_equal(z["du"], du.numpy())
-    D, P, lengths = 8, 4096, [4096, 3, 2001]
-    op, Pp = _make(D, P, seed=3)
-    u = _padded(len(lengths), P, D, lengths, seed=3)
-    got = {k[2:]: torch.from_numpy(z[k]) for k in z.files if k.startswith("g:")}
-    _check_truth((torch.from_numpy(z["y"]), torch.from_numpy(z["du"]), got), u, _dy(u, lengths), lengths, Pp, op,
-                 "pipelined")
 
 
 def test_long_row_2_20():

@@ -16,10 +16,9 @@ is missing shows.  Row starts are placed where a 3-tap window straddling them is
 | cp.async staging / float2 (vec) / scalar accesses          | L mod 4, operand addresses      | test_rows_core_sweep, test_rows_operand_addresses, test_rows_register_path |
 | short_conv_bwd_rows_kernel (dp) / rows_in_bias_grad (ds)   | return_ds                       | every GPU test                   |
 | fused route: in_proj GEMM + core + ds-fed projections      | HyenaInCoreFn                   | test_rows_fused_route            |
-| batch-1 backward: ROW_CONV_BWD1 / 2-CTA fallback           | B = 1, kspec alignment          | test_rows_batch_one              |
+| batch-1 backward: staged / unstaged ROW_CONV_BWD1          | B = 1, kspec alignment          | test_rows_batch_one              |
 | spectrum recompute (COL_GATE_ROWS in the backward)         | HYENA_B200_SAVE_SPECTRUM=0      | test_rows_spectrum_recompute     |
 | channel groups (c0 > 0, ragged last group)                 | workspace size                  | test_rows_channel_groups         |
-| pipelined row groups                                       | HYENA_B200_PIPE="S,G"           | test_rows_pipelined              |
 | pad contents: zeros, random, NaN, +-inf                    | the caller's pads               | test_rows_pad_contents           |
 | starts < 0 (mask nothing) and >= L (mask the whole row)    | row_start                       | test_rows_out_of_range_starts    |
 
@@ -27,10 +26,6 @@ Activations are held to 1e-3 rel with the absolute term scaled by max|ref|, para
 both against the fp32 twin of the reference and its fp64 truth (tests/parity_util.py).  The tests marked ``gpu`` need an
 H100; the reference self-checks and the coverage table run on the CPU.
 """
-import os
-import subprocess
-import sys
-
 import pytest
 import torch
 
@@ -41,8 +36,6 @@ from tests.test_gpu_ragged import _exact_workspace
 from tests.test_gpu_widths import NANS, _poison
 
 gpu = pytest.mark.gpu
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ROWS_PER_CALL = 16
 
 
@@ -409,12 +402,16 @@ def test_rows_fused_route(L):
 
 
 # ------------------------------------------------------------------------------------------ 3. paths
+# the left-padded prefills of tests/test_gpu_ragged.py at these lengths (rows of P, 517, 2, 1 and P, 3, P - 1, 40001)
+REGISTER_STARTS = {1024: [0, 507, 1022, 1023], 65536: [0, 65533, 1, 25535]}
+
+
 @gpu
-@pytest.mark.parametrize("L", [30000, 120000, 400000])              # LOGM1 = 5, 7, 9, L % 4 == 0
-def test_rows_register_path(monkeypatch, L):
-    """HYENA_B200_NO_STAGE=1: the register path of the TWO sizes where cp.async staging would run."""
-    monkeypatch.setenv("HYENA_B200_NO_STAGE", "1")
-    _run_and_check(_H(), _dev(), 3, L, _some_starts(L), seed=41 * L, tag=f"rows register L={L}")
+@pytest.mark.parametrize("L", [1024, 30000, 65536, 120000, 400000])  # LOGM1 = 0, 5, 6, 7, 9, L % 4 == 0
+def test_rows_register_path(L):
+    """p, dy_pre and c 8 bytes off (vec = 1, no cp.async staging): the register path at sizes where staging would run."""
+    starts = REGISTER_STARTS.get(L) or _some_starts(L)
+    _run_and_check(_H(), _dev(), 3, L, starts, seed=41 * L, tag=f"rows register L={L}", p_off=8)
 
 
 @gpu
@@ -428,7 +425,7 @@ def test_rows_operand_addresses(off):
 @gpu
 @pytest.mark.parametrize("kspec_off", [False, True])
 def test_rows_batch_one(kspec_off):
-    """B = 1 with the g spectrum saved: ROW_CONV_BWD1, or with kspec one complex element off the 2-CTA fallback."""
+    """B = 1 with the g spectrum saved: the staged ROW_CONV_BWD1, or with kspec one complex element off the unstaged one."""
     H = _H()
     dev = _dev()
     L = 40000
@@ -467,49 +464,6 @@ def test_rows_channel_groups(monkeypatch, L):
     assert prof["col_fwd<gate>"][1] == 3 and prof["col_fwd<dc>"][1] == 6, prof
     for n in ("y", "c", "dp", "ds", "dk"):
         assert torch.equal(got[n], base[n]), f"rows groups L={L}: {n} differs from the one-group run"
-
-
-PIPE_L, PIPE_D = 40000, 8
-
-
-def pipe_child(path):
-    """Entry point of the child process (HYENA_B200_PIPE is read once per process): writes its outputs and the profiled
-    kernel kinds to ``path``."""
-    import numpy as np
-    H = _H()
-    dev = _dev()
-    starts = _some_starts(PIPE_L)
-    t = rows_inputs(len(starts), PIPE_D, PIPE_L, starts, seed=61)
-    H._lib.profile_begin()
-    o = _rows_run(H, t, starts, dev)
-    prof = H._lib.profile_end()
-    np.savez(path, kinds=np.array(sorted(prof)), **{n: v.numpy() for n, v in o.items()})
-
-
-@gpu
-def test_rows_pipelined(tmp_path):
-    """HYENA_B200_PIPE="2,3" (groups of 3 channels on two streams) in a child process: y_pre and dp bit for bit the
-    non-pipelined run's, every output against the per-row truth."""
-    import numpy as np
-    H = _H()
-    dev = _dev()
-    out = tmp_path / "pipe.npz"
-    env = dict(os.environ, HYENA_B200_PIPE="2,3")
-    code = (f"import sys; sys.path.insert(0, {ROOT!r}); from tests.test_gpu_rows_core_paths import pipe_child; "
-            f"pipe_child({str(out)!r})")
-    res = subprocess.run([sys.executable, "-c", code], env=env, cwd=ROOT, capture_output=True, text=True, timeout=600)
-    assert res.returncode == 0, res.stdout[-2000:] + res.stderr[-4000:]
-    z = np.load(out)
-    kinds = set(z["kinds"].tolist())
-    assert {"conv_fwd<pipelined>", "conv_bwd<pipelined>"} <= kinds, kinds
-    assert "col_fwd<gate>" not in kinds, kinds
-    starts = _some_starts(PIPE_L)
-    t = rows_inputs(len(starts), PIPE_D, PIPE_L, starts, seed=61)
-    o = _rows_run(H, t, starts, dev)
-    for n in ("y", "dp"):
-        assert np.array_equal(z[n], o[n].numpy()), f"pipelined {n} differs from the non-pipelined run"
-    r32, r64 = rows_core_refs(*(t[n] for n in ("p", "ib", "sw", "sb", "k", "fb", "dy")), starts)
-    _check_rows({n: torch.from_numpy(z[n]) for n in z.files if n != "kinds"}, r32, r64, starts, "rows pipelined")
 
 
 # ------------------------------------------------------------------------------------------ 4. pad contents

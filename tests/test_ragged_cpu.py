@@ -27,7 +27,7 @@ def test_abi_present_and_no_new_kinds():
         header = f.read()
     for name in ("hyena_b200_core_fwd_rows", "hyena_b200_decode_hist_rows"):
         assert name in _lib.SIGNATURES and hasattr(L, name) and name + "(" in header
-    assert L.hyena_b200_abi_version() == 2 and L.hyena_b200_kind_count() == 39
+    assert L.hyena_b200_abi_version() == 3 and L.hyena_b200_kind_count() == 33
 
 
 def _core(p=P, sw=P, sb=P, kspec=P, fbias=P, y=P, rs=P, ib=None, c=None, gs=None, B=2, D=8, Lq=1024):

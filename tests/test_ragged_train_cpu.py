@@ -32,7 +32,7 @@ def test_abi_present_and_no_new_kinds():
         header = f.read()
     assert "hyena_b200_core_bwd_rows" in _lib.SIGNATURES and hasattr(L, "hyena_b200_core_bwd_rows")
     assert "hyena_b200_core_bwd_rows(" in header
-    assert L.hyena_b200_abi_version() == 2 and L.hyena_b200_kind_count() == 39
+    assert L.hyena_b200_abi_version() == 3 and L.hyena_b200_kind_count() == 33
 
 
 def _core_bwd(dy=PTR, p=PTR, kspec=PTR, c=PTR, dk=PTR, ds=PTR, rs=PTR, ib=None, gs=None, dp=None, dib=None, B=2, D=8,
