@@ -65,6 +65,12 @@ class Block(nn.Module):
         (HyenaOperator.forward); with the loss on real positions only, every gradient at the pads is 0."""
         if mixer_subset is not None:
             raise HyenaB200Error("Block: mixer_subset is not supported")
+        if mixer_kwargs and mixer_kwargs.get("cu_seqlens") is not None:
+            # flash-attention's unpadded convention: hidden_states (total, D), mixer_kwargs cu_seqlens / max_seqlen
+            kw = dict(mixer_kwargs)
+            kw["cu_seqlens"] = self._check_packed(hidden_states, kw.pop("cu_seqlens"), kw.pop("max_seqlen", None),
+                                                  kw.get("inference_params"), lengths, mask)
+            return self._run(hidden_states, residual, lambda y: self.mixer(y, **kw))
         if mask is not None:
             kw = dict(mixer_kwargs or {})
             pad = self._check_mask(hidden_states, mask, kw.get("inference_params"), lengths)
@@ -79,6 +85,11 @@ class Block(nn.Module):
         if not hasattr(self.mixer, "check_lengths"):
             raise HyenaB200Error(f"Block: the mixer {type(self.mixer).__name__} takes no lengths")
         self.mixer.check_lengths(hidden_states, lengths, cache, how)
+
+    def _check_packed(self, hidden_states, cu_seqlens, max_seqlen=None, cache=None, lengths=None, mask=None):
+        if not hasattr(self.mixer, "check_packed"):
+            raise HyenaB200Error(f"Block: the mixer {type(self.mixer).__name__} takes no cu_seqlens")
+        return self.mixer.check_packed(hidden_states, cu_seqlens, max_seqlen, cache, lengths, mask)
 
     def _check_mask(self, hidden_states, mask, cache=None, lengths=None):
         if not hasattr(self.mixer, "check_mask"):
@@ -153,9 +164,18 @@ class Backbone(nn.Module):
                   prenorm=True, residual_in_fp32=residual_in_fp32) for _ in range(n_layer)])
         self.ln_f = nn.LayerNorm(d_model, eps=layer_norm_epsilon)
 
-    def forward(self, hidden_states, lengths=None, mask=None):
+    def forward(self, hidden_states, lengths=None, mask=None, cu_seqlens=None, max_seqlen=None):
         """``lengths``: left-padded rows (HyenaOperator.forward), inference only.  ``mask``: the (B, L) attention mask of a
-        left-padded batch (the reference datamodules' ``mask`` batch kwarg), differentiable (HyenaOperator.forward)."""
+        left-padded batch (the reference datamodules' ``mask`` batch kwarg), differentiable (HyenaOperator.forward).
+        ``cu_seqlens`` / ``max_seqlen``: packed sequences, hidden_states (total, D) or (1, total, D) (HyenaOperator.forward),
+        validated once for all layers."""
+        if cu_seqlens is not None:
+            pk = self.layers[0]._check_packed(hidden_states, cu_seqlens, max_seqlen, None, lengths, mask)
+            residual = None
+            for layer in self.layers:
+                hidden_states, residual = layer(hidden_states, residual, mixer_kwargs={"cu_seqlens": pk})
+            y, _ = Block._add_norm(hidden_states, residual, self.ln_f)
+            return y.to(hidden_states.dtype)
         if mask is not None:                  # validated once: the layers get the LeftPadding
             mask = self.layers[0]._check_mask(hidden_states, mask, None, lengths)
         if lengths is not None:

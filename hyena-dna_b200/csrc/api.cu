@@ -397,10 +397,12 @@ HY_API int hyena_b200_spectrum_to_rfft(const float* dk, int fft_size, float* dfi
   return 0;
 }
 
-// the three forward passes of core_fwd; row_start non-null: the left-padded modes (core_fwd_rows), the same launch sequence
+// the three forward passes of core_fwd; row_start non-null: the left-padded modes (core_fwd_rows), seg_base non-null as
+// well: the packed modes (core_fwd_packed, channel stride `total`); the same launch sequence
 static int core_fwd_run(const float* p, const float* in_bias, const float* sw, const float* sb, const float* kspec,
                         const float* fbias, float* y_pre, float* c_save, float* gspec_save, const int* row_start, int B,
-                        int D, int L, void* workspace, size_t workspace_bytes, void* stream) {
+                        int D, int L, void* workspace, size_t workspace_bytes, void* stream,
+                        const long long* seg_base = nullptr, long long total = 0) {
   cudaStream_t s = (cudaStream_t)stream;
   Twiddles T;
   if (get_twiddles(s, &T)) return 1;
@@ -413,7 +415,13 @@ static int core_fwd_run(const float* p, const float* in_bias, const float* sw, c
   a.row_start = row_start;
   a.vec = ((L & 1) == 0) && aligned8(p) && aligned8(y_pre) && (!c_save || aligned8(c_save));
   a.stage = ((L & 3) == 0) && aligned16(p);
-  const int col_mode = row_start ? COL_GATE_ROWS : COL_GATE, inv_mode = row_start ? INV_CONV_FWD_ROWS : INV_CONV_FWD;
+  int col_mode = row_start ? COL_GATE_ROWS : COL_GATE, inv_mode = row_start ? INV_CONV_FWD_ROWS : INV_CONV_FWD;
+  if (seg_base) {            // packed: scalar accesses to p and y_pre; vec covers c_save only
+    a.seg_base = seg_base; a.cstride = total;
+    a.vec = ((L & 1) == 0) && (!c_save || aligned8(c_save));
+    a.stage = 0;
+    col_mode = COL_GATE_PACKED; inv_mode = INV_CONV_FWD_PACKED;
+  }
   for (int c0 = 0; c0 < D; c0 += c.nch) {
     const int n = (D - c0 < c.nch) ? D - c0 : c.nch;
     a.c0 = c0;
@@ -448,11 +456,13 @@ HY_API int hyena_b200_core_fwd_rows(const float* p, const float* in_bias, const 
                       workspace_bytes, stream);
 }
 
-// the backward passes of core_bwd; row_start non-null: the left-padded modes (core_bwd_rows), the same launch sequence
+// the backward passes of core_bwd; row_start non-null: the left-padded modes (core_bwd_rows), seg_base non-null as well:
+// the packed modes (core_bwd_packed: dp == NULL, ds_scratch packed); the same launch sequence
 static int core_bwd_run(const float* dy_pre, const float* p, const float* in_bias, const float* sw, const float* sb,
                         const float* kspec, const float* fbias, const float* c_saved, const float* gspec_saved, float* dp,
                         float* dk, float* dsw, float* dsb, float* dfbias, float* d_in_bias, float* ds_scratch,
-                        const int* row_start, int B, int D, int L, void* workspace, size_t workspace_bytes, void* stream) {
+                        const int* row_start, int B, int D, int L, void* workspace, size_t workspace_bytes, void* stream,
+                        const long long* seg_base = nullptr, long long total = 0) {
   cudaStream_t s = (cudaStream_t)stream;
   Twiddles T;
   if (get_twiddles(s, &T)) return 1;
@@ -462,11 +472,17 @@ static int core_bwd_run(const float* dy_pre, const float* p, const float* in_bia
   a.kspec = reinterpret_cast<const float2*>(kspec);
   a.p = p; a.in_bias = in_bias; a.sw = sw; a.sb = sb; a.fbias = fbias;
   a.row_start = row_start;
-  const int dc_mode = row_start ? COL_DC_ROWS : COL_DC, gate_mode = row_start ? COL_GATE_ROWS : COL_GATE,
-            dg_mode = row_start ? INV_BWD_DG_ROWS : INV_BWD_DG;
+  int dc_mode = row_start ? COL_DC_ROWS : COL_DC, gate_mode = row_start ? COL_GATE_ROWS : COL_GATE,
+      dg_mode = row_start ? INV_BWD_DG_ROWS : INV_BWD_DG;
   a.vec = ((L & 1) == 0) && aligned8(p) && aligned8(dy_pre) && aligned8(c_saved) && aligned8(dk) &&
           aligned8(ds_scratch);
   a.stage = ((L & 3) == 0) && aligned16(p) && aligned16(dy_pre) && aligned16(c_saved);
+  if (seg_base) {            // packed: scalar accesses to p, dy_pre and ds; vec covers c_saved and dk only
+    a.seg_base = seg_base; a.cstride = total;
+    a.vec = ((L & 1) == 0) && aligned8(c_saved) && aligned8(dk);
+    a.stage = 0;
+    dc_mode = COL_DC_PACKED; gate_mode = COL_GATE_PACKED; dg_mode = INV_BWD_DG_PACKED;
+  }
   for (int c0 = 0; c0 < D; c0 += c.nch) {
     const int n = (D - c0 < c.nch) ? D - c0 : c.nch;
     a.c0 = c0; a.B = B;
@@ -490,7 +506,8 @@ static int core_bwd_run(const float* dy_pre, const float* p, const float* in_bia
   // dp == NULL: the caller consumes ds directly (hyena_b200_proj_gemm / proj_wgrad apply the transposed short filter on
   // the fly and d in_proj.bias follows from dsb and two edge samples), so dp never exists in HBM.
   if (dp) {
-    ShortBwdArgs sa{ds_scratch, nullptr, in_bias, sw, dp, dsw, dsb, d_in_bias, L, 3 * D, a.vec && aligned8(dp), row_start};
+    ShortBwdArgs sa{ds_scratch, nullptr, in_bias, sw, dp, dsw, dsb, d_in_bias, L, 3 * D, a.vec && aligned8(dp), row_start,
+                    nullptr, 0};
     HY_CUDA(launch_short_bwd(sa, B, s));
   }
   return 0;
@@ -524,6 +541,60 @@ HY_API int hyena_b200_core_bwd_rows(const float* dy_pre, const float* p, const f
            "8-byte aligned");
   return core_bwd_run(dy_pre, p, in_bias, sw, sb, kspec, fbias, c_saved, gspec_saved, dp, dk, dsw, dsb, dfbias, d_in_bias,
                       ds_scratch, row_start, B, D, L, workspace, workspace_bytes, stream);
+}
+
+// the arguments every packed entry point shares: B rows of length L over a packed tensor of `total` positions
+static int check_packed(const long long* seg_base, const int* row_start, long long total, int B, int D, int L) {
+  if (check_shape(B, D, L)) return 1;
+  HY_CHECK(total >= 1, "bad packed length total=%lld", total);
+  HY_CHECK(seg_base && row_start, "null pointer");
+  HY_CHECK(aligned8(seg_base) && aligned4(row_start), "misaligned pointer: seg_base must be 8-byte and row_start 4-byte "
+           "aligned");
+  return 0;
+}
+
+HY_API int hyena_b200_core_fwd_packed(const float* p, const float* in_bias, const float* sw, const float* sb,
+                                      const float* kspec, const float* fbias, float* y_pre, float* c_save,
+                                      float* gspec_save, const long long* seg_base, const int* row_start, long long total,
+                                      int B, int D, int L, void* workspace, size_t workspace_bytes, void* stream) {
+  if (check_packed(seg_base, row_start, total, B, D, L)) return 1;
+  HY_CHECK(p && sw && sb && kspec && fbias && y_pre, "null pointer");
+  HY_CHECK(aligned4(p) && aligned4(sw) && aligned4(sb) && aligned4(fbias) && aligned4(y_pre) &&
+               (!in_bias || aligned4(in_bias)) && (!c_save || aligned4(c_save)),
+           "misaligned pointer: p, in_bias, sw, sb, fbias, y_pre and c_save must be 4-byte aligned");
+  HY_CHECK(aligned8(kspec) && (!gspec_save || aligned8(gspec_save)), "misaligned pointer: kspec and gspec_save must be "
+           "8-byte aligned");
+  return core_fwd_run(p, in_bias, sw, sb, kspec, fbias, y_pre, c_save, gspec_save, row_start, B, D, L, workspace,
+                      workspace_bytes, stream, seg_base, total);
+}
+
+HY_API int hyena_b200_core_bwd_packed(const float* dy_pre, const float* p, const float* in_bias, const float* sw,
+                                      const float* sb, const float* kspec, const float* fbias, const float* c_saved,
+                                      const float* gspec_saved, float* dk, float* dsw, float* dsb, float* dfbias,
+                                      float* ds, const long long* seg_base, const int* row_start, long long total, int B,
+                                      int D, int L, void* workspace, size_t workspace_bytes, void* stream) {
+  if (check_packed(seg_base, row_start, total, B, D, L)) return 1;
+  HY_CHECK(dy_pre && p && sw && sb && kspec && fbias && c_saved && dk && dsw && dsb && dfbias && ds, "null pointer");
+  HY_CHECK(aligned4(dy_pre) && aligned4(p) && aligned4(sw) && aligned4(sb) && aligned4(fbias) && aligned4(c_saved) &&
+               aligned4(dk) && aligned4(dsw) && aligned4(dsb) && aligned4(dfbias) && aligned4(ds) &&
+               (!in_bias || aligned4(in_bias)),
+           "misaligned pointer: every float operand must be 4-byte aligned");
+  HY_CHECK(aligned8(kspec) && (!gspec_saved || aligned8(gspec_saved)), "misaligned pointer: kspec and gspec_saved must be "
+           "8-byte aligned");
+  return core_bwd_run(dy_pre, p, in_bias, sw, sb, kspec, fbias, c_saved, gspec_saved, nullptr, dk, dsw, dsb, dfbias,
+                      nullptr, ds, row_start, B, D, L, workspace, workspace_bytes, stream, seg_base, total);
+}
+
+HY_API int hyena_b200_short_bwd_packed(const float* ds, const float* sw, float* dp, float* d_in_bias,
+                                       const long long* seg_base, const int* row_start, long long total, int B, int C3,
+                                       int L, void* stream) {
+  if (check_packed(seg_base, row_start, total, B, C3, L)) return 1;
+  HY_CHECK(ds && sw && dp, "null pointer");
+  HY_CHECK(aligned4(ds) && aligned4(sw) && aligned4(dp) && (!d_in_bias || aligned4(d_in_bias)),
+           "misaligned pointer: ds, sw, dp and d_in_bias must be 4-byte aligned");
+  ShortBwdArgs sa{ds, nullptr, nullptr, sw, dp, nullptr, nullptr, d_in_bias, L, C3, 0, row_start, seg_base, total};
+  HY_CUDA(launch_short_bwd(sa, B, (cudaStream_t)stream));
+  return 0;
 }
 
 /* OUT[pos][n] = sum_k ACT[pos][k] W'[n][k] (+ bias[n]) on wgmma, fp32 accuracy (3xTF32); see include/hyena_b200.h */

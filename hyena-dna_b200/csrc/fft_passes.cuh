@@ -137,20 +137,47 @@ __device__ __forceinline__ float2 mask_pair(float2 v, int t0, int rs) {
   return make_float2(t0 >= rs ? v.x : 0.f, t0 + 1 >= rs ? v.y : 0.f);
 }
 
+// Packed sequences (the *_PACKED modes): row b of a bucket is one sequence of a packed (C, total) tensor.  Its position t
+// sits at seg_base[b] + t of every channel (channel stride `total`), and its real positions are [rs, L).  Positions t < rs
+// lie in the previous sequence or before the buffer: every access is predicated on t >= rs, so nothing there is read (it
+// reads as the padding the *_ROWS modes mask) or written.  Scalar accesses: a sequence may start at any offset.
+__device__ __forceinline__ void load_window_seg(const float* __restrict__ row, int t0, int L, int rs, float ib,
+                                                float (&P)[4]) {
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const int t = t0 - 2 + j;
+    P[j] = (t >= rs && t < L) ? __ldg(row + t) + ib : 0.f;
+  }
+}
+__device__ __forceinline__ float2 load_pair_seg(const float* __restrict__ row, int t0, int L, int rs) {
+  return make_float2(t0 >= rs ? __ldg(row + t0) : 0.f, (t0 + 1 >= rs && t0 + 1 < L) ? __ldg(row + t0 + 1) : 0.f);
+}
+__device__ __forceinline__ void store_pair_seg(float* __restrict__ row, int t0, int L, int rs, float2 v) {
+  if (t0 >= rs) row[t0] = v.x;
+  if (t0 + 1 >= rs && t0 + 1 < L) row[t0 + 1] = v.y;
+}
+
 // ------------------------------------------------------------------------------------------------
 // argument blocks
 // ------------------------------------------------------------------------------------------------
 // *_ROWS: the core modes on left-padded rows; row b's samples t < row_start[b] are padding (g, y_pre and c_save are 0
 // there, and the short filters see zeros; backward: dc, dg and the three ds are 0 there).  Their launches count under the
 // kind of the plain mode (col_kind / inv_kind).
-enum ColMode { COL_FILTER = 0, COL_GATE = 1, COL_DC = 2, COL_PLAIN = 3, COL_GATE_ROWS = 4, COL_DC_ROWS = 5 };
+// *_PACKED: the same modes on packed sequences (see load_window_seg): p, dy_pre, y_pre and ds are packed (C, total) tensors
+// addressed through seg_base, c_save stays in the bucket's row layout (B, D, L); they run the register (unstaged) path.
+enum ColMode { COL_FILTER = 0, COL_GATE = 1, COL_DC = 2, COL_PLAIN = 3, COL_GATE_ROWS = 4, COL_DC_ROWS = 5,
+               COL_GATE_PACKED = 6, COL_DC_PACKED = 7 };
 enum InvMode { INV_CONV_FWD = 0, INV_BWD_DG = 1, INV_DK = 2, INV_PLAIN_FWD = 3, INV_PLAIN_BWD = 4, INV_CONV_FWD_ROWS = 5,
-               INV_BWD_DG_ROWS = 6 };
+               INV_BWD_DG_ROWS = 6, INV_CONV_FWD_PACKED = 7, INV_BWD_DG_PACKED = 8 };
 __host__ __device__ constexpr int col_kind(int mode) {
-  return mode == COL_GATE_ROWS ? COL_GATE : mode == COL_DC_ROWS ? COL_DC : mode;
+  return (mode == COL_GATE_ROWS || mode == COL_GATE_PACKED) ? COL_GATE
+         : (mode == COL_DC_ROWS || mode == COL_DC_PACKED)   ? COL_DC
+                                                             : mode;
 }
 __host__ __device__ constexpr int inv_kind(int mode) {
-  return mode == INV_CONV_FWD_ROWS ? INV_CONV_FWD : mode == INV_BWD_DG_ROWS ? INV_BWD_DG : mode;
+  return (mode == INV_CONV_FWD_ROWS || mode == INV_CONV_FWD_PACKED) ? INV_CONV_FWD
+         : (mode == INV_BWD_DG_ROWS || mode == INV_BWD_DG_PACKED)   ? INV_BWD_DG
+                                                                     : mode;
 }
 // the backward pass-3 epilogue (plain or on left-padded rows)
 __host__ __device__ constexpr bool inv_bwd_dg(int mode) { return mode == INV_BWD_DG || mode == INV_BWD_DG_ROWS; }
@@ -187,7 +214,9 @@ struct PassArgs {
   float* red;            // INV_BWD_DG: dfbias (D); INV_PLAIN_BWD: dD (H)   (atomicAdd)
   float* dsw;            // INV_BWD_DG: d short_filter.weight (3D,3) (atomicAdd)
   float* dsb;            // INV_BWD_DG: d short_filter.bias (3D)     (atomicAdd)
-  const int* row_start;  // *_ROWS modes: (B) first real position of each batch row
+  const int* row_start;  // *_ROWS and *_PACKED modes: (B) first real position of each batch row
+  const long long* seg_base;  // *_PACKED modes: (B) offset of row b's position 0 in a packed channel (may be < 0)
+  long long cstride;          // *_PACKED modes: channel stride of the packed tensors (total positions)
 };
 
 __device__ __forceinline__ size_t row_off(int b, int ch, int nch, int L) { return ((size_t)b * nch + ch) * (size_t)L; }
@@ -242,8 +271,21 @@ struct WarpSync { __device__ __forceinline__ void operator()() const { __syncwar
 // input sample pair (x[t0], x[t0+1]) of row (b, c) for the forward column pass
 template <int MODE>
 __device__ __forceinline__ float2 col_input(const PassArgs& a, int b, int c, int t0, bool vec,
-                                            const Taps& ka, const Taps& kb, int rs = 0) {
-  if constexpr (MODE == COL_GATE_ROWS) {         // COL_GATE on a left-padded row starting at rs
+                                            const Taps& ka, const Taps& kb, int rs = 0, long long sg = 0) {
+  if constexpr (MODE == COL_GATE_PACKED) {       // COL_GATE on a packed sequence (row base sg, real from rs)
+    float P[4];
+    load_window_seg(a.p + (sg + (long long)(a.D + c) * a.cstride), t0, a.L, rs, ka.ib, P);
+    const float2 x1 = conv_window(P, t0, a.L, ka);
+    load_window_seg(a.p + (sg + (long long)(2 * a.D + c) * a.cstride), t0, a.L, rs, kb.ib, P);
+    const float2 v = conv_window(P, t0, a.L, kb);
+    return mask_pair(make_float2(x1.x * v.x, x1.y * v.y), t0, rs);
+  } else if constexpr (MODE == COL_DC_PACKED) {  // COL_DC on a packed sequence: dc is 0 at t < rs
+    float P[4];
+    load_window_seg(a.p + (sg + (long long)c * a.cstride), t0, a.L, rs, ka.ib, P);
+    const float2 x0 = conv_window(P, t0, a.L, ka);
+    const float2 dy = load_pair_seg(a.src + (sg + (long long)c * a.cstride), t0, a.L, rs);
+    return mask_pair(make_float2(x0.x * dy.x, x0.y * dy.y), t0, rs);
+  } else if constexpr (MODE == COL_GATE_ROWS) {  // COL_GATE on a left-padded row starting at rs
     float P[4];
     load_window(a.p + row_off(b, a.D + c, 3 * a.D, a.L), t0, a.L, vec, ka.ib, P);
     mask_window(P, t0, rs);
@@ -298,15 +340,20 @@ __device__ __forceinline__ void col_fwd_body(const PassArgs& a, const int bx, co
 
   Taps ka{}, kb{};
   [[maybe_unused]] int rs = 0;
-  if constexpr (MODE == COL_GATE || MODE == COL_GATE_ROWS) {
+  [[maybe_unused]] long long sg = 0;
+  if constexpr (MODE == COL_GATE || MODE == COL_GATE_ROWS || MODE == COL_GATE_PACKED) {
     ka = load_taps(a.sw, a.sb, a.in_bias, a.D + c);
     kb = load_taps(a.sw, a.sb, a.in_bias, 2 * a.D + c);
     if constexpr (MODE == COL_GATE_ROWS) rs = __ldg(a.row_start + b);
-  } else if constexpr (MODE == COL_DC) {
+  } else if constexpr (MODE == COL_DC || MODE == COL_DC_PACKED) {
     ka = load_taps(a.sw, a.sb, a.in_bias, c);
   } else if constexpr (MODE == COL_DC_ROWS) {
     ka = load_taps(a.sw, a.sb, a.in_bias, c);
     rs = __ldg(a.row_start + b);
+  }
+  if constexpr (MODE == COL_GATE_PACKED || MODE == COL_DC_PACKED) {
+    rs = __ldg(a.row_start + b);
+    sg = __ldg(a.seg_base + b);
   }
 
   float2 v[32];
@@ -356,7 +403,7 @@ __device__ __forceinline__ void col_fwd_body(const PassArgs& a, const int bx, co
         constexpr int n1 = decltype(n_)::value;
         const int m1 = CG::R2 * n1 + q;
         const int t0 = 2 * (m1 * kM2 + m2);
-        v[n1] = (t0 < L) ? col_input<MODE>(a, b, c, t0, vec, ka, kb, rs) : make_float2(0.f, 0.f);
+        v[n1] = (t0 < L) ? col_input<MODE>(a, b, c, t0, vec, ka, kb, rs, sg) : make_float2(0.f, 0.f);
       });
     }
     static_for<16, 32>([&](auto n_) { v[decltype(n_)::value] = make_float2(0.f, 0.f); });
@@ -383,7 +430,7 @@ __device__ __forceinline__ void col_fwd_body(const PassArgs& a, const int bx, co
       static_for<0, M1>([&](auto m_) {
         constexpr int m1 = decltype(m_)::value;
         const int t0 = 2 * (m1 * kM2 + m2);
-        v[gi * M1 + m1] = (t0 < L) ? col_input<MODE>(a, b, c, t0, vec, ka, kb, rs) : make_float2(0.f, 0.f);
+        v[gi * M1 + m1] = (t0 < L) ? col_input<MODE>(a, b, c, t0, vec, ka, kb, rs, sg) : make_float2(0.f, 0.f);
       });
       dif<M1, gi * M1, false, 32>(v);
       static_for<0, M1>([&](auto k_) {
@@ -414,7 +461,8 @@ struct InvCtx {
   float red;           // per-thread partial of the reduction this mode produces
   float rw[3][3];      // INV_BWD_DG: partials of d short_filter.weight for the x0 / x1 / v channels
   float rb[3];         //             and of d short_filter.bias
-  int rs;              // INV_CONV_FWD_ROWS / INV_BWD_DG_ROWS: first real position of the row
+  int rs;              // INV_CONV_FWD_ROWS / INV_BWD_DG_ROWS / *_PACKED: first real position of the row
+  long long sg;        // *_PACKED: offset of the row's position 0 in a packed channel
 };
 
 // dw_j += ds[t0] P(t0-2+j) + ds[t0+1] P(t0-1+j);  db += ds[t0] + ds[t0+1]     (P = window of the filter input)
@@ -442,6 +490,14 @@ __device__ __forceinline__ void inv_load(const PassArgs& a, const InvCtx& cx, in
     in.b = load_pair(a.src + row_off(b, c, D, L), t0, L, vec);
   } else if constexpr (MODE == INV_CONV_FWD || MODE == INV_CONV_FWD_ROWS) {
     load_window(a.p + row_off(b, c, 3 * D, L), t0, L, vec, cx.k0.ib, in.P0);     // x0 only: c = y already holds bias * g
+  } else if constexpr (MODE == INV_CONV_FWD_PACKED) {
+    load_window_seg(a.p + (cx.sg + (long long)c * a.cstride), t0, L, cx.rs, cx.k0.ib, in.P0);
+  } else if constexpr (MODE == INV_BWD_DG_PACKED) {
+    load_window_seg(a.p + (cx.sg + (long long)c * a.cstride), t0, L, cx.rs, cx.k0.ib, in.P0);
+    load_window_seg(a.p + (cx.sg + (long long)(D + c) * a.cstride), t0, L, cx.rs, cx.k1.ib, in.P1);
+    load_window_seg(a.p + (cx.sg + (long long)(2 * D + c) * a.cstride), t0, L, cx.rs, cx.k2.ib, in.P2);
+    in.a = load_pair_seg(a.src + (cx.sg + (long long)c * a.cstride), t0, L, cx.rs);
+    in.b = load_pair(a.src2 + row_off(b, c, D, L), t0, L, vec);       // c_saved: the bucket's row layout
   } else if constexpr (inv_bwd_dg(MODE)) {
     load_window(a.p + row_off(b, c, 3 * D, L), t0, L, vec, cx.k0.ib, in.P0);
     load_window(a.p + row_off(b, D + c, 3 * D, L), t0, L, vec, cx.k1.ib, in.P1);
@@ -474,6 +530,26 @@ __device__ __forceinline__ void inv_finish(const PassArgs& a, InvCtx& cx, int b,
     const float2 cm = mask_pair(y, t0, cx.rs);
     if (a.out2) store_pair(a.out2 + row_off(b, c, D, L), t0, L, vec, cm);
     store_pair(a.out + row_off(b, c, D, L), t0, L, vec, mask_pair(pmul(y, x0), t0, cx.rs));
+  } else if constexpr (MODE == INV_CONV_FWD_PACKED) { // a packed sequence: y_pre is stored at t >= rs only, c_save (row
+    const float2 x0 = conv_window(in.P0, t0, L, cx.k0);  // layout) is 0 at t < rs; the windows are 0 there already
+    if (a.out2) store_pair(a.out2 + row_off(b, c, D, L), t0, L, vec, mask_pair(y, t0, cx.rs));
+    store_pair_seg(a.out + (cx.sg + (long long)c * a.cstride), t0, L, cx.rs, pmul(y, x0));
+  } else if constexpr (MODE == INV_BWD_DG_PACKED) {   // INV_BWD_DG_ROWS on a packed sequence: ds is stored at t >= rs only
+    const float2 x0 = conv_window(in.P0, t0, L, cx.k0), x1 = conv_window(in.P1, t0, L, cx.k1),
+                 vv = conv_window(in.P2, t0, L, cx.k2);
+    const float2 dy = in.a, cs = in.b;
+    const float2 dc = mask_pair(pmul(dy, x0), t0, cx.rs);
+    const float2 dg = mask_pair(y, t0, cx.rs);
+    cx.red = fmaf(dc.x, x1.x * vv.x, fmaf(dc.y, x1.y * vv.y, cx.red));
+    const float2 d0 = mask_pair(pmul(dy, cs), t0, cx.rs);
+    const float2 d1 = mask_pair(pmul(dg, vv), t0, cx.rs);
+    const float2 d2 = mask_pair(pmul(dg, x1), t0, cx.rs);
+    store_pair_seg(a.out2 + (cx.sg + (long long)c * a.cstride), t0, L, cx.rs, d0);
+    store_pair_seg(a.out2 + (cx.sg + (long long)(D + c) * a.cstride), t0, L, cx.rs, d1);
+    store_pair_seg(a.out2 + (cx.sg + (long long)(2 * D + c) * a.cstride), t0, L, cx.rs, d2);
+    tap_grads(cx.rw[0], cx.rb[0], d0, in.P0);
+    tap_grads(cx.rw[1], cx.rb[1], d1, in.P1);
+    tap_grads(cx.rw[2], cx.rb[2], d2, in.P2);
   } else if constexpr (MODE == INV_BWD_DG_ROWS) {     // INV_BWD_DG on a left-padded row: the windows are masked as the
     float P0[4], P1[4], P2[4];                        // forward masked them, dc, dg and the three ds are 0 at t < rs, so
 #pragma unroll                                        // dbias and the tap gradients see real positions only
@@ -543,7 +619,12 @@ __device__ __forceinline__ void col_inv_body(const PassArgs& a, const int bx, co
     cx.k0 = load_taps(a.sw, a.sb, a.in_bias, c);
     cx.rs = __ldg(a.row_start + b);
   }
-  if constexpr (inv_bwd_dg(MODE)) {
+  if constexpr (MODE == INV_CONV_FWD_PACKED || MODE == INV_BWD_DG_PACKED) {
+    cx.k0 = load_taps(a.sw, a.sb, a.in_bias, c);
+    cx.rs = __ldg(a.row_start + b);
+    cx.sg = __ldg(a.seg_base + b);
+  }
+  if constexpr (inv_bwd_dg(MODE) || MODE == INV_BWD_DG_PACKED) {
     cx.k1 = load_taps(a.sw, a.sb, a.in_bias, a.D + c);
     cx.k2 = load_taps(a.sw, a.sb, a.in_bias, 2 * a.D + c);
   }
@@ -625,7 +706,9 @@ __device__ __forceinline__ void col_inv_body(const PassArgs& a, const int bx, co
       });
     } else {
       // register path: slots are handled four at a time with all their loads issued before the first use
-      constexpr int NB = (MODE == INV_DK) ? 1 : 4;
+      // (the packed backward epilogue spills up to 204 bytes with four slots in flight, at most 8 with two: less than
+      // INV_BWD_DG_ROWS)
+      constexpr int NB = (MODE == INV_DK) ? 1 : (MODE == INV_BWD_DG_PACKED) ? 2 : 4;
       static_for<0, 16 / NB>([&](auto g_) {
         constexpr int s0 = decltype(g_)::value * NB;
         InvIn in[NB];
@@ -664,12 +747,12 @@ __device__ __forceinline__ void col_inv_body(const PassArgs& a, const int bx, co
     });
   }
 
-  if constexpr (inv_bwd_dg(MODE) || MODE == INV_PLAIN_BWD) {
-    constexpr int NR = inv_bwd_dg(MODE) ? 13 : 1;
+  if constexpr (inv_bwd_dg(MODE) || MODE == INV_BWD_DG_PACKED || MODE == INV_PLAIN_BWD) {
+    constexpr int NR = MODE == INV_PLAIN_BWD ? 1 : 13;
     __shared__ float red_all[8][NR];
     float vals[NR];
     vals[0] = cx.red;
-    if constexpr (inv_bwd_dg(MODE)) {
+    if constexpr (MODE != INV_PLAIN_BWD) {
 #pragma unroll
       for (int ch = 0; ch < 3; ++ch) {
 #pragma unroll

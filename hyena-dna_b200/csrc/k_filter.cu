@@ -25,7 +25,8 @@ cudaError_t launch_twiddle_init(float2* tw1024, float2* twlo, cudaStream_t s) {
 cudaError_t launch_short_bwd(const ShortBwdArgs& a, int B, cudaStream_t s) {
   dim3 grid((a.L + kScSpan - 1) / kScSpan, a.C3, B);
   prof_begin(K_SHORT_BWD, s);
-  if (a.row_start) short_conv_bwd_rows_kernel<<<grid, 256, 0, s>>>(a);
+  if (a.seg_base) short_conv_bwd_packed_kernel<<<grid, 256, 0, s>>>(a);
+  else if (a.row_start) short_conv_bwd_rows_kernel<<<grid, 256, 0, s>>>(a);
   else short_conv_bwd_kernel<<<grid, 256, 0, s>>>(a);
   prof_end(K_SHORT_BWD, s);
   return cudaGetLastError();

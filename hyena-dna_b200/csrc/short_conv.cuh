@@ -8,6 +8,9 @@
 // Left-padded rows (row_start non-null, short_conv_bwd_rows_kernel): positions t < row_start[b] are padding that the forward
 // zeroed before the filter, so dp is 0 there (the transposed filter would carry ds[rs], ds[rs+1] into rs-1, rs-2) and they
 // stay out of d in_bias; a pad sample of a window reads 0.
+// Packed sequences (seg_base non-null, short_conv_bwd_packed_kernel): row b is one sequence of the packed (3D, total) ds and
+// dp, addressed as in the *_PACKED FFT modes.  ds is read and dp written at t >= row_start[b] only, so the transposed filter
+// stops at the sequence's last position and nothing of the previous sequence is touched.  dsw / dsb come from pass 3.
 #pragma once
 #include "fft_passes.cuh"
 
@@ -26,6 +29,8 @@ struct ShortBwdArgs {
   float* dib;           // (3D)    atomicAdd (d in_proj.bias) or null
   int L, C3, vec;
   const int* row_start; // (B) first real position of each row, or null (plain kernel)
+  const long long* seg_base;   // (B) packed sequences: offset of row b's position 0 in a channel, or null
+  long long cstride;           // packed sequences: channel stride (total positions)
 };
 
 #ifdef HY_FILTER_KERNEL_TU
@@ -78,6 +83,42 @@ __device__ __forceinline__ void short_conv_bwd_body(const ShortBwdArgs& a) {
     if (threadIdx.x < 3) { if (a.p) atomicAdd(a.dsw + 3 * ch + threadIdx.x, s); }
     else if (threadIdx.x == 3) { if (a.p) atomicAdd(a.dsb + ch, s); }
     else if (a.dib) atomicAdd(a.dib + ch, s);
+  }
+}
+
+__global__ void __launch_bounds__(256) short_conv_bwd_packed_kernel(const ShortBwdArgs a) {
+  const int ch = blockIdx.y, b = blockIdx.z;
+  const int L = a.L;
+  const int rs = __ldg(a.row_start + b);
+  const int tbeg = blockIdx.x * kScSpan;
+  const int tend = min(L, tbeg + kScSpan);
+  if (tend <= rs) return;                      // the whole span is before the sequence (uniform per CTA)
+  const long long off = __ldg(a.seg_base + b) + (long long)ch * a.cstride;
+  const float* ds = a.ds + off;
+  float* dp = a.dp + off;
+  const float w0 = __ldg(a.sw + 3 * ch), w1 = __ldg(a.sw + 3 * ch + 1), w2 = __ldg(a.sw + 3 * ch + 2);
+  float r = 0.f;                               // d in_bias
+  for (int t0 = tbeg + 2 * threadIdx.x; t0 < tend; t0 += 512) {
+    if (t0 + 1 < rs) continue;
+    const float2 d0 = load_pair_seg(ds, t0, L, rs);
+    const float2 d1 = (t0 + 2 < L) ? load_pair_seg(ds, t0 + 2, L, rs) : make_float2(0.f, 0.f);
+    float2 o;
+    o.x = fmaf(w2, d0.x, fmaf(w1, d0.y, w0 * d1.x));
+    o.y = fmaf(w2, d0.y, fmaf(w1, d1.x, w0 * d1.y));
+    o = mask_pair(o, t0, rs);
+    store_pair_seg(dp, t0, L, rs, o);
+    r += o.x + ((t0 + 1 < L) ? o.y : 0.f);
+  }
+  if (!a.dib) return;
+  __shared__ float red[8];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) r += __shfl_xor_sync(0xffffffffu, r, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = r;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float s = 0.f;
+    for (int w = 0; w < 8; ++w) s += red[w];
+    atomicAdd(a.dib + ch, s);
   }
 }
 

@@ -328,6 +328,41 @@ def host_mask_starts(mask, batch, positions, device):
     return LeftPadding(starts, row_start, positions)
 
 
+class Packing:
+    """Validated packed sequences (HyenaOperator.check_packed): ``cu`` the cumulative lengths on the host, ``plan`` the
+    bucket plan (ops.packed_plan), ``tables`` its row bases and starts on the device, ``max_len`` the longest sequence.
+    Block and Backbone pass it on to their mixers as ``cu_seqlens`` so that it is validated, and copied, once per call."""
+
+    def __init__(self, cu, plan, tables, max_len, device):
+        self.cu, self.plan, self.tables, self.max_len, self.device = cu, plan, tables, max_len, device
+
+    @property
+    def total(self):
+        return self.cu[-1]
+
+
+def host_cu_seqlens(cu_seqlens, total, device):
+    """cu_seqlens ((N+1,) integer, on the CPU or on ``device``) -> the list on the host, checked with one device-to-host
+    copy: cu[0] == 0, non-decreasing, cu[N] == total."""
+    if not torch.is_tensor(cu_seqlens):
+        raise HyenaB200Error(f"cu_seqlens must be a (N+1,) integer tensor; got {type(cu_seqlens).__name__}")
+    if cu_seqlens.dtype.is_floating_point or cu_seqlens.dtype.is_complex or cu_seqlens.dtype == torch.bool:
+        raise HyenaB200Error(f"cu_seqlens must be an integer tensor; got {cu_seqlens.dtype}")
+    if cu_seqlens.dim() != 1 or cu_seqlens.numel() < 2:
+        raise HyenaB200Error(f"cu_seqlens must be (N+1,) with N >= 1; got shape {tuple(cu_seqlens.shape)}")
+    if cu_seqlens.device.type != "cpu" and cu_seqlens.device != device:
+        raise HyenaB200Error(f"cu_seqlens must be on the CPU or on the input's device {device}; got {cu_seqlens.device}")
+    cu = [int(x) for x in cu_seqlens.detach().cpu().tolist()]
+    if cu[0] != 0:
+        raise HyenaB200Error(f"cu_seqlens[0] must be 0; got {cu[0]}")
+    for i in range(len(cu) - 1):
+        if cu[i + 1] < cu[i]:
+            raise HyenaB200Error(f"cu_seqlens must be non-decreasing; cu_seqlens[{i + 1}] = {cu[i + 1]} < {cu[i]}")
+    if cu[-1] != total:
+        raise HyenaB200Error(f"cu_seqlens[-1] = {cu[-1]} must equal the number of packed positions {total}")
+    return cu
+
+
 class HyenaOperator(nn.Module):
     """Hyena operator (hyena.py:270-448): order 2 as one fused pass on sm_90a, order >= 3 as a chain of its kernels.
 
@@ -365,7 +400,7 @@ class HyenaOperator(nn.Module):
         self.filter_fn = HyenaFilter(self.head_dim * inner_factor * (order - 1), order=filter_order, seq_len=l_max,
                                      channels=1, dropout=filter_dropout, **filter_args)
 
-    def forward(self, u, *args, lengths=None, mask=None, **kwargs):
+    def forward(self, u, *args, lengths=None, mask=None, cu_seqlens=None, max_seqlen=None, **kwargs):
         """``lengths`` (B integers in [1, L]): u is left-padded, row b's real tokens are its last lengths[b] positions.  Its
         outputs there do not depend on the padding: they are the outputs of the unpadded row (DESIGN.md section 4.14); at a
         pad position the output is out_proj(0) = out_proj.bias.  Inference only: with grad required it raises (use
@@ -375,8 +410,17 @@ class HyenaOperator(nn.Module):
         same masked operator, differentiable (DESIGN.md section 4.17).  Outputs and every gradient at real positions are
         the unpadded rows', parameter gradients are the sums over rows of the unpadded rows', du is 0 at the pads and the
         pad contents (NaN and inf included) change nothing.  Under torch.no_grad() it gives the bits of
-        ``forward(u, lengths=mask.sum(-1))``.  Not with ``lengths`` or a DecodeCache (decoding takes ``lengths``)."""
+        ``forward(u, lengths=mask.sum(-1))``.  Not with ``lengths`` or a DecodeCache (decoding takes ``lengths``).
+
+        ``cu_seqlens`` ((N+1,) integer cumulative lengths, on the CPU or on u's device; flash-attention's unpadded
+        convention): u is (total, D) or (1, total, D), sequences packed without padding, sequence i at positions
+        [cu_seqlens[i], cu_seqlens[i+1]).  Each sequence runs as if alone (DESIGN.md section 4.18); the output has u's
+        shape.  ``max_seqlen``, when given, must be at least the longest sequence.  Order 2 with a causal filter only;
+        not with ``lengths``, ``mask`` or a DecodeCache."""
         cache = kwargs.get("inference_params")
+        if cu_seqlens is not None:
+            y = self._forward_packed(u, self.check_packed(u, cu_seqlens, max_seqlen, cache, lengths, mask))
+            return (y, None) if self.return_state else y
         if mask is not None:
             y = self._forward_masked(u, self.check_mask(u, mask, cache, lengths))
             return (y, None) if self.return_state else y
@@ -459,6 +503,60 @@ class HyenaOperator(nn.Module):
         if not u.is_cuda:
             raise HyenaB200Error("HyenaOperator (hyena_b200) runs on CUDA sm_90a only; there is no CPU fallback")
         return pad
+
+    def check_packed(self, u, cu_seqlens, max_seqlen=None, cache=None, lengths=None, mask=None):
+        """Every host check of ``forward(u, cu_seqlens=..., max_seqlen=...)`` without device work (Block and Backbone
+        run it before their first kernel) -> Packing (``cu_seqlens`` may be one already)."""
+        if lengths is not None or mask is not None:
+            raise HyenaB200Error("cu_seqlens does not combine with lengths or mask: packed sequences have no padding")
+        if isinstance(cache, DecodeCache):
+            raise HyenaB200Error("cu_seqlens does not combine with a DecodeCache: prefill packed prompts one by one, or "
+                                 "left-padded with lengths=")
+        if self.order != 2:
+            raise HyenaB200Error(f"cu_seqlens needs order 2; this operator has order {self.order}")
+        if self.filter_fn.bidirectional:
+            raise HyenaB200Error("cu_seqlens needs a causal filter; this HyenaFilter is bidirectional")
+        if not (u.dim() == 2 or (u.dim() == 3 and u.shape[0] == 1)) or u.shape[-1] != self.d_model:
+            raise HyenaB200Error(f"packed input must be (total, {self.d_model}) or (1, total, {self.d_model}); "
+                                 f"got {tuple(u.shape)}")
+        total = u.shape[-2]
+        if isinstance(cu_seqlens, Packing):
+            if cu_seqlens.total != total or cu_seqlens.device != u.device:
+                raise HyenaB200Error("this Packing was validated for another input length or device")
+            pk = cu_seqlens
+        else:
+            cu = host_cu_seqlens(cu_seqlens, total, u.device)
+            max_len = max(cu[i + 1] - cu[i] for i in range(len(cu) - 1))
+            pk = Packing(cu, None, None, max_len, u.device)
+        if pk.max_len > self.l_max:
+            raise HyenaB200Error(f"a packed sequence of {pk.max_len} positions exceeds l_max = {self.l_max}")
+        if max_seqlen is not None and int(max_seqlen) < pk.max_len:
+            raise HyenaB200Error(f"max_seqlen = {int(max_seqlen)} is shorter than the longest sequence ({pk.max_len})")
+        if not u.is_cuda:
+            raise HyenaB200Error("HyenaOperator (hyena_b200) runs on CUDA sm_90a only; there is no CPU fallback")
+        if pk.plan is None:
+            pk.plan = ops.packed_plan(pk.cu)
+            pk.tables = ops._bucket_tables(pk.plan, u.device)
+        return pk
+
+    def _forward_packed(self, u, pk):
+        """forward(u, cu_seqlens=...): in_proj and out_proj as one B = 1 GEMM each over the packed tokens, the fused core
+        per bucket of sequences (ops.PackedCoreFn: hyena_b200_core_fwd_packed / core_bwd_packed / short_bwd_packed)."""
+        if pk.total == 0 or pk.max_len == 0:
+            return u * 0
+        in_dtype, shape, total = u.dtype, u.shape, pk.total
+        u32 = u.reshape(total, self.d_model).to(torch.float32)
+        # the channel-major projection operands take their vector path at a length that is a multiple of 4: the packed
+        # tensors get up to 3 trailing positions that belong to no sequence (zero in u, y_pre and dp)
+        tp = -(-total // 4) * 4
+        if tp != total:
+            u32 = torch.nn.functional.pad(u32, (0, 0, 0, tp - total))
+        k = self.filter_fn.filter_channel_major(pk.max_len)
+        fb = self.filter_fn.bias if self.filter_fn.use_bias else 0 * self.filter_fn.bias
+        p = _InProj.apply(u32[None], self.in_proj.weight)                            # (1, 3D, tp)
+        y_pre = ops.PackedCoreFn.apply(p, self.in_proj.bias, self.short_filter.weight, self.short_filter.bias, k, fb, pk)
+        y = _OutProj.apply(y_pre, self.out_proj.weight, self.out_proj.bias)[0, :total]
+        return y.reshape(shape).to(in_dtype)
 
     def check_lengths(self, u, lengths, cache=None, how="forward"):
         """Every host check of ``how``(u, [cache,] lengths=lengths) -- "forward", "prefill", "extend" or "step" -- without

@@ -405,6 +405,162 @@ class HyenaInCoreFn(torch.autograd.Function):
         return du, dW, dib, dsw.reshape(ctx.sw_shape), dsb, dk, dfb, None, None
 
 
+# ------------------------------------------------------------------------------------------ packed sequences
+MAX_BUCKET_ROWS = 65535          # rows of one launch (the library's batch limit): larger buckets run in chunks
+
+
+def bucket_length(n):
+    """Row length of a packed sequence of n >= 1 positions: its transform size M = max(1024, 2^ceil(log2 n)), the row
+    length of hyena_b200_spectrum_elems."""
+    return max(1024, 1 << (int(n) - 1).bit_length())
+
+
+class PackedBucket:
+    """Sequences of one row length L: ``seqs`` their indices, ``seg_base`` the packed offset of each row's position 0
+    (cu[i+1] - L, may be negative) and ``row_start`` its first real position (L - n_i).  ``offset``: where the bucket's
+    rows start in the plan's concatenated device tables."""
+
+    def __init__(self, L, seqs, seg_base, row_start, offset):
+        self.L, self.seqs, self.seg_base, self.row_start, self.offset = L, seqs, seg_base, row_start, offset
+
+    def __repr__(self):
+        return f"PackedBucket(L={self.L}, rows={len(self.seqs)})"
+
+
+def packed_plan(cu):
+    """Bucket plan of packed sequences (DESIGN.md section 4.18), on the host: sequence i is positions [cu[i], cu[i+1]).
+    Each sequence runs as a row of bucket_length(n_i) positions, chosen from its own length alone, with its real positions
+    at the end of the row; zero-length sequences are skipped.  Buckets come in increasing L, rows in sequence order, and
+    a bucket of more than MAX_BUCKET_ROWS rows is split."""
+    by_len = {}
+    for i in range(len(cu) - 1):
+        n = cu[i + 1] - cu[i]
+        if n > 0:
+            by_len.setdefault(bucket_length(n), []).append(i)
+    plan, offset = [], 0
+    for L in sorted(by_len):
+        seqs = by_len[L]
+        for j in range(0, len(seqs), MAX_BUCKET_ROWS):
+            part = seqs[j:j + MAX_BUCKET_ROWS]
+            plan.append(PackedBucket(L, part, [cu[i + 1] - L for i in part], [L - (cu[i + 1] - cu[i]) for i in part],
+                                     offset))
+            offset += len(part)
+    return plan
+
+
+def _bucket_tables(plan, device):
+    """The plan's seg_base (int64) and row_start (int32) tables on ``device``: one host-to-device copy each."""
+    sb = torch.tensor([x for b in plan for x in b.seg_base], dtype=torch.int64)
+    rs = torch.tensor([x for b in plan for x in b.row_start], dtype=torch.int32)
+    if device.type == "cuda":
+        sb = sb.pin_memory().to(device, non_blocking=True)
+        rs = rs.pin_memory().to(device, non_blocking=True)
+    return sb, rs
+
+
+def _bucket_filter(k, L):
+    """k (D, Lk) cut or zero-padded to the bucket's row length L: taps past a sequence's length never reach its outputs."""
+    D, Lk = k.shape
+    if Lk >= L:
+        return k[:, :L].contiguous()
+    kb = torch.zeros(D, L, dtype=k.dtype, device=k.device)
+    kb[:, :Lk] = k
+    return kb
+
+
+def core_forward_packed(p, in_bias, sw, sb, k, fbias, plan, tables, save, total=None):
+    """y_pre (1, D, T) of the fused order-2 core on packed sequences: p (1, 3D, T) packed (channel stride T), k (D, Lk)
+    the filter of the longest sequence, plan / tables from packed_plan / _bucket_tables.  One core_fwd_packed per bucket.
+    Positions [total, T) belong to no sequence: y_pre is 0 there.  Returns y_pre and, per bucket, (kspec, c, g spectrum)
+    (c and the spectrum only when save)."""
+    _need_cuda(p, in_bias, sw, sb, fbias, k)
+    _, C3, T = p.shape
+    D = C3 // 3
+    if C3 != 3 * D or p.shape[0] != 1 or not p.is_contiguous():
+        raise _lib.HyenaB200Error("core_forward_packed: p must be contiguous (1, 3D, T)")
+    seg_base, row_start = tables
+    y = torch.empty(1, D, T, dtype=torch.float32, device=p.device)
+    y[..., T if total is None else total:] = 0.0
+    saved = []
+    with torch.cuda.device(p.device):
+        for bk in plan:
+            B, L = len(bk.seqs), bk.L
+            kspec = filter_spectrum(_bucket_filter(k, L))
+            c = torch.empty(B, D, L, dtype=torch.float32, device=p.device) if save else None
+            gs = (torch.empty(D * B, kspec.shape[-1], dtype=torch.complex64, device=p.device)
+                  if (save and _save_spectrum()) else None)
+            ws = workspace(B, D, L, False, p.device)
+            _lib.check(_lib.lib().hyena_b200_core_fwd_packed(
+                _ptr(p), _ptr(in_bias), _ptr(sw), _ptr(sb), _ptr(kspec), _ptr(fbias), _ptr(y), _ptr(c), _ptr(gs),
+                _ptr(seg_base[bk.offset:]), _ptr(row_start[bk.offset:]), T, B, D, L, _ptr(ws), ws.numel(), _stream()))
+            saved.append((kspec, c, gs))
+    return y, saved
+
+
+def core_backward_packed(dy_pre, p, in_bias, sw, sb, fbias, Lk, plan, tables, saved, total=None):
+    """Backward of core_forward_packed -> dp (1, 3D, T) packed (0 at [total, T)), dk (D, Lk) (each bucket's dk summed
+    into its first taps), and the sums over real positions dsw, dsb, dfbias and d in_bias (None without in_bias)."""
+    _need_cuda(dy_pre, p, in_bias, sw, sb, fbias)
+    _, C3, T = p.shape
+    D = C3 // 3
+    dev = p.device
+    if tuple(dy_pre.shape) != (1, D, T):
+        raise _lib.HyenaB200Error("core_backward_packed: dy_pre must be (1, D, T)")
+    dy_pre = dy_pre.contiguous()
+    seg_base, row_start = tables
+    ds = torch.empty_like(p)
+    dp = torch.empty_like(p)
+    dp[..., T if total is None else total:] = 0.0
+    dk = torch.zeros(D, Lk, dtype=torch.float32, device=dev)
+    dsw = torch.zeros(C3, 3, dtype=torch.float32, device=dev)
+    dsb = torch.zeros(C3, dtype=torch.float32, device=dev)
+    dfb = torch.zeros(D, dtype=torch.float32, device=dev)
+    dib = torch.zeros(C3, dtype=torch.float32, device=dev) if in_bias is not None else None
+    with torch.cuda.device(dev):
+        for bk, (kspec, c, gs) in zip(plan, saved):
+            B, L = len(bk.seqs), bk.L
+            sbase, rstart = _ptr(seg_base[bk.offset:]), _ptr(row_start[bk.offset:])
+            dkb = torch.empty(D, L, dtype=torch.float32, device=dev)
+            ws = workspace(B, D, L, True, dev)
+            _lib.check(_lib.lib().hyena_b200_core_bwd_packed(
+                _ptr(dy_pre), _ptr(p), _ptr(in_bias), _ptr(sw), _ptr(sb), _ptr(kspec), _ptr(fbias), _ptr(c), _ptr(gs),
+                _ptr(dkb), _ptr(dsw), _ptr(dsb), _ptr(dfb), _ptr(ds), sbase, rstart, T, B, D, L, _ptr(ws),
+                ws.numel(), _stream()))
+            _lib.check(_lib.lib().hyena_b200_short_bwd_packed(
+                _ptr(ds), _ptr(sw), _ptr(dp), _ptr(dib), sbase, rstart, T, B, C3, L, _stream()))
+            n = min(L, Lk)
+            dk[:, :n] += dkb[:, :n]
+    return dp, dk, dsw, dsb, dfb, dib
+
+
+class PackedCoreFn(torch.autograd.Function):
+    """(p, in_bias, short filter, k, filter bias) -> y_pre (1, D, total) on packed sequences (core_forward_packed); its
+    backward loops over the buckets (core_backward_packed).  ``packing``: a validated hyena.Packing."""
+
+    @staticmethod
+    def forward(ctx, p, in_bias, sw, sb, k, fbias, packing):
+        p = p.contiguous()
+        sw2 = sw.reshape(sw.shape[0], -1).contiguous()
+        sb = sb.contiguous(); fbias = fbias.reshape(-1).contiguous(); k = k.contiguous()
+        ib = in_bias.contiguous() if in_bias is not None else None
+        need = any(ctx.needs_input_grad)
+        y, saved = core_forward_packed(p, ib, sw2, sb, k, fbias, packing.plan, packing.tables, need, packing.total)
+        if need:
+            ctx.save_for_backward(p, ib, sw2, sb, fbias)
+            ctx.saved, ctx.packing, ctx.Lk = saved, packing, k.shape[1]
+            ctx.sw_shape, ctx.fb_shape = sw.shape, fbias.shape
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        p, ib, sw2, sb, fbias = ctx.saved_tensors
+        pk = ctx.packing
+        dp, dk, dsw, dsb, dfb, dib = core_backward_packed(dy, p, ib, sw2, sb, fbias, ctx.Lk, pk.plan, pk.tables,
+                                                          ctx.saved, pk.total)
+        ctx.saved = None
+        return dp, dib, dsw.reshape(ctx.sw_shape), dsb, dk, dfb.reshape(ctx.fb_shape), None
+
+
 # ------------------------------------------------------------------------------------------ plain fftconv
 def fftconv_forward(u, kspec, Dvec):
     _need_cuda(u, Dvec)

@@ -151,6 +151,39 @@ HY_API int hyena_b200_core_bwd_rows(const float* dy_pre, const float* p, const f
                                     float* d_in_bias, float* ds_scratch, const int* row_start, int B, int D, int L,
                                     void* workspace, size_t workspace_bytes, void* stream);
 
+/* core_fwd on packed sequences (variable-length batches without padding): one bucket of B sequences that all run at
+ * the row length L.  p (3D, total) and y_pre (D, total) are packed: position t of row b sits at seg_base[b] + t of every
+ * channel (seg_base (B) int64 on the device, may be negative), its real positions are [row_start[b], L) (row_start (B)
+ * int32 on the device).  Positions t < row_start[b] are neither read nor written (they belong to the previous sequence or
+ * lie before the buffer) and act as the short filters' padding, so row b's y_pre is that of the sequence run alone.
+ * c_save (B, D, L) and gspec_save keep the bucket's row layout and are 0 at t < row_start[b] as in core_fwd_rows.
+ * The values are not checked.  Any alignment of the packed sequences: their accesses are scalar.  Pointers 4-byte aligned
+ * (kspec, gspec_save and seg_base 8); the same three launches as core_fwd, counted under its kinds; no allocation, no
+ * synchronisation. */
+HY_API int hyena_b200_core_fwd_packed(const float* p, const float* in_bias, const float* sw, const float* sb,
+                                      const float* kspec, const float* fbias, float* y_pre, float* c_save,
+                                      float* gspec_save, const long long* seg_base, const int* row_start, long long total,
+                                      int B, int D, int L, void* workspace, size_t workspace_bytes, void* stream);
+
+/* backward of core_fwd_packed with the same seg_base / row_start: dy_pre (D, total) packed; c_saved and gspec_saved from
+ * core_fwd_packed.  ds (3D, total) packed receives ds, the gradient w.r.t. the short-filter outputs, at the bucket's real
+ * positions only; dk (D, L) is the sum over the bucket's sequences; (+=) dsw (3D,3), dsb (3D), dfbias (D) over real
+ * positions.  dp follows from hyena_b200_short_bwd_packed.  The same launches as core_bwd with dp == NULL, counted under
+ * its kinds; no allocation, no synchronisation. */
+HY_API int hyena_b200_core_bwd_packed(const float* dy_pre, const float* p, const float* in_bias, const float* sw,
+                                      const float* sb, const float* kspec, const float* fbias, const float* c_saved,
+                                      const float* gspec_saved, float* dk, float* dsw, float* dsb, float* dfbias,
+                                      float* ds, const long long* seg_base, const int* row_start, long long total, int B,
+                                      int D, int L, void* workspace, size_t workspace_bytes, void* stream);
+
+/* transposed short filter of one bucket of packed sequences: dp[t] = w2 ds[t] + w1 ds[t+1] + w0 ds[t+2] for row b's real
+ * positions t in [row_start[b], L), with ds past L and before row_start[b] read as 0; ds and dp (C3, total) packed as in
+ * core_fwd_packed.  (+=) d_in_bias (C3) (may be NULL) sums dp over real positions.  One launch, counted under
+ * short_conv_bwd; no allocation, no synchronisation. */
+HY_API int hyena_b200_short_bwd_packed(const float* ds, const float* sw, float* dp, float* d_in_bias,
+                                       const long long* seg_base, const int* row_start, long long total, int B, int C3,
+                                       int L, void* stream);
+
 /* ---- plain long convolution (the reference extension's own surface) ---------------------------
  * fftconv_fwd replaces csrc/fftconv/fftconv.cpp:53-132 for fp32, gelu=false, no dropout mask, no q/v,
  * head_dim=1:  out[b,h,:] = causal_conv(u[b,h,:], k[h,:]) + u[b,h,:] * Dvec[h]     (fftconv_ref,
