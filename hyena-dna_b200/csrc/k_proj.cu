@@ -129,6 +129,20 @@ cudaError_t launch_proj_gemm(const float* act, int act_layout, const float* W, i
   return cudaErrorInvalidValue;
 }
 
+#ifdef HYENA_B200_PROJ_PHASES
+// Copy (and with `reset`, clear) the per-phase cycle counters of proj_gemm_kernel: n <= kPhaseCtas * kPhases values,
+// row-major [CTA][phase].  Exported by the -DHYENA_B200_PROJ_PHASES build only, for tools/proj_phases.py.
+extern "C" HY_API int hyena_b200_proj_phases(unsigned long long* host, int n, int reset) {
+  const size_t bytes = sizeof(unsigned long long) * (size_t)(n < pg::kPhaseCtas * pg::kPhases ? n : pg::kPhaseCtas * pg::kPhases);
+  if (cudaDeviceSynchronize() != cudaSuccess) return 1;
+  if (host && cudaMemcpyFromSymbol(host, pg::g_proj_phases, bytes) != cudaSuccess) return 1;
+  if (reset) {
+    static unsigned long long zeros[pg::kPhaseCtas][pg::kPhases];
+    if (cudaMemcpyToSymbol(pg::g_proj_phases, zeros, sizeof(zeros)) != cudaSuccess) return 1;
+  }
+  return 0;
+}
+#endif
 
 // weight gradient: dW (M, N) [or (N, M) when transposed_out] = sum_{b,pos} X[b][m][pos] Y[b][pos][n]
 void proj_wgrad_plan(int M, int N, int sms, int* mtiles, int* ntiles, int* splits) {

@@ -6,7 +6,8 @@
 // channel-major (n, pos) (p, dy_pre: what the FFT passes read) or row-major (pos, n) (y, du).  One persistent,
 // warp-specialised kernel (proj_gemm_kernel):
 //
-//   tile      128 positions x 128 outputs, K streamed in chunks of 32; two consumer warpgroups of 64 positions each
+//   tile      128 positions x 128 outputs, K streamed in chunks of 32; two consumer warpgroups of 64 positions each, a
+//             producer warpgroup; setmaxnreg moves registers to the consumers
 //   A operand the activation chunk: global -> shared-memory staging ring by TMA (one tiled copy per chunk, issued by a
 //             producer warp, four chunks in flight) -> registers in the wgmma A-fragment layout -> (hi, lo) tf32 split.
 //             The MMAs read A from registers, so only B goes through the shared-memory port.
@@ -79,7 +80,11 @@ __device__ __forceinline__ float act_grad(float x) {
 namespace pg {
 
 constexpr int kKC = 32;                 // K chunk (one chunk = 4 MMAs of K = 8 per product)
-constexpr int kThreads = 288;           // 9 warps: 0-7 two consumer warpgroups, 8 TMA producer
+constexpr int kThreads = 384;           // warpgroups: 0, 1 consumers; 2 producer (its first warp issues the copies)
+// setmaxnreg: 168 each at launch (the limit for 384 threads); acc 64 + sum 64 + this chunk's A fragments 32 + the next
+// chunk's 16 fragment values per consumer thread
+constexpr int kRegConsumer = 224, kRegProducer = 56;
+static_assert(2 * kRegConsumer + kRegProducer <= 3 * 168, "register file of one CTA");
 constexpr uint32_t kSBO = 1024, kLBO = 128;
 constexpr uint32_t kAPitchCh = 132 * 4; // ACT_CH staging row: 128 positions + one look-ahead quad (fused FIR)
 constexpr uint32_t kAStageBytes = 32 * kAPitchCh;      // 16.5 KB (>= the 16 KB an ACT_ROW tile needs)
@@ -134,6 +139,7 @@ __host__ __device__ constexpr size_t wimg_floats(int N, int K, int NT) {
 }
 
 // ------------------------------------------------------------------------------------------------ the kernel
+
 // Activation staging slot (17 KB, 1024-byte aligned):
 //   ACT_ROW  128 rows x 32 floats (128-byte rows), 16-byte pieces XOR-swizzled by the row (= TMA SWIZZLE_128B): the
 //            A-fragment loads (8 rows x 4 consecutive k per warp) are bank-conflict free
@@ -143,6 +149,24 @@ constexpr uint32_t kSStageBytes = 17408;
 constexpr uint32_t kTapOff = 32 * kAPitchCh;
 static_assert(kSStageBytes >= kTapOff + 32 * 3 * 4 && kSStageBytes >= 128 * 128 && kSStageBytes % 1024 == 0,
               "staging slot");
+
+// Per-phase clock64() counters of proj_gemm_kernel, compiled in only with -DHYENA_B200_PROJ_PHASES (tools/proj_phases.py):
+// every warp adds the cycles it spent in each phase into g_proj_phases[CTA][phase] when it finishes.  Without the flag the
+// macros expand to nothing and the kernel is unchanged.
+enum Phase { PH_FULL = 0, PH_PREP, PH_MMA, PH_SUM, PH_EPI, PH_EMPTY, PH_ISSUE, kPhases = 8 };
+constexpr int kPhaseCtas = 1024;
+#ifdef HYENA_B200_PROJ_PHASES
+__device__ unsigned long long g_proj_phases[kPhaseCtas][kPhases];
+#define PG_PH_BEGIN unsigned long long ph_[kPhases] = {}; long long ph_t_ = clock64();
+#define PG_PH(i) { const long long n_ = clock64(); ph_[i] += (unsigned long long)(n_ - ph_t_); ph_t_ = n_; }
+#define PG_PH_END                                                                                               \
+  if (lane == 0 && blockIdx.x < kPhaseCtas)                                                                      \
+    for (int i_ = 0; i_ < kPhases; ++i_) atomicAdd(&g_proj_phases[blockIdx.x][i_], ph_[i_]);
+#else
+#define PG_PH_BEGIN
+#define PG_PH(i)
+#define PG_PH_END
+#endif
 
 template <int NT> struct Cfg {
   static constexpr int STAGES = 4;                                     // weight stages = staging slots
@@ -154,11 +178,13 @@ template <int NT> struct Cfg {
   static_assert(SMEM <= 227 * 1024, "shared memory budget");
 };
 
-// Warp roles (288 threads):
+// Warp roles (384 threads, three warpgroups):
 //   warps 0-3, 4-7  consumer warpgroups, positions [0, 64) and [64, 128) of the tile: staged activation -> A fragments
-//                   (-> fused FIR) -> (hi, lo) split -> wgmma against the weight stage -> register accumulators -> stores
+//                   (-> fused FIR) -> (hi, lo) split -> wgmma against the weight stage -> register accumulators -> stores;
+//                   the next chunk's fragment values are loaded while this chunk's MMAs run
 //   warp 8          producer: per chunk one TMA bulk copy of the weight images and one tiled TMA copy of the activation
 //                   tile (lane 0); stages the activation by hand when it does not qualify for TMA (all lanes)
+//   warps 9-11      exit after giving their registers back (setmaxnreg)
 // FN != FN_NONE: GELU prologue (ACT_CH -> OUT_ROW) or GELU-gradient epilogue (ACT_ROW -> OUT_CH), see the top of the file
 template <int NT, int ACT, int OUT, int FN = FN_NONE>
 __global__ void __launch_bounds__(kThreads, 1) proj_gemm_kernel(const Args a, const __grid_constant__ CUtensorMap tmap) {
@@ -189,12 +215,15 @@ __global__ void __launch_bounds__(kThreads, 1) proj_gemm_kernel(const Args a, co
     lt = a.l0 + (mt - b * a.mtiles_per_b) * 128;
   };
 
-  if (warp == 8) {
-    // ================================================================== producer
+  if (warp >= 8) {
+    // ================================================================== producer warpgroup: warp 8 issues the copies
+    tc::setmaxnreg_dec<kRegProducer>();
+    if (warp != 8) return;
     // Out-of-range coordinates are zero-filled by the copy engine (end of the tensor: exactly the zero padding the fused
     // FIR needs; K tail).  Activations that do not qualify for TMA (rows not 16-byte aligned) are staged by the 32 lanes
     // with plain loads and stores instead.  With the FIR fused, lane j also stages the taps of the chunk's channel j.
     if (lane == 0 && a.vec) tc::tma_prefetch_desc(&tmap);
+    PG_PH_BEGIN
     uint32_t it = 0;
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
       int b, lt, nt;
@@ -207,7 +236,9 @@ __global__ void __launch_bounds__(kThreads, 1) proj_gemm_kernel(const Args a, co
 #pragma unroll
           for (int j = 0; j < 3; ++j) tap[j] = k0 + lane < a.K ? __ldg(a.fir + 3 * (k0 + lane) + j) : 0.f;
         }
+        PG_PH(PH_ISSUE)
         tc::mbar_wait_u(EMPTY(s), ((it >> 2) & 1u) ^ 1u);
+        PG_PH(PH_EMPTY)
         const float* wsrc = a.wimg + ((size_t)nt * a.kchunks + kc) * (C::STAGE_BYTES / 4);
         const uint32_t st_u = sbase + (uint32_t)C::OFF_A + (uint32_t)s * kSStageBytes;
         unsigned char* st = smem + C::OFF_A + (size_t)s * kSStageBytes;
@@ -232,7 +263,7 @@ __global__ void __launch_bounds__(kThreads, 1) proj_gemm_kernel(const Args a, co
           for (int i = 0; i < 4; ++i) {
             const int r = lane + 32 * i, l = lt + r;
             const float* src = a.act + ((size_t)b * a.L + (l < lend ? l : 0)) * a.K + k0;
-#pragma unroll
+#pragma unroll 2                                                   // 16 loads in flight fit the producer's 56 registers
             for (int c = 0; c < 8; ++c) {
               float4 v;
               v.x = (l < lend && k0 + 4 * c + 0 < a.K) ? __ldg(src + 4 * c + 0) : 0.f;
@@ -256,12 +287,53 @@ __global__ void __launch_bounds__(kThreads, 1) proj_gemm_kernel(const Args a, co
         }
       }
     }
+    PG_PH(PH_ISSUE)
+    PG_PH_END
     return;
   }
 
   // ================================================================== consumers: warpgroup wg = positions [64 wg, 64 wg + 64)
+  tc::setmaxnreg_inc<kRegConsumer>();
   const int wg = warp >> 2, g = lane >> 2, t = lane & 3;
   const int r0 = 64 * wg + 16 * (warp & 3) + g;                  // fragment rows r0, r0 + 8 of the tile
+  // this thread's A-fragment values of the chunk in staging slot s, after the fused FIR / GELU prologue
+  auto load_frags = [&](int s, float (&fx)[4][4]) {
+    const unsigned char* st = smem + C::OFF_A + (size_t)s * kSStageBytes;
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int row = r0 + ((q & 1) ? 8 : 0), k = 8 * ks + t + ((q & 2) ? 4 : 0);
+        float& x = fx[ks][q];
+        if constexpr (ACT == ACT_ROW) {
+          x = *reinterpret_cast<const float*>(st + row * 128 + (((k >> 2) ^ (row & 7)) << 4) + (k & 3) * 4);
+        } else {
+          const float* sp = reinterpret_cast<const float*>(st + k * kAPitchCh) + row;
+          if constexpr (FN != FN_NONE) {
+            x = act_fn<FN>(sp[0]);       // zero-filled staging (tails of K and L) stays zero: gelu(0) = 0
+          } else if (!use_fir) {
+            x = sp[0];
+          } else {
+            // dp[t] = w2 ds[t] + w1 ds[t+1] + w0 ds[t+2]; ds beyond the tensor end is staged as zero, a position
+            // beyond the processed range produces a value nobody stores; channels >= K are staged as zero, taps too
+            const float* w = reinterpret_cast<const float*>(st + kTapOff) + 3 * k;
+            x = fmaf(w[2], sp[0], fmaf(w[1], sp[1], w[0] * sp[2]));
+          }
+        }
+      }
+    }
+  };
+  // The CTA's chunks run as one sequence across its tiles, so that the fragment values of the next chunk (possibly the
+  // first chunk of the next tile) are loaded while this chunk's MMAs run.  A slot is released after the MMAs that
+  // read its weights have completed; its activation values were loaded before they were issued.
+  const int my_tiles = blockIdx.x < ntiles ? (ntiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
+  const uint32_t nchunks = (uint32_t)my_tiles * (uint32_t)a.kchunks;
+  PG_PH_BEGIN
+  float nx[4][4];
+  if (nchunks > 0) {
+    tc::mbar_wait_u(FULL(0), 0u);
+    load_frags(0, nx);
+  }
   uint32_t it = 0;
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     int b, lt, nt;
@@ -269,35 +341,16 @@ __global__ void __launch_bounds__(kThreads, 1) proj_gemm_kernel(const Args a, co
     float sum[64], acc[64];
     for (int kc = 0; kc < a.kchunks; ++kc, ++it) {
       const int s = (int)(it & 3u);
-      tc::mbar_wait_u(FULL(s), (it >> 2) & 1u);                    // weights and activation of this chunk have landed
-      const unsigned char* st = smem + C::OFF_A + (size_t)s * kSStageBytes;
       uint32_t ahi[4][4], alo[4][4];
 #pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
+      for (int ks = 0; ks < 4; ++ks)
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
-          const int row = r0 + ((q & 1) ? 8 : 0), k = 8 * ks + t + ((q & 2) ? 4 : 0);
-          float x;
-          if constexpr (ACT == ACT_ROW) {
-            x = *reinterpret_cast<const float*>(st + row * 128 + (((k >> 2) ^ (row & 7)) << 4) + (k & 3) * 4);
-          } else {
-            const float* sp = reinterpret_cast<const float*>(st + k * kAPitchCh) + row;
-            if constexpr (FN != FN_NONE) {
-              x = act_fn<FN>(sp[0]);       // zero-filled staging (tails of K and L) stays zero: gelu(0) = 0
-            } else if (!use_fir) {
-              x = sp[0];
-            } else {
-              // dp[t] = w2 ds[t] + w1 ds[t+1] + w0 ds[t+2]; ds beyond the tensor end is staged as zero, a position
-              // beyond the processed range produces a value nobody stores; channels >= K are staged as zero, taps too
-              const float* w = reinterpret_cast<const float*>(st + kTapOff) + 3 * k;
-              x = fmaf(w[2], sp[0], fmaf(w[1], sp[1], w[0] * sp[2]));
-            }
-          }
           float hh, lw;
-          tc::split_tf32(x, hh, lw);
+          tc::split_tf32(nx[ks][q], hh, lw);
           ahi[ks][q] = __float_as_uint(hh); alo[ks][q] = __float_as_uint(lw);
         }
-      }
+      PG_PH(PH_SUM)
       // a fresh accumulation per chunk: the correction products (lo*hi, hi*lo; 2^-11 of the result) first, the four
       // hi*hi products last, so that only those add at full scale; chunks are summed with round-to-nearest adds
       const uint32_t bhi = sbase + s * C::STAGE_BYTES, blo = bhi + C::STAGE_BYTES / 2;
@@ -312,8 +365,19 @@ __global__ void __launch_bounds__(kThreads, 1) proj_gemm_kernel(const Args a, co
       for (int ks = 0; ks < 4; ++ks)
         tc::wgmma_rs_n128(acc, ahi[ks], tc::make_desc_ls(bhi + ks * 2 * kLBO, kLBO, kSBO), 1u);
       tc::wgmma_commit();
+      PG_PH(PH_MMA)
+      if (it + 1 < nchunks) {                                        // the next chunk's fragment values, under the MMAs
+        const uint32_t n1 = it + 1;
+        tc::mbar_wait_u(FULL((int)(n1 & 3u)), (n1 >> 2) & 1u);
+        PG_PH(PH_FULL)
+        load_frags((int)(n1 & 3u), nx);
+        PG_PH(PH_PREP)
+      }
       tc::wgmma_wait<0>();
       tc::fence_regs(acc);
+      tc::fence_frags(ahi);                                          // read by the MMAs up to here
+      tc::fence_frags(alo);
+      PG_PH(PH_MMA)
       __syncwarp();
       if (lane == 0) tc::mbar_arrive(EMPTY(s));                    // weight stage and staging slot are free
       if (kc == 0) {
@@ -324,6 +388,7 @@ __global__ void __launch_bounds__(kThreads, 1) proj_gemm_kernel(const Args a, co
         for (int i = 0; i < 64; ++i) sum[i] += acc[i];
       }
     }
+    PG_PH(PH_SUM)
     // epilogue: element i of the fragment = (row r0 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 t + (i & 1))
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -367,7 +432,9 @@ __global__ void __launch_bounds__(kThreads, 1) proj_gemm_kernel(const Args a, co
         }
       }
     }
+    PG_PH(PH_EPI)
   }
+  PG_PH_END
 }
 
 }  // namespace pg
