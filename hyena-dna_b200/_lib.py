@@ -66,6 +66,7 @@ SIGNATURES = {
     "hyena_b200_decode_hist": (_i, [c_fp] * 6 + [_i] * 6 + [_vp]),
     "hyena_b200_decode_hist_rows": (_i, [c_fp] * 7 + [_i] * 6 + [_vp]),
     "hyena_b200_decode_admit": (_i, [c_fp] * 8 + [_i] * 7 + [_vp]),
+    "hyena_b200_decode_admit_packed": (_i, [c_fp] * 9 + [ctypes.c_longlong] + [_i] * 7 + [_vp]),
     "hyena_b200_decode_shift": (_i, [c_fp] + [_i] * 6 + [_vp]),
     "hyena_b200_decode_step": (_i, [c_fp] * 12 + [_i] * 7 + [_vp]),
     "hyena_b200_decode_win_step": (_i, [c_fp] * 13 + [_i] * 10 + [_vp]),

@@ -91,14 +91,23 @@ class Block(nn.Module):
             raise HyenaB200Error(f"Block: the mixer {type(self.mixer).__name__} takes no cu_seqlens")
         return self.mixer.check_packed(hidden_states, cu_seqlens, max_seqlen, cache, lengths, mask)
 
+    def _check_packed_decode(self, hidden_states, cache, cu_seqlens, max_seqlen=None, lengths=None, rows=None):
+        if not hasattr(self.mixer, "check_packed_decode"):
+            raise HyenaB200Error(f"Block: the mixer {type(self.mixer).__name__} takes no packed prompts")
+        return self.mixer.check_packed_decode(hidden_states, cache, cu_seqlens, max_seqlen, lengths, rows)
+
     def _check_mask(self, hidden_states, mask, cache=None, lengths=None):
         if not hasattr(self.mixer, "check_mask"):
             raise HyenaB200Error(f"Block: the mixer {type(self.mixer).__name__} takes no mask")
         return self.mixer.check_mask(hidden_states, mask, cache, lengths)
 
-    def prefill(self, hidden_states, residual, cache, lengths=None):
+    def prefill(self, hidden_states, residual, cache, lengths=None, cu_seqlens=None, max_seqlen=None):
         """forward over the first positions, filling the mixer's DecodeCache (HyenaOperator.prefill); ``lengths``:
-        left-padded prompts of different lengths."""
+        left-padded prompts of different lengths; ``cu_seqlens`` / ``max_seqlen``: prompts packed back to back,
+        hidden_states (total, D) or (1, total, D)."""
+        if cu_seqlens is not None:
+            pk = self._check_packed_decode(hidden_states, cache, cu_seqlens, max_seqlen, lengths)[1]
+            return self._decode(hidden_states, residual, lambda y: self.mixer.prefill(y, cache, cu_seqlens=pk))
         if lengths is not None:
             self._check_lengths(hidden_states, lengths, cache, "prefill")
             return self._decode(hidden_states, residual, lambda y: self.mixer.prefill(y, cache, lengths))
@@ -117,11 +126,14 @@ class Block(nn.Module):
             return self._decode(hidden_states, residual, lambda y: self.mixer.extend(y, cache, lengths))
         return self._decode(hidden_states, residual, lambda y: self.mixer.extend(y, cache))
 
-    def admit(self, hidden_states, residual, cache, rows, lengths=None):
+    def admit(self, hidden_states, residual, cache, rows, lengths=None, cu_seqlens=None):
         """forward of k prompts (k, P, D) that join the running cache in the rows ``rows`` (HyenaOperator.admit); the
-        outputs are those of ``prefill`` on a fresh k-row cache."""
+        outputs are those of ``prefill`` on a fresh k-row cache.  ``cu_seqlens``: the k prompts packed back to back."""
         if not hasattr(self.mixer, "admit"):
             raise HyenaB200Error(f"Block: the mixer {type(self.mixer).__name__} has no incremental decoding")
+        if cu_seqlens is not None:
+            pk = self._check_packed_decode(hidden_states, cache, cu_seqlens, None, lengths, rows)[1]
+            return self._decode(hidden_states, residual, lambda y: self.mixer.admit(y, cache, rows, cu_seqlens=pk))
         self.mixer.check_admit(hidden_states, cache, rows, lengths)
         return self._decode(hidden_states, residual, lambda y: self.mixer.admit(y, cache, rows, lengths))
 
@@ -192,9 +204,17 @@ class Backbone(nn.Module):
         return DecodeCache.stack(layer.mixer.allocate_decode_cache(batch_size, max_seqlen, history_dtype)
                                  for layer in self.layers)
 
-    def prefill(self, hidden_states, cache, lengths=None):
+    def prefill(self, hidden_states, cache, lengths=None, cu_seqlens=None, max_seqlen=None):
         """forward over the first P positions (B, P, D), filling ``cache`` for step(); ``lengths``: left-padded prompts of
-        different lengths (HyenaOperator.prefill)."""
+        different lengths; ``cu_seqlens`` / ``max_seqlen``: B prompts packed back to back, hidden_states (total, D) or
+        (1, total, D), validated once for all layers (HyenaOperator.prefill)."""
+        if cu_seqlens is not None:
+            if hidden_states.requires_grad:
+                raise HyenaB200Error("decoding is inference only: the input requires grad (run under torch.no_grad())")
+            pk = cu_seqlens
+            for layer in self.layers:
+                pk = layer._check_packed_decode(hidden_states, cache, pk, max_seqlen, lengths)[1]
+            return self._packed(hidden_states, lambda layer, h, res: layer.prefill(h, res, cache, cu_seqlens=pk))
         return self._decode(hidden_states, cache, "prefill", lengths)
 
     def step(self, hidden_states, cache):
@@ -205,11 +225,19 @@ class Backbone(nn.Module):
         """The outputs of n more positions (B, n, D); on a fresh cache this is prefill (``lengths`` there only)."""
         return self._decode(hidden_states, cache, "extend", lengths)
 
-    def admit(self, hidden_states, cache, rows, lengths=None):
+    def admit(self, hidden_states, cache, rows, lengths=None, cu_seqlens=None):
         """k prompts (k, P, D) join the running ``cache`` in the rows ``rows`` (HyenaOperator.admit): the outputs of
-        ``prefill`` on a fresh k-row cache.  Every layer is checked, and shifted when P > t, before the first layer admits."""
+        ``prefill`` on a fresh k-row cache.  Every layer is checked, and shifted when P > t, before the first layer admits.
+        ``cu_seqlens``: the k prompts packed back to back, hidden_states (total, D) or (1, total, D)."""
         if hidden_states.requires_grad:
             raise HyenaB200Error("decoding is inference only: the input requires grad (run under torch.no_grad())")
+        if cu_seqlens is not None:
+            pk = cu_seqlens
+            for layer in self.layers:
+                pk = layer._check_packed_decode(hidden_states, cache, pk, None, lengths, rows)[1]
+            with torch.no_grad():
+                cache._admit_clock(pk.max_len)
+            return self._packed(hidden_states, lambda layer, h, res: layer.admit(h, res, cache, rows, cu_seqlens=pk))
         for layer in self.layers:
             if not hasattr(layer.mixer, "admit"):
                 raise HyenaB200Error(f"Block: the mixer {type(layer.mixer).__name__} has no incremental decoding")
@@ -225,6 +253,15 @@ class Backbone(nn.Module):
     def capture_step(self, cache, batch_size=None, dtype=torch.float32):
         """A decode.StepGraph of ``step`` on ``cache``: every layer and ln_f in one CUDA graph per route."""
         return StepGraph(self, cache, batch_size, dtype)
+
+    def _packed(self, hidden_states, run):
+        """Packed prompts through every layer (``run(layer, hidden_states, residual)``) and ln_f, under no_grad."""
+        with torch.no_grad():
+            residual = None
+            for layer in self.layers:
+                hidden_states, residual = run(layer, hidden_states, residual)
+            y, _ = Block._add_norm(hidden_states, residual, self.ln_f)
+            return y.to(hidden_states.dtype)
 
     def _decode(self, hidden_states, cache, how, lengths=None):
         if hidden_states.requires_grad:

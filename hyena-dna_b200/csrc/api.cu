@@ -843,6 +843,25 @@ static int decode_admit(const float* p, const float* in_bias, const float* sw, c
 }
 
 template <class T>
+static int decode_admit_packed(const float* p, const float* in_bias, const float* sw, const float* sb, T* h, float* tail,
+                               const int* rows, const long long* seg_base, const int* row_start, long long Tp, int k,
+                               int cache_B, int D, int order, int P, int t, int Lcap, void* stream) {
+  if (check_decode_shape(k, k, D, order, Lcap)) return 1;
+  HY_CHECK(k <= cache_B, "%d prompts for a decode cache of %d rows", k, cache_B);
+  HY_CHECK(p && sw && sb && h && tail && rows && seg_base && row_start, "null pointer");
+  HY_CHECK(aligned4(p) && aligned4(sw) && aligned4(sb) && elem_aligned(h) && aligned4(tail) && aligned4(rows) &&
+               aligned4(row_start) && aligned8(seg_base) && (!in_bias || aligned4(in_bias)),
+           "misaligned pointer: p, in_bias, sw, sb, h, tail, rows and row_start must be 4-byte aligned, seg_base 8-byte");
+  HY_CHECK(t >= 0 && t <= Lcap, "position %d outside the decode cache [0, %d]", t, Lcap);
+  HY_CHECK(P >= 1 && P <= t, "a prompt of %d positions cannot end at position %d (it needs 1 <= P <= t)", P, t);
+  HY_CHECK(Tp >= P, "bad packed length %lld: the channel stride must hold the longest prompt (%d)", Tp, P);
+  dec::AdmitPackedArgsT<T> a{{{p, in_bias, sw, sb, h, tail, k, D, (order + 1) * D, P, dec::ld_for(Lcap), (order - 1) * D,
+                               row_start}, rows, t - P, t}, seg_base, Tp};
+  HY_CUDA(launch_decode_admit_packed(a, (cudaStream_t)stream));
+  return 0;
+}
+
+template <class T>
 static int decode_shift(T* h, int B, int D, int order, int t, int shift, int Lcap, void* stream) {
   if (check_decode_shape(B, B, D, order, Lcap)) return 1;
   HY_CHECK(h, "null pointer");
@@ -1165,6 +1184,23 @@ HY_API int hyena_b200_decode_admit_h16(int hist_dtype, const float* p, const flo
   return with_hist_type(hist_dtype, [&](auto tag) { using T = decltype(tag);
     return decode_admit<T>(p, in_bias, sw, sb, static_cast<T*>(h), tail, rows, row_start, k, cache_B, D, order, P, t,
                            Lcap, stream);
+  });
+}
+
+HY_API int hyena_b200_decode_admit_packed(const float* p, const float* in_bias, const float* sw, const float* sb,
+                                          float* h, float* tail, const int* rows, const long long* seg_base,
+                                          const int* row_start, long long Tp, int k, int cache_B, int D, int order, int P,
+                                          int t, int Lcap, void* stream) {
+  return decode_admit_packed<float>(p, in_bias, sw, sb, h, tail, rows, seg_base, row_start, Tp, k, cache_B, D, order, P, t,
+                                    Lcap, stream);
+}
+HY_API int hyena_b200_decode_admit_packed_h16(int hist_dtype, const float* p, const float* in_bias, const float* sw,
+                                              const float* sb, void* h, float* tail, const int* rows,
+                                              const long long* seg_base, const int* row_start, long long Tp, int k,
+                                              int cache_B, int D, int order, int P, int t, int Lcap, void* stream) {
+  return with_hist_type(hist_dtype, [&](auto tag) { using T = decltype(tag);
+    return decode_admit_packed<T>(p, in_bias, sw, sb, static_cast<T*>(h), tail, rows, seg_base, row_start, Tp, k, cache_B,
+                                  D, order, P, t, Lcap, stream);
   });
 }
 

@@ -5,6 +5,7 @@
 // so a step is one dot product per (b, channel) over the stored history g[0..t) plus O(1) work at position t.
 //   decode_hist_kernel     after a prefill of P positions: g[0..P) of recurrence 0 and the short-filter tail
 //   decode_admit_kernel    the same for prompts placed into chosen rows of a running cache so that they end at its position
+//                          (PACKED: prompts packed back to back, cu_seqlens; also a packed prefill at t = P into rows 0..N-1)
 //   decode_shift_kernel    in-place shift of every history row by a multiple of 4 positions (compaction, room for a prompt)
 //   decode_dot_kernel      split over positions: one warp per (1024-position chunk, channel), each k row read once for
 //                          all batch rows of its group; the filter is stored time-reversed so that h and k both stream in
@@ -80,9 +81,13 @@ __global__ void __launch_bounds__(256) decode_hist_rows_kernel(const HistArgsT<T
 // first real position, 0 without row_start) in the same pass, so no separate memset runs.  A row whose history is zero
 // before its first real position decodes like the unpadded prompt (time invariance, DESIGN.md section 4.15).  The tail of
 // all C channels of row rows[i] is the prompt's last two positions, a pad position there 0.
+// PACKED: the prompts are packed back to back in p (1, C, T); position j of prompt i is read at p[c T + seg_base[i] + j]
+// (64-bit), and only at j >= s = row_start[i] = P - n_i, so nothing before a prompt is read.  Otherwise wp.seg_base and
+// wp.cstride are unused and the kernel is the plain admission (AdmitArgs in wp.adm).
 // Grid: (k * D rows, up to 64 position CTAs per row); the rows go on x, which has no 65535 limit.
-template <class T>
-__global__ void __launch_bounds__(256) decode_admit_kernel(const AdmitArgsT<T> w) {
+template <bool PACKED, class T>
+__global__ void __launch_bounds__(256) decode_admit_kernel(const AdmitPackedArgsT<T> wp) {
+  const AdmitArgsT<T>& w = wp.adm;
   const HistArgsT<T>& a = w.hist;
   const int row = blockIdx.x;                    // i * D + d
   const int i = row / a.D, d = row - i * a.D;
@@ -90,8 +95,9 @@ __global__ void __launch_bounds__(256) decode_admit_kernel(const AdmitArgsT<T> w
   const int s0 = w.off + s;                      // first real position in cache positions
   const int r = __ldg(w.rows + i);
   const int cv = a.C - a.D + d, cg = a.gate + d;
-  const float* pv = a.p + ((size_t)i * a.C + cv) * a.P;
-  const float* pg = a.p + ((size_t)i * a.C + cg) * a.P;
+  const long long sbase = PACKED ? __ldg(wp.seg_base + i) : 0;
+  const float* pv = PACKED ? a.p + (cv * wp.cstride + sbase) : a.p + ((size_t)i * a.C + cv) * a.P;
+  const float* pg = PACKED ? a.p + (cg * wp.cstride + sbase) : a.p + ((size_t)i * a.C + cg) * a.P;
   const float ibv = a.in_bias ? __ldg(a.in_bias + cv) : 0.f, ibg = a.in_bias ? __ldg(a.in_bias + cg) : 0.f;
   const float v0 = __ldg(a.sw + 3 * cv), v1 = __ldg(a.sw + 3 * cv + 1), v2 = __ldg(a.sw + 3 * cv + 2), vb = __ldg(a.sb + cv);
   const float g0 = __ldg(a.sw + 3 * cg), g1 = __ldg(a.sw + 3 * cg + 1), g2 = __ldg(a.sw + 3 * cg + 2), gb = __ldg(a.sb + cg);
@@ -107,7 +113,7 @@ __global__ void __launch_bounds__(256) decode_admit_kernel(const AdmitArgsT<T> w
   const int nj = a.C / a.D;
   if (blockIdx.y == 0 && (int)threadIdx.x < nj) {
     const int c = threadIdx.x * a.D + d;
-    const float* pc = a.p + ((size_t)i * a.C + c) * a.P;
+    const float* pc = PACKED ? a.p + (c * wp.cstride + sbase) : a.p + ((size_t)i * a.C + c) * a.P;
     const float ib = a.in_bias ? __ldg(a.in_bias + c) : 0.f;
     float* tl = a.tail + ((size_t)r * a.C + c) * 2;
     tl[0] = a.P - 2 >= s ? pc[a.P - 2] + ib : 0.f;

@@ -55,6 +55,16 @@ struct AdmitArgsT {
 };
 using AdmitArgs = AdmitArgsT<float>;
 
+// Admission of N packed prompts (decode_admit_kernel<true>; decode_admit_kernel<false> takes the plain AdmitArgs in adm): adm as above with adm.hist.P = the longest prompt and
+// adm.hist.row_start[i] = P - n_i; adm.hist.p is (1, C, T) packed, and position j of prompt i is read at
+// p[c T + seg_base[i] + j] with seg_base[i] = cu[i+1] - P (may be negative).  Positions j < row_start[i] are never read.
+template <class T>
+struct AdmitPackedArgsT {
+  AdmitArgsT<T> adm;
+  const long long* seg_base;  // (N) int64
+  long long cstride;          // channel stride T of p (the packed length rounded up to a multiple of 4)
+};
+
 // In-place shift of every history row (rows of ld floats) by `shift` positions (a multiple of 4; < 0 left, > 0 right) over
 // the positions [0, round4(t)) (decode_shift_kernel)
 template <class T>

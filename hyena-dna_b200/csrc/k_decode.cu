@@ -21,7 +21,18 @@ cudaError_t launch_decode_admit(const dec::AdmitArgsT<T>& a, cudaStream_t s) {
   const int per_row = (a.t + 255) / 256;
   dim3 grid(a.hist.B * a.hist.D, per_row < 64 ? per_row : 64);
   prof_begin(K_DECODE_HIST, s);
-  dec::decode_admit_kernel<T><<<grid, 256, 0, s>>>(a);
+  dec::decode_admit_kernel<false, T><<<grid, 256, 0, s>>>(dec::AdmitPackedArgsT<T>{a, nullptr, 0});
+  prof_end(K_DECODE_HIST, s);
+  return cudaGetLastError();
+}
+
+// packed prompts (cu_seqlens): the same kernel in its packed mode, with the same grid and kind
+template <class T>
+cudaError_t launch_decode_admit_packed(const dec::AdmitPackedArgsT<T>& a, cudaStream_t s) {
+  const int per_row = (a.adm.t + 255) / 256;
+  dim3 grid(a.adm.hist.B * a.adm.hist.D, per_row < 64 ? per_row : 64);
+  prof_begin(K_DECODE_HIST, s);
+  dec::decode_admit_kernel<true, T><<<grid, 256, 0, s>>>(a);
   prof_end(K_DECODE_HIST, s);
   return cudaGetLastError();
 }
@@ -166,6 +177,7 @@ cudaError_t launch_decode_pos_advance(int* pos, cudaStream_t s) {
 #define HY_DECODE_INSTANTIATE(T)                                                                                          \
   template cudaError_t launch_decode_hist<T>(const dec::HistArgsT<T>&, cudaStream_t);                                     \
   template cudaError_t launch_decode_admit<T>(const dec::AdmitArgsT<T>&, cudaStream_t);                                   \
+  template cudaError_t launch_decode_admit_packed<T>(const dec::AdmitPackedArgsT<T>&, cudaStream_t);                      \
   template cudaError_t launch_decode_shift<T>(const dec::ShiftArgsT<T>&, long long, cudaStream_t);                        \
   template cudaError_t launch_decode_step<T>(const dec::DotArgsT<T>&, const dec::StepArgsT<T>&, cudaStream_t);            \
   template cudaError_t launch_decode_win_step<T>(const dec::DotArgsT<T>&, const dec::WinStepArgsT<T>&, cudaStream_t);     \

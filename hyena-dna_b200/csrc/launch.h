@@ -64,6 +64,7 @@ cudaError_t launch_add_ln_bwd(ln::BwdArgs a, float* dw, float* db, cudaStream_t 
 // k_decode.cu: incremental decoding (decode.cuh)
 template <class T> cudaError_t launch_decode_hist(const dec::HistArgsT<T>& a, cudaStream_t s);
 template <class T> cudaError_t launch_decode_admit(const dec::AdmitArgsT<T>& a, cudaStream_t s);
+template <class T> cudaError_t launch_decode_admit_packed(const dec::AdmitPackedArgsT<T>& a, cudaStream_t s);
 template <class T> cudaError_t launch_decode_shift(const dec::ShiftArgsT<T>& a, long long rows, cudaStream_t s);
 template <class T>
 cudaError_t launch_decode_step(const dec::DotArgsT<T>& dot, const dec::StepArgsT<T>& st, cudaStream_t s);

@@ -510,8 +510,12 @@ class HyenaOperator(nn.Module):
         if lengths is not None or mask is not None:
             raise HyenaB200Error("cu_seqlens does not combine with lengths or mask: packed sequences have no padding")
         if isinstance(cache, DecodeCache):
-            raise HyenaB200Error("cu_seqlens does not combine with a DecodeCache: prefill packed prompts one by one, or "
-                                 "left-padded with lengths=")
+            raise HyenaB200Error("forward(u, cu_seqlens=...) does not combine with a DecodeCache: packed prompts enter a "
+                                 "cache through prefill(u, cache, cu_seqlens=...) or admit(u, cache, rows, cu_seqlens=...)")
+        return self._packed_on_device(u, self._packed_host(u, cu_seqlens, max_seqlen))
+
+    def _packed_host(self, u, cu_seqlens, max_seqlen):
+        """The host checks of packed input that need no device -> Packing without its plan (or the given Packing)."""
         if self.order != 2:
             raise HyenaB200Error(f"cu_seqlens needs order 2; this operator has order {self.order}")
         if self.filter_fn.bidirectional:
@@ -532,6 +536,9 @@ class HyenaOperator(nn.Module):
             raise HyenaB200Error(f"a packed sequence of {pk.max_len} positions exceeds l_max = {self.l_max}")
         if max_seqlen is not None and int(max_seqlen) < pk.max_len:
             raise HyenaB200Error(f"max_seqlen = {int(max_seqlen)} is shorter than the longest sequence ({pk.max_len})")
+        return pk
+
+    def _packed_on_device(self, u, pk):
         if not u.is_cuda:
             raise HyenaB200Error("HyenaOperator (hyena_b200) runs on CUDA sm_90a only; there is no CPU fallback")
         if pk.plan is None:
@@ -539,9 +546,10 @@ class HyenaOperator(nn.Module):
             pk.tables = ops._bucket_tables(pk.plan, u.device)
         return pk
 
-    def _forward_packed(self, u, pk):
+    def _forward_packed(self, u, pk, return_p=False):
         """forward(u, cu_seqlens=...): in_proj and out_proj as one B = 1 GEMM each over the packed tokens, the fused core
-        per bucket of sequences (ops.PackedCoreFn: hyena_b200_core_fwd_packed / core_bwd_packed / short_bwd_packed)."""
+        per bucket of sequences (ops.PackedCoreFn: hyena_b200_core_fwd_packed / core_bwd_packed / short_bwd_packed).
+        ``return_p``: -> (y, the in_proj output p (1, 3D, T) without its bias), for a packed prefill or admission."""
         if pk.total == 0 or pk.max_len == 0:
             return u * 0
         in_dtype, shape, total = u.dtype, u.shape, pk.total
@@ -556,7 +564,46 @@ class HyenaOperator(nn.Module):
         p = _InProj.apply(u32[None], self.in_proj.weight)                            # (1, 3D, tp)
         y_pre = ops.PackedCoreFn.apply(p, self.in_proj.bias, self.short_filter.weight, self.short_filter.bias, k, fb, pk)
         y = _OutProj.apply(y_pre, self.out_proj.weight, self.out_proj.bias)[0, :total]
-        return y.reshape(shape).to(in_dtype)
+        y = y.reshape(shape).to(in_dtype)
+        return (y, p) if return_p else y
+
+    def check_packed_decode(self, u, cache, cu_seqlens, max_seqlen=None, lengths=None, rows=None):
+        """Every host check of ``prefill(u, cache, cu_seqlens=..., max_seqlen=...)`` (``rows`` None) or of ``admit(u,
+        cache, rows, cu_seqlens=...)`` without device work (Block and Backbone run it before their first kernel) -> (the
+        operator's cache, Packing, the rows as a list)."""
+        if lengths is not None:
+            raise HyenaB200Error("cu_seqlens does not combine with lengths: packed prompts have no padding")
+        what = "prefill" if rows is None else "admit"
+        if not isinstance(cache, DecodeCache):
+            raise HyenaB200Error(f"{what} needs a DecodeCache (allocate_decode_cache), got {type(cache).__name__}")
+        c = cache.for_module(self)
+        if u.requires_grad:
+            raise HyenaB200Error("decoding is inference only: the input requires grad (run under torch.no_grad())")
+        pk = self._packed_host(u, cu_seqlens, max_seqlen)
+        n = [pk.cu[i + 1] - pk.cu[i] for i in range(len(pk.cu) - 1)]
+        if 0 in n:
+            raise HyenaB200Error(f"{what}: packed prompt {n.index(0)} is empty; every prompt needs at least one position")
+        P = pk.max_len
+        if c.branched:
+            raise HyenaB200Error(f"{what}: this cache is branched (DecodeCache.fork); packed prompts need a full cache")
+        if rows is None:
+            if c.t != 0:
+                raise HyenaB200Error(f"prefill needs a fresh cache; this one is at position {c.t}")
+            if len(n) != c.batch_size:
+                raise HyenaB200Error(f"prefill: {len(n)} packed prompts for a decode cache of {c.batch_size} rows")
+            if P > c.lcap:
+                raise HyenaB200Error(f"prefill: a prompt of {P} positions exceeds Lcap = {c.lcap}")
+        else:
+            rows = _host_index(rows, c.batch_size, "admit: rows")
+            if len(set(rows)) != len(rows):
+                raise HyenaB200Error(f"admit: rows {rows} repeat a row")
+            if len(rows) != len(n):
+                raise HyenaB200Error(f"admit: {len(rows)} rows for {len(n)} packed prompts")
+            ops.decode_admit_plan(c.t, c.lcap, P, c.win_b, c.win_wc)        # P <= Lcap, and the right shift fits
+        pk = self._packed_on_device(u, pk)
+        if not c.k.is_cuda:
+            raise HyenaB200Error("decoding runs on CUDA sm_90a only; there is no CPU fallback")
+        return c, pk, rows
 
     def check_lengths(self, u, lengths, cache=None, how="forward"):
         """Every host check of ``how``(u, [cache,] lengths=lengths) -- "forward", "prefill", "extend" or "step" -- without
@@ -708,7 +755,7 @@ class HyenaOperator(nn.Module):
         return (self.in_proj.bias.detach().contiguous() if self.in_proj.bias is not None else None,
                 self.short_filter.weight.detach().reshape(C, -1).contiguous(), self.short_filter.bias.detach().contiguous())
 
-    def prefill(self, u, cache, lengths=None):
+    def prefill(self, u, cache, lengths=None, cu_seqlens=None, max_seqlen=None):
         """Run the first P positions, u (B, P, D), and fill ``cache`` (which must be fresh) for stepping.  The output is
         the one ``forward(u)`` gives, bit for bit: the same kernels run in the same order.
 
@@ -716,7 +763,15 @@ class HyenaOperator(nn.Module):
         positions [P - lengths[b], P).  Pad positions enter neither the outputs nor the cache: the output at a real position
         and everything decoded after the prefill are those of the unpadded row; the output at a pad position is
         out_proj(0) = out_proj.bias.  Every row ends at position P, so the rows step together; row b can hold at most
-        Lcap - (P - lengths[b]) real positions.  ``forward(u, lengths=...)`` gives the same outputs, bit for bit."""
+        Lcap - (P - lengths[b]) real positions.  ``forward(u, lengths=...)`` gives the same outputs, bit for bit.
+
+        ``cu_seqlens`` ((N+1,) integer cumulative lengths, as for ``forward``; N = the cache's batch size): u (total, D) or
+        (1, total, D) holds N prompts of at least one position packed back to back, prompt i going into row i.  The output
+        has u's shape and the bits of ``forward(u, cu_seqlens=...)``; the cache is left bit for bit as ``prefill`` of the
+        same prompts left-padded to the longest, P, with ``lengths`` leaves it: every row ends at position P (DESIGN.md
+        section 4.19).  ``max_seqlen``, when given, must be at least P."""
+        if cu_seqlens is not None:
+            return self._prefill_packed(u, cache, cu_seqlens, max_seqlen, lengths)
         if lengths is not None:
             return self._prefill_left_padded(u, cache, lengths)
         c = self._decode_checks(u, cache, u.shape[1] if u.dim() == 3 else -1, fresh=True)
@@ -781,7 +836,7 @@ class HyenaOperator(nn.Module):
             raise HyenaB200Error("decoding runs on CUDA sm_90a only; there is no CPU fallback")
         return c, rows, starts
 
-    def admit(self, u, cache, rows, lengths=None):
+    def admit(self, u, cache, rows, lengths=None, cu_seqlens=None):
         """Prompts join a running cache: u (k, P, D) goes into the cache rows ``rows`` (k distinct rows, typically ones
         freed by ``DecodeCache.release``) -> y (k, P, D), the bits ``prefill`` of u gives on a fresh k-row cache.  Each
         prompt is placed so that it ends at the cache's position t, with a zero history before it, so its row decodes
@@ -790,7 +845,13 @@ class HyenaOperator(nn.Module):
         that takes no prompt is free).  ``lengths`` (k integers in [1, P]): the prompts are left-padded, as for prefill.
         The other rows' history, tail and window are not touched; an open window stays open (the admitted rows' part of
         it is recomputed).  Every row can hold up to Lcap - (t - m) more positions after a ``compact`` by m: the room is
-        bounded by the longest live row, not by the row's own length."""
+        bounded by the longest live row, not by the row's own length.
+
+        ``cu_seqlens``: the k prompts packed back to back, as for ``prefill``; P is the longest.  The output has u's shape
+        and the bits of ``forward(u, cu_seqlens=...)``; each admitted row is left bit for bit as ``admit`` of the prompts
+        left-padded to P leaves it."""
+        if cu_seqlens is not None:
+            return self._admit_packed(u, cache, rows, cu_seqlens, lengths)
         c, rows, starts = self.check_admit(u, cache, rows, lengths)
         P = u.shape[1]
         with torch.no_grad():
@@ -804,6 +865,33 @@ class HyenaOperator(nn.Module):
             ib, sw, sb = self._decode_params()
             ops.decode_admit(p.contiguous(), ib, sw, sb, gs, c, rows, row_start)
             c._took(rows, [c.t - P + s for s in starts])
+        return y
+
+    def _prefill_packed(self, u, cache, cu_seqlens, max_seqlen, lengths):
+        c, pk, _ = self.check_packed_decode(u, cache, cu_seqlens, max_seqlen, lengths)
+        with torch.no_grad():
+            y, p = self._forward_packed(u, pk, return_p=True)
+            P, cu = pk.max_len, pk.cu
+            c.t = P
+            c.set_start([P - (cu[i + 1] - cu[i]) for i in range(len(cu) - 1)])
+            ib, sw, sb = self._decode_params()
+            seg_base = torch.tensor([x - P for x in cu[1:]], dtype=torch.int64, device=u.device)
+            ops.decode_admit_packed(p, ib, sw, sb, c, list(range(len(cu) - 1)), seg_base, c.start_dev, P)
+            c.reset_window()
+        return y
+
+    def _admit_packed(self, u, cache, rows, cu_seqlens, lengths):
+        c, pk, rows = self.check_packed_decode(u, cache, cu_seqlens, None, lengths, rows)
+        with torch.no_grad():
+            y, p = self._forward_packed(u, pk, return_p=True)
+            P, cu = pk.max_len, pk.cu
+            n = [cu[i + 1] - cu[i] for i in range(len(cu) - 1)]
+            c._admit_clock(P)
+            ib, sw, sb = self._decode_params()
+            seg_base = torch.tensor([x - P for x in cu[1:]], dtype=torch.int64, device=u.device)
+            row_start = torch.tensor([P - m for m in n], dtype=torch.int32, device=u.device)
+            ops.decode_admit_packed(p, ib, sw, sb, c, rows, seg_base, row_start, P)
+            c._took(rows, [c.t - m for m in n])
         return y
 
     def _prefill_left_padded(self, u, cache, lengths):

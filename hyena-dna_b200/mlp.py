@@ -9,7 +9,13 @@ With the projections on this library's wgmma kernels (ops.proj_mode() == "tc", t
 node (ops.MlpFn) whose GELU and GELU gradient are fused into the GEMMs; it saves one hidden-sized tensor.  Under the
 library GEMM modes (HYENA_B200_PROJ=lt / torch, or torch.backends.cuda.matmul.allow_tf32) it is the reference's own
 F.linear + F.gelu composition, exactly as the projections of HyenaOperator follow that switch.  There is no CPU path.
+
+When no gradient is needed, a row count L > 4 that is not a multiple of 4 (a packed batch, whose L is its token count) is
+zero-padded to one: the hidden activation's channel stride is then a multiple of 4 and fc2 reads it on the vector path.
+Each output element sums over the features in the same order whatever L is, so the real rows keep their bits.  Training
+keeps L as it is: the weight-gradient sums over L would change order.
 """
+import torch
 import functools
 
 import torch.nn as nn
@@ -52,8 +58,17 @@ class Mlp(nn.Module):
         if ops.proj_mode() == "tc":
             shape = x.shape
             x3 = x.reshape(-1, shape[-2], shape[-1]) if x.dim() >= 2 else x.reshape(1, 1, -1)
+            L = x3.shape[1]
+            pad = (-L) % 4 if L > 4 and not self._needs_grad(x) else 0
+            if pad:
+                x3 = F.pad(x3, (0, 0, 0, pad))
             y = ops.MlpFn.apply(x3, self.fc1.weight, self.fc1.bias, self.fc2.weight, self.fc2.bias, self.approximate)
+            if pad:
+                y = y[:, :L]
             y = y.reshape(*shape[:-1], y.shape[-1])
         else:
             y = self.fc2(self.activation(self.fc1(x)))
         return y if not self.return_residual else (y, x)
+
+    def _needs_grad(self, x):
+        return torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters()))

@@ -1298,6 +1298,12 @@ def decode_admit(p, in_bias, sw, sb, gs, cache, rows, row_start=None):
         g = torch.zeros(k, D, t, dtype=cache.h.dtype, device=dev)
         g[:, :, off:] = gs[o]                       # rounded to a 16-bit history here
         cache.h[o, ridx, :, :t] = g
+    _admit_window(cache, ridx, off)
+
+
+def _admit_window(cache, ridx, off):
+    """With a window open, rewrite the F of the admitted rows ``ridx`` (long, on the device), whose history is zero before
+    ``off``: zero when off is at or after the window base, else the convolution of their history [floor4(off), win_b)."""
     if cache.win_wc > 0:
         b, wc = cache.win_b, cache.win_wc
         if off >= b:
@@ -1305,9 +1311,33 @@ def decode_admit(p, in_bias, sw, sb, gs, cache, rows, row_start=None):
         else:
             a = off - off % 4
             ld = cache.h.shape[-1]
-            for o in range(O - 1):
+            for o in range(cache.order - 1):
                 conv = _history_conv(cache, ld, cache.h[o, ridx, :, a:b], o, b - a, b - a + wc)
                 cache.win_f[o, ridx, :, :wc] = conv[:, :, b - a:]
+
+
+def decode_admit_packed(p, in_bias, sw, sb, cache, rows, seg_base, row_start, P):
+    """decode_admit of N prompts packed back to back (order 2): p (1, 3D, T) their packed in_proj output without its bias
+    (channel stride T), P the longest prompt, ``rows`` (N host integers) the destination rows, seg_base ((N,) int64 on the
+    device, cu[i+1] - P) and row_start ((N,) int32 on the device, P - n_i) where prompt i sits.  One decode_admit_packed
+    launch writes each row as decode_admit writes the prompts left-padded to P; the window as decode_admit.  At t = P on
+    rows 0..N-1 of a fresh cache this is the prefill of the packed prompts."""
+    _need_cuda(p, in_bias, sw, sb)
+    _, C, T = p.shape
+    N = len(rows)
+    D, O, t = cache.d_model, cache.order, int(cache.t)
+    if p.shape[0] != 1 or not p.is_contiguous() or C != (O + 1) * D or O != 2:
+        raise _lib.HyenaB200Error(f"decode_admit_packed: p must be contiguous (1, {(O + 1) * D}, T) of an order-2 cache")
+    for x, dt, what in ((seg_base, torch.int64, "seg_base"), (row_start, torch.int32, "row_start")):
+        if x.dtype != dt or x.device != p.device or tuple(x.shape) != (N,) or not x.is_contiguous():
+            raise _lib.HyenaB200Error(f"decode_admit_packed: {what} must be a contiguous ({N},) {dt} tensor on {p.device}")
+    dev = p.device
+    rows_dev = torch.tensor(rows, dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(_decode_fn("admit_packed", cache.h)(
+            _ptr(p), _ptr(in_bias), _ptr(sw), _ptr(sb), _ptr(cache.h), _ptr(cache.tail), _ptr(rows_dev), _ptr(seg_base),
+            _ptr(row_start), T, N, cache.batch_size, D, O, int(P), t, cache.lcap, _stream()))
+    _admit_window(cache, rows_dev.to(torch.long), t - int(P))
 
 
 # ------------------------------------------------------------------------------------------ device-position steps

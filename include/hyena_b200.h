@@ -335,6 +335,18 @@ HY_API int hyena_b200_decode_admit(const float* p, const float* in_bias, const f
                                    float* tail, const int* rows, const int* row_start, int k, int cache_B, int D, int order,
                                    int P, int t, int Lcap, void* stream);
 HY_API int hyena_b200_decode_shift(float* h, int B, int D, int order, int t, int shift, int Lcap, void* stream);
+/*   decode_admit_packed: decode_admit of k prompts packed back to back (cu_seqlens, see core_fwd_packed): p (1, C, T)
+ *                channel-major WITHOUT in_proj.bias, channel stride T >= P (the packed length rounded up to a multiple of
+ *                4); P is the longest prompt.  Prompt i has n_i = P - row_start[i] positions, and its position j (j >=
+ *                row_start[i]) is read at p[c T + seg_base[i] + j] with seg_base (k) int64 on the device, seg_base[i] =
+ *                cu[i+1] - P (may be negative).  Nothing before a prompt is read.  Row rows[i] gets what decode_admit gives
+ *                the same prompts left-padded to P: 0 at [0, t - n_i), g_0 of the prompt's positions to t, and the tail.
+ *                With t = P and rows 0..k-1 of a fresh cache it is the prefill of packed prompts: bit for bit what
+ *                decode_hist_rows writes for the left-padded prompts.  One launch, counted under the kind decode_hist. */
+HY_API int hyena_b200_decode_admit_packed(const float* p, const float* in_bias, const float* sw, const float* sb,
+                                          float* h, float* tail, const int* rows, const long long* seg_base,
+                                          const int* row_start, long long T, int k, int cache_B, int D, int order, int P,
+                                          int t, int Lcap, void* stream);
 HY_API int hyena_b200_decode_step(const float* p_t, const float* in_bias, const float* sw, const float* sb, const float* k,
                                   const float* fbias, float* h, float* tail, float* s_t, const float* v_in, float* out,
                                   float* part, int B, int cache_B, int D, int order, int o, int t, int Lcap, void* stream);
@@ -446,6 +458,10 @@ HY_API int hyena_b200_decode_hist_rows_h16(int hist_dtype, const float* p, const
 HY_API int hyena_b200_decode_admit_h16(int hist_dtype, const float* p, const float* in_bias, const float* sw,
                                        const float* sb, void* h, float* tail, const int* rows, const int* row_start,
                                        int k, int cache_B, int D, int order, int P, int t, int Lcap, void* stream);
+HY_API int hyena_b200_decode_admit_packed_h16(int hist_dtype, const float* p, const float* in_bias, const float* sw,
+                                              const float* sb, void* h, float* tail, const int* rows,
+                                              const long long* seg_base, const int* row_start, long long T, int k,
+                                              int cache_B, int D, int order, int P, int t, int Lcap, void* stream);
 HY_API int hyena_b200_decode_shift_h16(int hist_dtype, void* h, int B, int D, int order, int t, int shift, int Lcap,
                                        void* stream);
 HY_API int hyena_b200_decode_step_h16(int hist_dtype, const float* p_t, const float* in_bias, const float* sw,

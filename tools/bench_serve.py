@@ -46,8 +46,9 @@ def pct(xs, q):
     return xs[min(len(xs) - 1, int(math.ceil(q * len(xs))) - 1)]
 
 
-def continuous(m, trace, B, D, lcap, dev, hd=torch.float32):
-    """(a): -> (seconds, latencies, admit times, compact times, compactions)."""
+def continuous(m, trace, B, D, lcap, dev, hd=torch.float32, packed=False):
+    """(a): -> (seconds, latencies, admit times, compact times, compactions).  ``packed``: each admission's prompts are
+    packed back to back (Backbone.admit with cu_seqlens) instead of left-padded to the longest."""
     cache = m.allocate_decode_cache(B, lcap, history_dtype=hd)
     queue = list(range(len(trace)))
     left, lat, adm, cmp_ = {}, [], [], []
@@ -57,11 +58,18 @@ def continuous(m, trace, B, D, lcap, dev, hd=torch.float32):
         reqs = [queue.pop(0) for _ in rows]
         P = max(trace[i][0] for i in reqs)
         lengths = [trace[i][0] for i in reqs]
-        u = torch.zeros(len(rows), P, D, device=dev)
-        for j, i in enumerate(reqs):
-            u[j, P - lengths[j]:] = 0.5 * torch.randn(lengths[j], D, device=dev)
+        if packed:
+            u = 0.5 * torch.randn(sum(lengths), D, device=dev)
+            cu = torch.tensor([0] + torch.tensor(lengths).cumsum(0).tolist(), dtype=torch.int32)
+        else:
+            u = torch.zeros(len(rows), P, D, device=dev)
+            for j, i in enumerate(reqs):
+                u[j, P - lengths[j]:] = 0.5 * torch.randn(lengths[j], D, device=dev)
         a = now()
-        m.admit(u, cache, rows, lengths)
+        if packed:
+            m.admit(u, cache, rows, cu_seqlens=cu)
+        else:
+            m.admit(u, cache, rows, lengths)
         adm.append(now() - a)
         for r, i in zip(rows, reqs):
             left[r] = [i, trace[i][1]]
