@@ -199,8 +199,11 @@ class Backbone(nn.Module):
         return y.to(hidden_states.dtype)
 
     def allocate_decode_cache(self, batch_size, max_seqlen, history_dtype=torch.float32):
-        """One DecodeCache holding the state of every layer's mixer (decode.py), each history stored as ``history_dtype``."""
+        """One DecodeCache holding the state of every layer's mixer (decode.py), each history stored as ``history_dtype``.
+        ``max_seqlen`` None: unbounded, every layer sliding together (the layers' mixers must share l_max)."""
         check_history_dtype(history_dtype)
+        if max_seqlen is None and len({getattr(layer.mixer, "l_max", None) for layer in self.layers}) > 1:
+            raise HyenaB200Error("DecodeCache.stack: an unbounded stack needs every layer unbounded with the same l_max")
         return DecodeCache.stack(layer.mixer.allocate_decode_cache(batch_size, max_seqlen, history_dtype)
                                  for layer in self.layers)
 
@@ -268,6 +271,15 @@ class Backbone(nn.Module):
             raise HyenaB200Error("decoding is inference only: the input requires grad (run under torch.no_grad())")
         if lengths is not None:
             self.layers[0]._check_lengths(hidden_states, lengths, cache, how)
+        elif isinstance(cache, DecodeCache) and cache.unbounded:
+            # an unbounded stack is checked before any device work, then slides every layer once, before the first layer
+            # runs (each mixer would slide its own cache alike); an extend longer than S runs in pieces inside each mixer,
+            # the first being this one
+            n = hidden_states.shape[1] if hidden_states.dim() == 3 else -1
+            self.layers[0].mixer._decode_checks(hidden_states, cache, n, fresh=how == "prefill")
+            if how != "prefill" and cache.t > 0:
+                with torch.no_grad():
+                    cache._make_room(min(n, cache.slide), step=how == "step")
         with torch.no_grad():
             residual = None
             for layer in self.layers:

@@ -11,6 +11,11 @@ exactly that; ``HyenaOperator.prefill`` / ``step`` fill and use it (csrc/decode.
 The filter is generated once, at allocation, for Lcap = min(max_seqlen, l_max) positions.  That is valid for any shorter
 prefix: k[j] depends on position j only -- z and t are sliced per position, the modulation is per position and the
 ``normalized`` option divides by the L1 norm over channels at each position (hyena.py:235-236).
+
+An *unbounded* cache (max_seqlen=None, DESIGN.md section 4.20) has no position limit.  The filter has l_max taps, so the
+output at t reads no history position s <= t - l_max: before an operation would pass Lcap, the history slides left past
+every position no later output reaches (ops.decode_slide_plan).  Its buffer holds Lcap = unbounded_lcap(l_max) positions
+and its stored filter is the l_max taps with zeros up to the row stride, so every kernel runs on it unchanged.
 """
 import torch
 
@@ -25,6 +30,22 @@ def _ld(lcap):
 
 def _chunks(lcap):
     return (lcap + CHUNK - 1) // CHUNK
+
+
+SLIDE_MAX = 4096      # positions an unbounded cache holds beyond its filter's reach (at most)
+MAX_LCAP = 1 << 20    # longest history a decode cache can hold (csrc/api.cu check_decode_shape)
+
+
+def slide_room(l_max):
+    """S = min(4096, l_max rounded up to a multiple of 4): the positions an unbounded cache of an operator with l_max filter
+    taps has room for after a slide, and the longest piece an extend of it runs at once."""
+    return min(SLIDE_MAX, _ld(int(l_max)))
+
+
+def unbounded_lcap(l_max):
+    """Lcap of an unbounded cache: l_max + S + 3 rounded up to a multiple of 4.  A slide leaves t in [l_max - 1, l_max + 2]
+    (its shift is rounded down to a multiple of 4), so any n <= S more positions fit after it."""
+    return _ld(int(l_max) + slide_room(l_max) + 3)
 
 
 HISTORY_DTYPES = (torch.float32, torch.float16, torch.bfloat16)
@@ -102,6 +123,11 @@ class DecodeCache:
       part  (B, D, ceil(Lcap / 1024))  partial dot products of one step
     ``t`` is the number of positions consumed so far.
 
+    Unbounded cache (``allocate(op, B, None)``, DESIGN.md section 4.20): ``reach`` = l_max, the filter's taps, and Lcap =
+    unbounded_lcap(l_max); k holds the l_max taps and zeros from tap l_max to ld, so k[j] = 0 for every l_max <= j < ld.
+    Every step, extend, StepGraph replay and fork first calls ``_make_room``, which slides every layer left when the next
+    positions would pass Lcap (ops.decode_slide_plan, on decode_shift_kernel).  ``dropped`` counts the positions slid out.
+
     Window state of the windowed step (ops.decode_window_plan, DESIGN.md section 4.11): a window [win_b, win_b + win_wc)
     is valid while win_b <= t < win_b + win_wc; ``win_f`` (O-1, B, D, W) holds F_o[j] = sum_{s < win_b} k_o[win_b+j-s]
     g_o[s] for j < win_wc.  F depends on h[:, :, :, :win_b] only, so an extend inside the window leaves it valid.  It is
@@ -134,9 +160,11 @@ class DecodeCache:
     use and written only by ``sync_position`` and by a replayed StepGraph; ``t`` on the host stays authoritative."""
 
     def __init__(self, owner=None, batch_size=0, max_seqlen=0, lcap=0, k=None, bias=None, h=None, tail=None, s_t=None,
-                 part=None, layers=None):
+                 part=None, layers=None, reach=None):
         self.owner = owner
-        self.batch_size, self.max_seqlen, self.lcap = int(batch_size), int(max_seqlen), int(lcap)
+        self.batch_size, self.lcap = int(batch_size), int(lcap)
+        self.max_seqlen = None if max_seqlen is None else int(max_seqlen)
+        self.reach, self._dropped = (None if reach is None else int(reach)), 0
         self.k, self.bias, self.h, self.tail, self.s_t, self.part = k, bias, h, tail, s_t, part
         self.layers = list(layers) if layers is not None else []
         self._t = 0
@@ -151,38 +179,57 @@ class DecodeCache:
     @classmethod
     def allocate(cls, op, batch_size, max_seqlen, history_dtype=torch.float32):
         """Decoding state of ``op`` for ``batch_size`` rows and up to min(max_seqlen, op.l_max) positions, with the history
-        stored as ``history_dtype`` (torch.float32, torch.float16 or torch.bfloat16)."""
+        stored as ``history_dtype`` (torch.float32, torch.float16 or torch.bfloat16).  ``max_seqlen`` None: an unbounded
+        cache, which slides past the filter's l_max taps instead of stopping at Lcap (DESIGN.md section 4.20)."""
         check_history_dtype(history_dtype)
         if op.filter_fn.bidirectional:
             raise HyenaB200Error("decoding needs a causal filter; this HyenaFilter is bidirectional")
-        if batch_size < 1 or max_seqlen < 1:
-            raise HyenaB200Error(f"allocate_decode_cache: batch_size {batch_size} and max_seqlen {max_seqlen} must be >= 1")
+        lk = cls.check_allocation(batch_size, max_seqlen, op.l_max)
         w = op.in_proj.weight
         if not w.is_cuda:
             raise HyenaB200Error("decoding runs on CUDA sm_90a only; the operator's parameters are on the CPU")
         B, D, O = int(batch_size), op.d_model, op.order
-        lcap = min(int(max_seqlen), op.l_max)
+        lcap = unbounded_lcap(lk) if lk is not None else min(int(max_seqlen), op.l_max)
+        taps = min(lcap, op.l_max)
         ld = _ld(lcap)
         F = (O - 1) * D
         dev = w.device
         with torch.no_grad():
-            k = op.filter_fn.filter_channel_major(lcap)                  # (F, lcap)
+            k = op.filter_fn.filter_channel_major(taps)                  # (F, taps); zero taps from l_max on
             krev = torch.zeros(F * ld + 4, dtype=torch.float32, device=dev)
-            krev[:F * ld].view(F, ld)[:, ld - lcap:] = k.flip(-1)
+            krev[:F * ld].view(F, ld)[:, ld - taps:] = k.flip(-1)
             fb = op.filter_fn.bias if op.filter_fn.use_bias else 0 * op.filter_fn.bias
             fb = fb.detach().reshape(-1).to(torch.float32).contiguous().clone()
         h = torch.zeros(O - 1, B, D, ld, dtype=history_dtype, device=dev)
         tail = torch.zeros(B, (O + 1) * D, 2, dtype=torch.float32, device=dev)
         s_t = torch.zeros(B, (O + 1) * D, dtype=torch.float32, device=dev)
         part = torch.zeros(B, D, _chunks(lcap), dtype=torch.float32, device=dev)
-        return cls(op, B, max_seqlen, lcap, krev, fb, h, tail, s_t, part)
+        return cls(op, B, max_seqlen, lcap, krev, fb, h, tail, s_t, part, reach=lk)
+
+    @staticmethod
+    def check_allocation(batch_size, max_seqlen, l_max):
+        """Host checks of an allocation -> the filter reach l_max of an unbounded cache (``max_seqlen`` None), else None."""
+        if max_seqlen is None:
+            if batch_size < 1:
+                raise HyenaB200Error(f"allocate_decode_cache: batch_size {batch_size} must be >= 1")
+            if unbounded_lcap(l_max) > MAX_LCAP:
+                raise HyenaB200Error(f"allocate_decode_cache: an unbounded cache holds l_max + S + 3 = "
+                                     f"{unbounded_lcap(l_max)} positions (l_max = {l_max}), more than the {MAX_LCAP} a "
+                                     "decode cache can hold; give max_seqlen")
+            return int(l_max)
+        if batch_size < 1 or max_seqlen < 1:
+            raise HyenaB200Error(f"allocate_decode_cache: batch_size {batch_size} and max_seqlen {max_seqlen} must be >= 1")
+        return None
 
     @classmethod
     def stack(cls, caches):
-        """One cache for several operators (one per layer of a stack), each found by ``for_module``."""
+        """One cache for several operators (one per layer of a stack), each found by ``for_module``.  The layers of an
+        unbounded stack share one filter reach, so that they slide together."""
         caches = list(caches)
         if not caches:
             raise HyenaB200Error("DecodeCache.stack needs at least one operator cache")
+        if len({c.reach for c in caches}) > 1:
+            raise HyenaB200Error("DecodeCache.stack: an unbounded stack needs every layer unbounded with the same l_max")
         return cls(None, caches[0].batch_size, caches[0].max_seqlen, min(c.lcap for c in caches), layers=caches)
 
     @staticmethod
@@ -192,6 +239,40 @@ class DecodeCache:
         B, D, O = batch_size, d_model, order
         ld, F, C = _ld(lcap), (order - 1) * d_model, (order + 1) * d_model
         return 4 * ((F * ld + 4) + F + B * C * 2 + B * C + B * D * _chunks(lcap)) + e * (O - 1) * B * D * ld
+
+    @property
+    def unbounded(self):
+        """True for a cache allocated with max_seqlen=None: it slides instead of stopping at Lcap (a branch never is)."""
+        return self.layers[0].unbounded if self.layers else self.reach is not None
+
+    @property
+    def dropped(self):
+        """Positions slid out of an unbounded cache so far, summed over its slides (0 for any other cache): position t of
+        the cache is position dropped + t of the sequence, as long as no ``compact`` or right-shifting ``admit`` moved t."""
+        return self.layers[0].dropped if self.layers else self._dropped
+
+    @property
+    def slide(self):
+        """S (``slide_room``) of an unbounded cache, None for any other: the longest piece an extend of it runs at once."""
+        if not self.unbounded:
+            return None
+        return slide_room(self.layers[0].reach if self.layers else self.reach)
+
+    def _make_room(self, n, step=False):
+        """Before n more positions of an unbounded cache (``step``: one step, which may open a window): when
+        ops.decode_slide_plan asks for it, slide every layer left by m (decode_shift_kernel, one launch per layer) and add m
+        to ``dropped``; returns m (0: no slide, or a bounded cache, whose room the callers check)."""
+        if not self.unbounded:
+            return 0
+        from . import ops
+        c0 = self.layers[0] if self.layers else self
+        shift, _, keep = ops.decode_slide_plan(self.t, n, c0.reach, c0.lcap, *self._window(), step=step)
+        if shift == 0:
+            return 0
+        for c in (self.layers or [self]):
+            c._reposition(shift, keep)
+            c._dropped -= shift
+        return -shift
 
     @property
     def history_dtype(self):
@@ -217,13 +298,17 @@ class DecodeCache:
         """A branched cache of len(rows) rows: row i continues row ``rows[i]`` of this cache from its current position t0
         (repeat a row for several branches of one context) and can be stepped and extended up to horizon positions past
         its base t0 - t0 mod 4, or to Lcap.  A snapshot: this cache can go on decoding without changing the branches.  A
-        stack's cache forks every layer."""
+        stack's cache forks every layer.  An unbounded cache first slides in place when the branches would otherwise get
+        fewer than min(horizon, S) positions (DecodeCache._make_room): its outputs do not change, but its t, ``dropped``
+        and window move as after any slide."""
         if self.branched:
             raise HyenaB200Error("fork: this cache is branched already; use select() to reorder, repeat or drop branches")
         rows = _host_index(rows, self.batch_size, "fork: rows")
         horizon = int(horizon)
         if horizon < 1:
             raise HyenaB200Error(f"fork: horizon {horizon} must be >= 1")
+        if self.unbounded and self.t >= 1:
+            self._make_room(min(horizon, self.slide))     # an unbounded parent slides first, so the branches get room
         for c in (self.layers or [self]):
             if c.owner.filter_fn.bidirectional:
                 raise HyenaB200Error("decoding needs a causal filter; this HyenaFilter is bidirectional")
@@ -253,8 +338,8 @@ class DecodeCache:
         return 0 if self.win_f is None else self.win_f.numel() * self.win_f.element_size()
 
     def reset_window(self):
-        """Close the window and restart the step count (a prefill starts a new sequence)."""
-        self.win_b, self.win_wc, self.steps = 0, 0, 0
+        """Close the window and restart the step and slide counts (a prefill starts a new sequence)."""
+        self.win_b, self.win_wc, self.steps, self._dropped = 0, 0, 0, 0
 
     @property
     def start(self):
@@ -429,6 +514,7 @@ class StepGraph:
         self.res_dtype = (torch.float32 if module.residual_in_fp32 else dtype) if residual else None
         self._graphs, self._keys, self._side, self._scratch = {}, {}, None, []
         self._check_room()
+        self._slide()
         self._in = torch.zeros(self.shape, dtype=dtype, device=self.device)
         self._res = torch.zeros(self.shape, dtype=self.res_dtype, device=self.device) if residual else None
         self._graph(self.plan()[0])
@@ -449,8 +535,19 @@ class StepGraph:
         if c.branched and c.t >= c.base + c.hc:
             raise HyenaB200Error(f"StepGraph: decoding past the branch horizon: position {c.t} is base + Hc = {c.base} + "
                                  f"{c.hc} (fork with a larger horizon, up to Lcap = {c.lcap})")
-        if c.t >= c.lcap:
+        if not c.unbounded and c.t >= c.lcap:
             raise HyenaB200Error(f"StepGraph: decoding past the cache: position {c.t} is Lcap = {c.lcap}")
+
+    def _slide(self):
+        """An unbounded cache slides eagerly between replays, outside the graphs, once every check has passed
+        (DecodeCache._make_room); step() then syncs the position."""
+        if self.caches[0].unbounded:
+            self.cache._make_room(1, step=True)
+
+    def _check_key(self, route):
+        if route in self._keys and self._key(route) != self._keys[route]:
+            raise HyenaB200Error("StepGraph.step: a buffer of the decode cache was replaced since the capture (reallocated, "
+                                 "re-forked or re-synced elsewhere); capture a new StepGraph")
 
     _READS = {"plain": ("k", "bias", "h", "tail", "s_t", "part", "pos"),
               "window": ("k", "bias", "h", "tail", "s_t", "part", "pos", "win_f"),
@@ -478,10 +575,12 @@ class StepGraph:
         from . import ops
         self._check_input(u_t, residual)
         self._check_room()
+        if self.caches[0].unbounded:
+            for r in self._keys:              # any route may run after the slide: all are checked before it
+                self._check_key(r)
+        self._slide()
         route, refresh = self.plan()
-        if route in self._keys and self._key(route) != self._keys[route]:
-            raise HyenaB200Error("StepGraph.step: a buffer of the decode cache was replaced since the capture (reallocated, "
-                                 "re-forked or re-synced elsewhere); capture a new StepGraph")
+        self._check_key(route)
         if refresh:
             for c in self.caches:
                 ops.decode_window_refresh(c)

@@ -475,20 +475,20 @@ class HyenaOperator(nn.Module):
             return y, None
         return y
 
-    def _padded_checks(self, u, what):
-        """Host validation of a left-padded input's filter and shape -> (B, P)."""
+    def _padded_checks(self, u, what, hint=""):
+        """Host validation of a left-padded input's filter and shape -> (B, P); ``hint`` ends a too-long input's error."""
         if self.filter_fn.bidirectional:
             raise HyenaB200Error(f"{what} needs a causal filter; this HyenaFilter is bidirectional")
         if u.dim() != 3 or u.shape[-1] != self.d_model:
             raise HyenaB200Error(f"left-padded input must be (B, L, {self.d_model}); got {tuple(u.shape)}")
         B, P = u.shape[0], u.shape[1]
         if P > self.l_max:
-            raise HyenaB200Error(f"left-padded input of {P} positions exceeds l_max = {self.l_max}")
+            raise HyenaB200Error(f"left-padded input of {P} positions exceeds l_max = {self.l_max}{hint}")
         return B, P
 
-    def _ragged_checks(self, u, lengths):
+    def _ragged_checks(self, u, lengths, hint=""):
         """Host validation of a left-padded input before any device work -> the rows' first real positions."""
-        B, P = self._padded_checks(u, "lengths")
+        B, P = self._padded_checks(u, "lengths", hint)
         return [P - n for n in host_lengths(lengths, B, P)]
 
     def check_mask(self, u, mask, cache=None, lengths=None):
@@ -514,8 +514,9 @@ class HyenaOperator(nn.Module):
                                  "cache through prefill(u, cache, cu_seqlens=...) or admit(u, cache, rows, cu_seqlens=...)")
         return self._packed_on_device(u, self._packed_host(u, cu_seqlens, max_seqlen))
 
-    def _packed_host(self, u, cu_seqlens, max_seqlen):
-        """The host checks of packed input that need no device -> Packing without its plan (or the given Packing)."""
+    def _packed_host(self, u, cu_seqlens, max_seqlen, hint=""):
+        """The host checks of packed input that need no device -> Packing without its plan (or the given Packing);
+        ``hint`` ends a too-long sequence's error."""
         if self.order != 2:
             raise HyenaB200Error(f"cu_seqlens needs order 2; this operator has order {self.order}")
         if self.filter_fn.bidirectional:
@@ -533,7 +534,7 @@ class HyenaOperator(nn.Module):
             max_len = max(cu[i + 1] - cu[i] for i in range(len(cu) - 1))
             pk = Packing(cu, None, None, max_len, u.device)
         if pk.max_len > self.l_max:
-            raise HyenaB200Error(f"a packed sequence of {pk.max_len} positions exceeds l_max = {self.l_max}")
+            raise HyenaB200Error(f"a packed sequence of {pk.max_len} positions exceeds l_max = {self.l_max}{hint}")
         if max_seqlen is not None and int(max_seqlen) < pk.max_len:
             raise HyenaB200Error(f"max_seqlen = {int(max_seqlen)} is shorter than the longest sequence ({pk.max_len})")
         return pk
@@ -579,7 +580,7 @@ class HyenaOperator(nn.Module):
         c = cache.for_module(self)
         if u.requires_grad:
             raise HyenaB200Error("decoding is inference only: the input requires grad (run under torch.no_grad())")
-        pk = self._packed_host(u, cu_seqlens, max_seqlen)
+        pk = self._packed_host(u, cu_seqlens, max_seqlen, self._prompt_hint(c, what))
         n = [pk.cu[i + 1] - pk.cu[i] for i in range(len(pk.cu) - 1)]
         if 0 in n:
             raise HyenaB200Error(f"{what}: packed prompt {n.index(0)} is empty; every prompt needs at least one position")
@@ -622,7 +623,7 @@ class HyenaOperator(nn.Module):
         c = cache.for_module(self) if isinstance(cache, DecodeCache) else cache
         if how == "extend" and isinstance(c, DecodeCache) and (c.branched or c.t != 0):
             self._no_ragged(lengths, "extend on a cache that holds history or is branched")
-        starts = self._ragged_checks(u, lengths)
+        starts = self._ragged_checks(u, lengths, self._prompt_hint(c, "prefill") if isinstance(c, DecodeCache) else "")
         self._decode_checks(u, cache, u.shape[1], fresh=True)
         return starts
 
@@ -721,8 +722,22 @@ class HyenaOperator(nn.Module):
     # ------------------------------------------------------------------------------ incremental decoding
     def allocate_decode_cache(self, batch_size, max_seqlen, history_dtype=torch.float32):
         """A DecodeCache for ``batch_size`` rows and up to min(max_seqlen, l_max) positions (decode.py), its history stored
-        as ``history_dtype``: torch.float32, or torch.float16 / torch.bfloat16 for half the state (DESIGN.md section 4.16)."""
+        as ``history_dtype``: torch.float32, or torch.float16 / torch.bfloat16 for half the state (DESIGN.md section 4.16).
+        ``max_seqlen`` None: an unbounded cache, which steps and extends past any position by sliding out the history the
+        filter's l_max taps no longer reach (DESIGN.md section 4.20)."""
         return DecodeCache.allocate(self, batch_size, max_seqlen, history_dtype)
+
+    @staticmethod
+    def _prompt_hint(c, what):
+        """The end of a too-long prompt's error for the cache ``c``: an unbounded cache points to extend."""
+        return (f", the most an unbounded cache takes in one {what}; give it the first {c.reach} positions and extend by "
+                "the rest") if c.unbounded else ""
+
+    @classmethod
+    def _check_prompt(cls, c, P, what):
+        """An unbounded cache takes prompts of at most l_max positions (the filter's reach) in one prefill or admit."""
+        if c.unbounded and P > c.reach:
+            raise HyenaB200Error(f"{what}: a prompt of {P} positions exceeds l_max = {c.reach}{cls._prompt_hint(c, what)}")
 
     def _decode_checks(self, u, cache, n, fresh=False):
         if not isinstance(cache, DecodeCache):
@@ -743,7 +758,10 @@ class HyenaOperator(nn.Module):
         if c.branched and c.t + n > c.base + c.hc:
             raise HyenaB200Error(f"decoding past the branch horizon: positions [{c.t}, {c.t + n}) exceed base + Hc = "
                                  f"{c.base} + {c.hc} = {c.base + c.hc} (fork with a larger horizon, up to Lcap = {c.lcap})")
-        if c.t + n > c.lcap:
+        if c.unbounded:
+            if fresh:
+                self._check_prompt(c, n, "prefill")
+        elif c.t + n > c.lcap:
             raise HyenaB200Error(f"decoding past the cache: positions [{c.t}, {c.t + n}) exceed Lcap = min(max_seqlen, "
                                  f"l_max) = {c.lcap} (l_max = {self.l_max}: the filter has no taps beyond it)")
         if not u.is_cuda or not c.k.is_cuda:
@@ -831,6 +849,7 @@ class HyenaOperator(nn.Module):
         if len(rows) != k:
             raise HyenaB200Error(f"admit: {len(rows)} rows for {k} prompts")
         starts = [P - n for n in host_lengths(lengths, k, P)] if lengths is not None else [0] * k
+        self._check_prompt(c, P, "admit")
         ops.decode_admit_plan(c.t, c.lcap, P, c.win_b, c.win_wc)        # P <= Lcap, and the right shift fits
         if not u.is_cuda or not c.k.is_cuda:
             raise HyenaB200Error("decoding runs on CUDA sm_90a only; there is no CPU fallback")
@@ -921,9 +940,10 @@ class HyenaOperator(nn.Module):
         matrix-vector products (F.linear); the operator itself runs in csrc/decode.cuh, two launches per recurrence.  After
         a run of steps at a long history the step reads only the positions of a window opened by one FFT refresh
         (ops.decode_window_plan chooses).  On a branched cache (DecodeCache.fork) the step reads each branch's positions since
-        the fork base only (ops.decode_branch_step)."""
+        the fork base only (ops.decode_branch_step).  An unbounded cache at Lcap slides first (DecodeCache._make_room)."""
         self._no_ragged(lengths, "step")
         c = self._decode_checks(u_t, cache, 1)
+        c._make_room(1, step=True)
         y = self._step_with(u_t, c, ops.decode_branch_step if c.branched else ops.decode_step_auto)
         c.t += 1
         return y
@@ -952,7 +972,8 @@ class HyenaOperator(nn.Module):
         Toeplitz kernel over the cached history, or for large n the FFT convolution of the whole history
         (ops.decode_extend_uses_fft chooses from t and n).  On a branched cache the same routes run over each branch's
         positions since the fork base only (ops.decode_branch_extend).  ``lengths`` is accepted on a fresh cache only,
-        where this is ``prefill(u, cache, lengths)``."""
+        where this is ``prefill(u, cache, lengths)``.  An unbounded cache slides first when the n positions would pass
+        Lcap, and runs more than S positions (l_max on a fresh cache) as consecutive extends (DESIGN.md section 4.20)."""
         n = u.shape[1] if u.dim() == 3 else -1
         if n < 1:
             raise HyenaB200Error(f"extend input must be (B, n, {self.d_model}) with n >= 1; got {tuple(u.shape)}")
@@ -962,9 +983,27 @@ class HyenaOperator(nn.Module):
         c = self._decode_checks(u, cache, n)
         if c.branched:
             return self._extend(u, c, ops.decode_branch_extend)
+        if c.unbounded and n > (c.slide if c.t else c.reach):
+            return self._extend_pieces(u, c)
         if c.t == 0:
             return self.prefill(u, c)
+        c._make_room(n)
         return self._extend(u, c, ops.decode_extend)
+
+    def _extend_pieces(self, u, c):
+        """extend of the unbounded operator cache ``c`` by more positions than it takes at once: consecutive extends of at
+        most S positions (the first a prefill of at most l_max on a fresh cache), each after its own slide, written into
+        one output tensor."""
+        B, n, D = u.shape
+        y, i = None, 0
+        while i < n:
+            m = min(n - i, c.slide if c.t else c.reach)
+            yi = self.extend(u[:, i:i + m].contiguous(), c)
+            if y is None:
+                y = torch.empty(B, n, D, dtype=yi.dtype, device=yi.device)
+            y[:, i:i + m] = yi
+            i += m
+        return y
 
     def _extend(self, u, c, core):
         """extend on a non-fresh cache with ``core`` (ops.decode_extend or one of its two routes) for the operator."""

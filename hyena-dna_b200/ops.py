@@ -1219,7 +1219,7 @@ def decode_branch_step(p_t, in_bias, sw, sb, cache):
 # step, extend, window and StepGraph replay runs unchanged.  Room is reclaimed by shifting the whole history left by the
 # smallest first real position of the live rows (rounded down to a multiple of 4); a prompt longer than t shifts it right
 # first.  F of an open window is translation invariant, so the window survives a shift that keeps t inside it.  DESIGN.md
-# section 4.15.
+# section 4.15.  An unbounded cache slides the same way past the positions its filter no longer reaches (section 4.20).
 def _window_holds(t, win_b, win_wc):
     return win_wc > 0 and win_b <= t < win_b + win_wc
 
@@ -1252,6 +1252,29 @@ def decode_compact_plan(t, starts, free, win_b=0, win_wc=0):
     live = [int(s) for b, s in enumerate(starts) if b not in free]
     m = min(min(live), t) if live else t
     m -= m % 4
+    return -m, t - m, _window_holds(t, win_b, win_wc) and m <= win_b
+
+
+def decode_slide_plan(t, n, lk, lcap, win_b=0, win_wc=0, step=False):
+    """(shift, t', keep) of making room for n more positions at position t of an unbounded cache whose filter reaches lk
+    positions (its taps are zero from lk on) and whose buffer holds Lcap = lcap (DESIGN.md section 4.20): shift = 0 when
+    there is room, else -m with m = t - lk + 1 rounded down to a multiple of 4, every position no output at t or later
+    reaches; keep whether the window, moved by -m, still holds t' = t - m (compact's rule: it does unless m > win_b).
+    There is room when t + n <= lcap and, for a ``step``, no window would open short: a step at t >= WINDOW_MIN_T outside
+    the window may refresh it, and decode_window_bounds(t, lcap) would give it fewer than WINDOW positions, a full FFT
+    refresh for a window the next slide ends.  Sliding first gives it WINDOW positions (when lk >= WINDOW - 3, the only
+    case in which t reaches WINDOW_MIN_T).  Raises when the n positions do not fit even after the slide (an extend runs
+    in pieces of at most S that do)."""
+    t, n, lk, lcap = int(t), int(n), int(lk), int(lcap)
+    short = step and t >= WINDOW_MIN_T and not _window_holds(t, win_b, win_wc) and \
+        decode_window_bounds(t, lcap)[1] < WINDOW
+    if t + n <= lcap and not short:
+        return 0, t, _window_holds(t, win_b, win_wc)
+    m = max(t - lk + 1, 0)
+    m -= m % 4
+    if t - m + n > lcap:
+        raise _lib.HyenaB200Error(f"decoding past the cache: positions [{t}, {t + n}) exceed Lcap = {lcap} even after a "
+                                  f"slide by {m} (the filter reaches {lk} positions); extend in smaller pieces")
     return -m, t - m, _window_holds(t, win_b, win_wc) and m <= win_b
 
 
