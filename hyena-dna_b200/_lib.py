@@ -43,6 +43,8 @@ SIGNATURES = {
     "hyena_b200_core_bwd": (_i, [c_fp] * 16 + [_i, _i, _i, _vp, _sz, _vp]),
     "hyena_b200_core_bwd_rows": (_i, [c_fp] * 17 + [_i, _i, _i, _vp, _sz, _vp]),
     "hyena_b200_core_fwd_packed": (_i, [c_fp] * 11 + [ctypes.c_longlong, _i, _i, _i, _vp, _sz, _vp]),
+    "hyena_b200_core_fwd_windows": (_i, [c_fp] * 10 + [ctypes.c_longlong, _i, _i, _i, _vp, _sz, _vp]),
+    "hyena_b200_fftconv_fwd_windows": (_i, [c_fp] * 7 + [ctypes.c_longlong, _i, _i, _i, _vp, _sz, _vp]),
     "hyena_b200_core_bwd_packed": (_i, [c_fp] * 16 + [ctypes.c_longlong, _i, _i, _i, _vp, _sz, _vp]),
     "hyena_b200_short_bwd_packed": (_i, [c_fp] * 6 + [ctypes.c_longlong, _i, _i, _i, _vp]),
     "hyena_b200_fftconv_fwd": (_i, [c_fp] * 4 + [_i, _i, _i, _vp, _sz, _vp]),

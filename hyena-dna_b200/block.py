@@ -65,6 +65,11 @@ class Block(nn.Module):
         (HyenaOperator.forward); with the loss on real positions only, every gradient at the pads is 0."""
         if mixer_subset is not None:
             raise HyenaB200Error("Block: mixer_subset is not supported")
+        if mixer_kwargs and mixer_kwargs.get("stream"):
+            # streaming forward (HyenaOperator.forward(u, stream=True)): every position of a sequence of any length
+            kw = dict(mixer_kwargs)
+            self._check_stream(hidden_states, kw.get("inference_params"), lengths, mask, kw.get("cu_seqlens"))
+            return self._run_stream(hidden_states, residual, lambda y: self.mixer(y, **kw))
         if mixer_kwargs and mixer_kwargs.get("cu_seqlens") is not None:
             # flash-attention's unpadded convention: hidden_states (total, D), mixer_kwargs cu_seqlens / max_seqlen
             kw = dict(mixer_kwargs)
@@ -95,6 +100,11 @@ class Block(nn.Module):
         if not hasattr(self.mixer, "check_packed_decode"):
             raise HyenaB200Error(f"Block: the mixer {type(self.mixer).__name__} takes no packed prompts")
         return self.mixer.check_packed_decode(hidden_states, cache, cu_seqlens, max_seqlen, lengths, rows)
+
+    def _check_stream(self, hidden_states, cache=None, lengths=None, mask=None, cu_seqlens=None, device=True):
+        if not hasattr(self.mixer, "check_stream"):
+            raise HyenaB200Error(f"Block: the mixer {type(self.mixer).__name__} takes no stream")
+        return self.mixer.check_stream(hidden_states, cache, lengths, mask, cu_seqlens, device)
 
     def _check_mask(self, hidden_states, mask, cache=None, lengths=None):
         if not hasattr(self.mixer, "check_mask"):
@@ -150,6 +160,46 @@ class Block(nn.Module):
         with torch.no_grad():
             return self._run(hidden_states, residual, mix)
 
+    @staticmethod
+    def _stream_add_norm(hidden_states, residual, norm):
+        """_add_norm of a (B, L, D) stream in pieces of ops.STREAM_CHUNK_POSITIONS positions of all rows, so that no
+        launch takes more positions than a 2^20-position forward: -> (y, residual), both fp32 (B, L, D)."""
+        B, L, D = hidden_states.shape
+        n = max(1, ops.STREAM_CHUNK_POSITIONS // B)
+        y = torch.empty(B, L, D, dtype=torch.float32, device=hidden_states.device)
+        res = torch.empty(B, L, D, dtype=torch.float32, device=hidden_states.device)
+        for a in range(0, L, n):
+            yc, rc = Block._add_norm(hidden_states[:, a:a + n], residual[:, a:a + n] if residual is not None else None,
+                                     norm)
+            y[:, a:a + n] = yc
+            res[:, a:a + n] = rc
+        return y, res
+
+    def _run_stream(self, hidden_states, residual, mix):
+        """_run for a stream (inference): the mixer runs on the whole sequence (it cuts its own chunks); the fused add +
+        LayerNorm and the MLP act per position and run in pieces of ops.STREAM_CHUNK_POSITIONS positions of all rows."""
+        in_dtype = hidden_states.dtype
+        B, L, _ = hidden_states.shape
+        with torch.no_grad():
+            y, residual = self._stream_add_norm(hidden_states, residual, self.norm1)
+            hidden_states = mix(y.to(in_dtype))
+            del y
+            if isinstance(hidden_states, tuple):            # mixers built with return_state
+                hidden_states = hidden_states[0]
+            if not isinstance(self.mlp, nn.Identity):
+                y, residual = self._stream_add_norm(hidden_states, residual, self.norm2)
+                n = max(1, ops.STREAM_CHUNK_POSITIONS // B)
+                out = None
+                for a in range(0, L, n):
+                    oc = self.mlp(y[:, a:a + n].to(in_dtype))
+                    if out is None:
+                        out = torch.empty(B, L, oc.shape[-1], dtype=oc.dtype, device=oc.device)
+                    out[:, a:a + n] = oc
+                hidden_states = out
+            if not self.residual_in_fp32:
+                residual = residual.to(in_dtype)
+        return hidden_states, residual
+
     def _run(self, hidden_states, residual, mix):
         in_dtype = hidden_states.dtype
         y, residual = self._add_norm(hidden_states, residual, self.norm1)
@@ -176,11 +226,23 @@ class Backbone(nn.Module):
                   prenorm=True, residual_in_fp32=residual_in_fp32) for _ in range(n_layer)])
         self.ln_f = nn.LayerNorm(d_model, eps=layer_norm_epsilon)
 
-    def forward(self, hidden_states, lengths=None, mask=None, cu_seqlens=None, max_seqlen=None):
+    def forward(self, hidden_states, lengths=None, mask=None, cu_seqlens=None, max_seqlen=None, stream=False):
         """``lengths``: left-padded rows (HyenaOperator.forward), inference only.  ``mask``: the (B, L) attention mask of a
         left-padded batch (the reference datamodules' ``mask`` batch kwarg), differentiable (HyenaOperator.forward).
         ``cu_seqlens`` / ``max_seqlen``: packed sequences, hidden_states (total, D) or (1, total, D) (HyenaOperator.forward),
-        validated once for all layers."""
+        validated once for all layers.  ``stream=True``: every position of a (B, L, D) input of any length, each layer
+        streaming its own l_max - 1 positions of context (HyenaOperator.forward(u, stream=True)); inference only, every
+        layer checked before the first kernel."""
+        if stream:
+            for layer in self.layers:
+                layer._check_stream(hidden_states, None, lengths, mask, cu_seqlens, device=False)
+            self.layers[0]._check_stream(hidden_states)
+            residual = None
+            for layer in self.layers:
+                hidden_states, residual = layer(hidden_states, residual, mixer_kwargs={"stream": True})
+            with torch.no_grad():
+                y, _ = Block._stream_add_norm(hidden_states, residual, self.ln_f)
+                return y.to(hidden_states.dtype)
         if cu_seqlens is not None:
             pk = self.layers[0]._check_packed(hidden_states, cu_seqlens, max_seqlen, None, lengths, mask)
             residual = None

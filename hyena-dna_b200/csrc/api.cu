@@ -402,7 +402,7 @@ HY_API int hyena_b200_spectrum_to_rfft(const float* dk, int fft_size, float* dfi
 static int core_fwd_run(const float* p, const float* in_bias, const float* sw, const float* sb, const float* kspec,
                         const float* fbias, float* y_pre, float* c_save, float* gspec_save, const int* row_start, int B,
                         int D, int L, void* workspace, size_t workspace_bytes, void* stream,
-                        const long long* seg_base = nullptr, long long total = 0) {
+                        const long long* seg_base = nullptr, long long total = 0, const int* out_start = nullptr) {
   cudaStream_t s = (cudaStream_t)stream;
   Twiddles T;
   if (get_twiddles(s, &T)) return 1;
@@ -421,6 +421,7 @@ static int core_fwd_run(const float* p, const float* in_bias, const float* sw, c
     a.vec = ((L & 1) == 0) && (!c_save || aligned8(c_save));
     a.stage = 0;
     col_mode = COL_GATE_PACKED; inv_mode = INV_CONV_FWD_PACKED;
+    if (out_start) { a.out_start = out_start; inv_mode = INV_CONV_FWD_WIN; }   // windows: COL_GATE_PACKED reads them as is
   }
   for (int c0 = 0; c0 < D; c0 += c.nch) {
     const int n = (D - c0 < c.nch) ? D - c0 : c.nch;
@@ -568,6 +569,28 @@ HY_API int hyena_b200_core_fwd_packed(const float* p, const float* in_bias, cons
                       workspace_bytes, stream, seg_base, total);
 }
 
+// the guards both window entry points share (check_packed, plus out_start)
+static int check_windows(const long long* seg_base, const int* row_start, const int* out_start, long long total, int B,
+                         int D, int L) {
+  if (check_packed(seg_base, row_start, total, B, D, L)) return 1;
+  HY_CHECK(out_start && aligned4(out_start), "null or misaligned pointer: out_start must be 4-byte aligned");
+  return 0;
+}
+
+HY_API int hyena_b200_core_fwd_windows(const float* p, const float* in_bias, const float* sw, const float* sb,
+                                       const float* kspec, const float* fbias, float* y_pre, const long long* seg_base,
+                                       const int* row_start, const int* out_start, long long total, int B, int D, int L,
+                                       void* workspace, size_t workspace_bytes, void* stream) {
+  if (check_windows(seg_base, row_start, out_start, total, B, D, L)) return 1;
+  HY_CHECK(p && sw && sb && kspec && fbias && y_pre, "null pointer");
+  HY_CHECK(aligned4(p) && aligned4(sw) && aligned4(sb) && aligned4(fbias) && aligned4(y_pre) &&
+               (!in_bias || aligned4(in_bias)),
+           "misaligned pointer: p, in_bias, sw, sb, fbias and y_pre must be 4-byte aligned");
+  HY_CHECK(aligned8(kspec), "misaligned pointer: kspec must be 8-byte aligned");
+  return core_fwd_run(p, in_bias, sw, sb, kspec, fbias, y_pre, nullptr, nullptr, row_start, B, D, L, workspace,
+                      workspace_bytes, stream, seg_base, total, out_start);
+}
+
 HY_API int hyena_b200_core_bwd_packed(const float* dy_pre, const float* p, const float* in_bias, const float* sw,
                                       const float* sb, const float* kspec, const float* fbias, const float* c_saved,
                                       const float* gspec_saved, float* dk, float* dsw, float* dsb, float* dfbias,
@@ -701,6 +724,33 @@ HY_API int hyena_b200_fftconv_fwd(const float* u, const float* kspec, const floa
     HY_CUDA(launch_col_fwd(COL_PLAIN, a, n * B, s));
     HY_CUDA(launch_row_pass(ROW_CONV_FWD, a, n * B, s));
     HY_CUDA(launch_col_inv(INV_PLAIN_FWD, a, n * B, s));
+  }
+  return 0;
+}
+
+HY_API int hyena_b200_fftconv_fwd_windows(const float* u, const float* kspec, const float* Dvec, float* out,
+                                          const long long* seg_base, const int* row_start, const int* out_start,
+                                          long long total, int B, int H, int L, void* workspace, size_t workspace_bytes,
+                                          void* stream) {
+  if (check_windows(seg_base, row_start, out_start, total, B, H, L)) return 1;
+  HY_CHECK(u && kspec && Dvec && out, "null pointer");
+  HY_CHECK(aligned4(u) && aligned4(Dvec) && aligned4(out) && aligned8(kspec),
+           "misaligned pointer: u, Dvec and out must be 4-byte aligned, kspec 8-byte aligned");
+  cudaStream_t s = (cudaStream_t)stream;
+  Twiddles T;
+  if (get_twiddles(s, &T)) return 1;
+  Carve c;
+  if (carve(workspace, workspace_bytes, B, H, L, false, &c)) return 1;
+  PassArgs a = base_args(B, H, L, T);
+  a.A = c.A; a.kspec = reinterpret_cast<const float2*>(kspec);
+  a.src = u; a.fbias = Dvec; a.out = out;
+  a.row_start = row_start; a.seg_base = seg_base; a.cstride = total; a.out_start = out_start;
+  for (int c0 = 0; c0 < H; c0 += c.nch) {
+    const int n = (H - c0 < c.nch) ? H - c0 : c.nch;
+    a.c0 = c0;
+    HY_CUDA(launch_col_fwd(COL_PLAIN_WIN, a, n * B, s));
+    HY_CUDA(launch_row_pass(ROW_CONV_FWD, a, n * B, s));
+    HY_CUDA(launch_col_inv(INV_PLAIN_FWD_WIN, a, n * B, s));
   }
   return 0;
 }

@@ -165,20 +165,28 @@ __device__ __forceinline__ void store_pair_seg(float* __restrict__ row, int t0, 
 // kind of the plain mode (col_kind / inv_kind).
 // *_PACKED: the same modes on packed sequences (see load_window_seg): p, dy_pre, y_pre and ds are packed (C, total) tensors
 // addressed through seg_base, c_save stays in the bucket's row layout (B, D, L); they run the register (unstaged) path.
+// *_WIN: overlapping windows of long sequences (streaming forward, DESIGN.md section 4.21): the packed addressing, and
+// the outputs stored only at t >= out_start[b] (positions before it are the window's context, whose outputs another
+// window stores).  COL_PLAIN_WIN / INV_PLAIN_FWD_WIN are the plain convolution (u and out packed, the D skip term in the
+// spectrum as for COL_PLAIN); INV_CONV_FWD_WIN is INV_CONV_FWD_PACKED without c_save, after COL_GATE_PACKED.
 enum ColMode { COL_FILTER = 0, COL_GATE = 1, COL_DC = 2, COL_PLAIN = 3, COL_GATE_ROWS = 4, COL_DC_ROWS = 5,
-               COL_GATE_PACKED = 6, COL_DC_PACKED = 7 };
+               COL_GATE_PACKED = 6, COL_DC_PACKED = 7, COL_PLAIN_WIN = 8 };
 enum InvMode { INV_CONV_FWD = 0, INV_BWD_DG = 1, INV_DK = 2, INV_PLAIN_FWD = 3, INV_PLAIN_BWD = 4, INV_CONV_FWD_ROWS = 5,
-               INV_BWD_DG_ROWS = 6, INV_CONV_FWD_PACKED = 7, INV_BWD_DG_PACKED = 8 };
+               INV_BWD_DG_ROWS = 6, INV_CONV_FWD_PACKED = 7, INV_BWD_DG_PACKED = 8, INV_CONV_FWD_WIN = 9,
+               INV_PLAIN_FWD_WIN = 10 };
 __host__ __device__ constexpr int col_kind(int mode) {
   return (mode == COL_GATE_ROWS || mode == COL_GATE_PACKED) ? COL_GATE
          : (mode == COL_DC_ROWS || mode == COL_DC_PACKED)   ? COL_DC
+         : (mode == COL_PLAIN_WIN)                           ? COL_PLAIN
                                                              : mode;
 }
 __host__ __device__ constexpr int inv_kind(int mode) {
-  return (mode == INV_CONV_FWD_ROWS || mode == INV_CONV_FWD_PACKED) ? INV_CONV_FWD
-         : (mode == INV_BWD_DG_ROWS || mode == INV_BWD_DG_PACKED)   ? INV_BWD_DG
-                                                                     : mode;
+  return (mode == INV_CONV_FWD_ROWS || mode == INV_CONV_FWD_PACKED || mode == INV_CONV_FWD_WIN) ? INV_CONV_FWD
+         : (mode == INV_BWD_DG_ROWS || mode == INV_BWD_DG_PACKED)                               ? INV_BWD_DG
+         : (mode == INV_PLAIN_FWD_WIN)                                                          ? INV_PLAIN_FWD
+                                                                                                 : mode;
 }
+__host__ __device__ constexpr bool inv_win(int mode) { return mode == INV_CONV_FWD_WIN || mode == INV_PLAIN_FWD_WIN; }
 // the backward pass-3 epilogue (plain or on left-padded rows)
 __host__ __device__ constexpr bool inv_bwd_dg(int mode) { return mode == INV_BWD_DG || mode == INV_BWD_DG_ROWS; }
 enum RowMode { ROW_FILTER = 0, ROW_CONV_FWD = 1, ROW_CONV_BWD = 2, ROW_CONV_BWD1 = 3 };
@@ -217,6 +225,7 @@ struct PassArgs {
   const int* row_start;  // *_ROWS and *_PACKED modes: (B) first real position of each batch row
   const long long* seg_base;  // *_PACKED modes: (B) offset of row b's position 0 in a packed channel (may be < 0)
   long long cstride;          // *_PACKED modes: channel stride of the packed tensors (total positions)
+  const int* out_start;       // *_WIN modes: (B) first position of row b whose output is stored
 };
 
 __device__ __forceinline__ size_t row_off(int b, int ch, int nch, int L) { return ((size_t)b * nch + ch) * (size_t)L; }
@@ -301,6 +310,8 @@ __device__ __forceinline__ float2 col_input(const PassArgs& a, int b, int c, int
     const float2 x0 = conv_window(P, t0, a.L, ka);
     const float2 dy = load_pair(a.src + row_off(b, c, a.D, a.L), t0, a.L, vec);
     return mask_pair(make_float2(x0.x * dy.x, x0.y * dy.y), t0, rs);
+  } else if constexpr (MODE == COL_PLAIN_WIN) {  // COL_PLAIN on a window (packed addressing, read from rs)
+    return load_pair_seg(a.src + (sg + (long long)c * a.cstride), t0, a.L, rs);
   } else if constexpr (MODE == COL_FILTER) {
     return load_pair(a.src + (size_t)c * a.L, t0, a.L, vec);
   } else if constexpr (MODE == COL_PLAIN) {
@@ -351,7 +362,7 @@ __device__ __forceinline__ void col_fwd_body(const PassArgs& a, const int bx, co
     ka = load_taps(a.sw, a.sb, a.in_bias, c);
     rs = __ldg(a.row_start + b);
   }
-  if constexpr (MODE == COL_GATE_PACKED || MODE == COL_DC_PACKED) {
+  if constexpr (MODE == COL_GATE_PACKED || MODE == COL_DC_PACKED || MODE == COL_PLAIN_WIN) {
     rs = __ldg(a.row_start + b);
     sg = __ldg(a.seg_base + b);
   }
@@ -462,7 +473,8 @@ struct InvCtx {
   float rw[3][3];      // INV_BWD_DG: partials of d short_filter.weight for the x0 / x1 / v channels
   float rb[3];         //             and of d short_filter.bias
   int rs;              // INV_CONV_FWD_ROWS / INV_BWD_DG_ROWS / *_PACKED: first real position of the row
-  long long sg;        // *_PACKED: offset of the row's position 0 in a packed channel
+  long long sg;        // *_PACKED / *_WIN: offset of the row's position 0 in a packed channel
+  int os;              // *_WIN: first position whose output is stored (never before rs)
 };
 
 // dw_j += ds[t0] P(t0-2+j) + ds[t0+1] P(t0-1+j);  db += ds[t0] + ds[t0+1]     (P = window of the filter input)
@@ -490,7 +502,7 @@ __device__ __forceinline__ void inv_load(const PassArgs& a, const InvCtx& cx, in
     in.b = load_pair(a.src + row_off(b, c, D, L), t0, L, vec);
   } else if constexpr (MODE == INV_CONV_FWD || MODE == INV_CONV_FWD_ROWS) {
     load_window(a.p + row_off(b, c, 3 * D, L), t0, L, vec, cx.k0.ib, in.P0);     // x0 only: c = y already holds bias * g
-  } else if constexpr (MODE == INV_CONV_FWD_PACKED) {
+  } else if constexpr (MODE == INV_CONV_FWD_PACKED || MODE == INV_CONV_FWD_WIN) {
     load_window_seg(a.p + (cx.sg + (long long)c * a.cstride), t0, L, cx.rs, cx.k0.ib, in.P0);
   } else if constexpr (MODE == INV_BWD_DG_PACKED) {
     load_window_seg(a.p + (cx.sg + (long long)c * a.cstride), t0, L, cx.rs, cx.k0.ib, in.P0);
@@ -534,6 +546,11 @@ __device__ __forceinline__ void inv_finish(const PassArgs& a, InvCtx& cx, int b,
     const float2 x0 = conv_window(in.P0, t0, L, cx.k0);  // layout) is 0 at t < rs; the windows are 0 there already
     if (a.out2) store_pair(a.out2 + row_off(b, c, D, L), t0, L, vec, mask_pair(y, t0, cx.rs));
     store_pair_seg(a.out + (cx.sg + (long long)c * a.cstride), t0, L, cx.rs, pmul(y, x0));
+  } else if constexpr (MODE == INV_CONV_FWD_WIN) {    // a window: y_pre is stored at t >= os only (the windows of x0
+    const float2 x0 = conv_window(in.P0, t0, L, cx.k0);  // are 0 before rs, and os >= rs)
+    store_pair_seg(a.out + (cx.sg + (long long)c * a.cstride), t0, L, cx.os, pmul(y, x0));
+  } else if constexpr (MODE == INV_PLAIN_FWD_WIN) {   // a window of the plain convolution: out stored at t >= os only
+    store_pair_seg(a.out + (cx.sg + (long long)c * a.cstride), t0, L, cx.os, y);
   } else if constexpr (MODE == INV_BWD_DG_PACKED) {   // INV_BWD_DG_ROWS on a packed sequence: ds is stored at t >= rs only
     const float2 x0 = conv_window(in.P0, t0, L, cx.k0), x1 = conv_window(in.P1, t0, L, cx.k1),
                  vv = conv_window(in.P2, t0, L, cx.k2);
@@ -623,6 +640,12 @@ __device__ __forceinline__ void col_inv_body(const PassArgs& a, const int bx, co
     cx.k0 = load_taps(a.sw, a.sb, a.in_bias, c);
     cx.rs = __ldg(a.row_start + b);
     cx.sg = __ldg(a.seg_base + b);
+  }
+  if constexpr (inv_win(MODE)) {
+    if constexpr (MODE == INV_CONV_FWD_WIN) cx.k0 = load_taps(a.sw, a.sb, a.in_bias, c);
+    cx.rs = __ldg(a.row_start + b);
+    cx.sg = __ldg(a.seg_base + b);
+    cx.os = max(__ldg(a.out_start + b), cx.rs);
   }
   if constexpr (inv_bwd_dg(MODE) || MODE == INV_BWD_DG_PACKED) {
     cx.k1 = load_taps(a.sw, a.sb, a.in_bias, a.D + c);

@@ -11,6 +11,7 @@ cudaError_t launch_col_fwd(int mode, const PassArgs& a, int rows, cudaStream_t s
     case COL_DC_ROWS: return launch_col_fwd_mode<COL_DC_ROWS>(a, rows, s);
     case COL_GATE_PACKED: return launch_col_fwd_mode<COL_GATE_PACKED>(a, rows, s);
     case COL_DC_PACKED: return launch_col_fwd_mode<COL_DC_PACKED>(a, rows, s);
+    case COL_PLAIN_WIN: return launch_col_fwd_mode<COL_PLAIN_WIN>(a, rows, s);
   }
   return cudaErrorInvalidValue;
 }

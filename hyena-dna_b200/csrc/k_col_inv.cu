@@ -12,6 +12,8 @@ cudaError_t launch_col_inv(int mode, const PassArgs& a, int rows, cudaStream_t s
     case INV_BWD_DG_ROWS: return launch_col_inv_mode<INV_BWD_DG_ROWS>(a, rows, s);
     case INV_CONV_FWD_PACKED: return launch_col_inv_mode<INV_CONV_FWD_PACKED>(a, rows, s);
     case INV_BWD_DG_PACKED: return launch_col_inv_mode<INV_BWD_DG_PACKED>(a, rows, s);
+    case INV_CONV_FWD_WIN: return launch_col_inv_mode<INV_CONV_FWD_WIN>(a, rows, s);
+    case INV_PLAIN_FWD_WIN: return launch_col_inv_mode<INV_PLAIN_FWD_WIN>(a, rows, s);
   }
   return cudaErrorInvalidValue;
 }

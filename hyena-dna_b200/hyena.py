@@ -400,7 +400,7 @@ class HyenaOperator(nn.Module):
         self.filter_fn = HyenaFilter(self.head_dim * inner_factor * (order - 1), order=filter_order, seq_len=l_max,
                                      channels=1, dropout=filter_dropout, **filter_args)
 
-    def forward(self, u, *args, lengths=None, mask=None, cu_seqlens=None, max_seqlen=None, **kwargs):
+    def forward(self, u, *args, lengths=None, mask=None, cu_seqlens=None, max_seqlen=None, stream=False, **kwargs):
         """``lengths`` (B integers in [1, L]): u is left-padded, row b's real tokens are its last lengths[b] positions.  Its
         outputs there do not depend on the padding: they are the outputs of the unpadded row (DESIGN.md section 4.14); at a
         pad position the output is out_proj(0) = out_proj.bias.  Inference only: with grad required it raises (use
@@ -416,8 +416,19 @@ class HyenaOperator(nn.Module):
         convention): u is (total, D) or (1, total, D), sequences packed without padding, sequence i at positions
         [cu_seqlens[i], cu_seqlens[i+1]).  Each sequence runs as if alone (DESIGN.md section 4.18); the output has u's
         shape.  ``max_seqlen``, when given, must be at least the longest sequence.  Order 2 with a causal filter only;
-        not with ``lengths``, ``mask`` or a DecodeCache."""
+        not with ``lengths``, ``mask`` or a DecodeCache.
+
+        ``stream=True``: u (B, L, D) of any length, every position's output (DESIGN.md section 4.21).  The output at t is
+        the layer with its l_max-tap causal convolution applied as a stream, the outputs an unbounded DecodeCache gives,
+        computed on overlapping windows of the FFT core; for L <= l_max it is ``forward(u)``, bit for bit.  Inference
+        only (run under torch.no_grad()), a causal filter, l_max <= 2^20 - 2; not with ``lengths``, ``mask``,
+        ``cu_seqlens`` or a DecodeCache."""
         cache = kwargs.get("inference_params")
+        if stream:
+            plan = self.check_stream(u, cache, lengths, mask, cu_seqlens)
+            if plan is not None:
+                y = self._forward_stream(u, plan)
+                return (y, None) if self.return_state else y
         if cu_seqlens is not None:
             y = self._forward_packed(u, self.check_packed(u, cu_seqlens, max_seqlen, cache, lengths, mask))
             return (y, None) if self.return_state else y
@@ -474,6 +485,86 @@ class HyenaOperator(nn.Module):
         if self.return_state:
             return y, None
         return y
+
+    def check_stream(self, u, cache=None, lengths=None, mask=None, cu_seqlens=None, device=True):
+        """Every host check of ``forward(u, stream=True)`` without device work (Block and Backbone run it before their first
+        kernel) -> the plan (ops.stream_plan), or None when L <= l_max (then ``forward(u)`` runs).  ``device`` False: all
+        but the check that u is on the GPU (a Backbone checks every layer before it checks the device)."""
+        if lengths is not None or mask is not None or cu_seqlens is not None:
+            raise HyenaB200Error("stream=True does not combine with lengths, mask or cu_seqlens: a streamed row is one "
+                                 "sequence from its first position")
+        if isinstance(cache, DecodeCache):
+            raise HyenaB200Error("stream=True does not combine with a DecodeCache: decode with prefill, step and extend")
+        if self.filter_fn.bidirectional:
+            raise HyenaB200Error("stream=True needs a causal filter; this HyenaFilter is bidirectional")
+        if torch.is_grad_enabled() and (u.requires_grad or any(p.requires_grad for p in self.parameters())):
+            raise HyenaB200Error("forward(u, stream=True) is inference only (run under torch.no_grad())")
+        if u.dim() != 3 or u.shape[-1] != self.d_model or u.shape[1] < 1:
+            raise HyenaB200Error(f"stream=True takes u (B, L, {self.d_model}) with L >= 1; got {tuple(u.shape)}")
+        if self.l_max > ops.STREAM_MAX_WINDOW - 2:
+            raise HyenaB200Error(f"stream=True: l_max = {self.l_max} leaves no room for an output in a window of at "
+                                 f"most {ops.STREAM_MAX_WINDOW} positions (l_max <= {ops.STREAM_MAX_WINDOW - 2})")
+        if device and not u.is_cuda:
+            raise HyenaB200Error("HyenaOperator (hyena_b200) runs on CUDA sm_90a only; there is no CPU fallback")
+        B, L = u.shape[0], u.shape[1]
+        return None if L <= self.l_max else ops.stream_plan(L, self.l_max, self.order, B)
+
+    def _forward_stream(self, u, plan):
+        """forward(u, stream=True) past l_max: the chunks of ``plan`` in turn.  A chunk takes every row's positions
+        [in_start, out_end) as one packed (1, B n) in_proj GEMM, the core on the chunk's overlapping windows (order 2:
+        hyena_b200_core_fwd_windows; order >= 3: the short filter and gates in torch, every recurrence's convolution as
+        its own windowed pass, hyena_b200_fftconv_fwd_windows), out_proj, and keeps the outputs [out_start, out_end)."""
+        B, L, D = u.shape
+        dev, L_b = u.device, plan.L_b
+        y = torch.empty(B, L, D, dtype=u.dtype, device=dev)
+        with torch.no_grad():
+            k = self.filter_fn.filter_channel_major(self.l_max)                      # (D*(order-1), l_max)
+            fb = (self.filter_fn.bias if self.filter_fn.use_bias else 0 * self.filter_fn.bias).reshape(-1)
+            fb = fb.to(torch.float32).contiguous()
+            C = self.short_filter.weight.shape[0]
+            sw = self.short_filter.weight.reshape(C, -1).contiguous()
+            sb = self.short_filter.bias.contiguous()
+            ib = self.in_proj.bias.contiguous() if self.in_proj.bias is not None else None
+            O1 = self.order - 1
+            kk = k.reshape(D, O1, self.l_max)                                        # filter channels are ordered (v o)
+            kspecs = [ops.filter_spectrum(ops._bucket_filter(kk[:, o].contiguous(), L_b)) for o in range(O1)]
+            bb = fb.reshape(D, O1)
+            tables = {}
+            for s, a, e in plan.chunks:
+                n = e - s
+                if n not in tables:
+                    tables[n] = ops.stream_tables(plan.windows(n), B, n if self.order == 2 else D * n, dev)
+                uc = u[:, s:e].to(torch.float32)
+                if self.order == 2:
+                    # one packed (1, B n) layout: row b's position t at b n + t, padded to a multiple of 4 positions
+                    total = B * n
+                    tp = -(-total // 4) * 4
+                    u32 = uc.reshape(total, D)
+                    if tp != total:
+                        u32 = torch.nn.functional.pad(u32, (0, 0, 0, tp - total))
+                    p = _InProj.apply(u32[None].contiguous(), self.in_proj.weight)    # (1, 3D, tp)
+                    y_pre = ops.core_forward_windows(p, ib, sw, sb, kspecs[0], fb, L_b, tables[n], total)
+                    yc = _OutProj.apply(y_pre, self.out_proj.weight, self.out_proj.bias)[0, :total].reshape(B, n, D)
+                else:
+                    y_pre = self._stream_chained(uc.contiguous(), kspecs, bb, L_b, tables[n])
+                    yc = _OutProj.apply(y_pre, self.out_proj.weight, self.out_proj.bias)
+                y[:, a:e] = yc[:, a - s:]
+        return y
+
+    def _stream_chained(self, u, kspecs, bb, L_b, tables):
+        """y_pre (B, D, n) of order >= 3 on a chunk u (B, n, D): _forward_chained's recurrence with every convolution a
+        windowed pass over the chunk's rows (ops.fftconv_forward_windows, channel stride n)."""
+        D = self.d_model
+        n = u.shape[1]
+        p = _InProj.apply(u, self.in_proj.weight)                                   # (B, (order+1) D, n)
+        if self.in_proj.bias is not None:
+            p = p + self.in_proj.bias[None, :, None]
+        uc = torch.nn.functional.conv1d(p, self.short_filter.weight, self.short_filter.bias,
+                                        padding=self.short_filter_order - 1, groups=p.shape[1])[..., :n]
+        *x, v = uc.split(D, dim=1)
+        for o, x_i in enumerate(reversed(x[1:])):
+            v = ops.fftconv_forward_windows((v * x_i).contiguous(), kspecs[o], bb[:, o].contiguous(), L_b, tables)
+        return (v * x[0]).contiguous()
 
     def _padded_checks(self, u, what, hint=""):
         """Host validation of a left-padded input's filter and shape -> (B, P); ``hint`` ends a too-long input's error."""

@@ -561,6 +561,171 @@ class PackedCoreFn(torch.autograd.Function):
         return dp, dib, dsw.reshape(ctx.sw_shape), dsb, dk, dfb.reshape(ctx.fb_shape), None
 
 
+# ------------------------------------------------------------------------------------------ streaming forward
+STREAM_MIN_WINDOW, STREAM_MAX_WINDOW = 1024, 1 << 20
+STREAM_WINDOW_FACTOR = 4        # a window holds at least this many times its context (DESIGN.md section 4.21)
+STREAM_WINDOW_FLOOR = 1 << 16   # and at least this many positions: measured fastest at 1026 taps (H100, DESIGN.md 4.21)
+STREAM_CHUNK_POSITIONS = 1 << 20   # positions of all rows that one chunk holds, context included, when the context allows
+
+
+def stream_context(l_max, order):
+    """Positions of context an output needs before it so that a stream that starts there gives it exactly.  Order 1 is one
+    plain causal convolution (a recurrence of order >= 3): its l_max - 1 earlier inputs.  Order 2: the gated core, whose
+    first two short-filter outputs in a window read zeros before the window, and reach outputs up to l_max positions
+    later: l_max + 1.  Order >= 3: each of the order - 1 recurrences needs its own l_max - 1 valid inputs, plus the two of
+    the short filter: (order - 1) (l_max - 1) + 2."""
+    if l_max < 1 or order < 1:
+        raise _lib.HyenaB200Error(f"stream_context: bad l_max {l_max} or order {order}")
+    if order == 1:
+        return l_max - 1
+    if order == 2:
+        return l_max + 1
+    return (order - 1) * (l_max - 1) + 2
+
+
+def stream_window_length(context):
+    """Window row length L_b for windows with ``context`` positions of context: the smallest power of two holding
+    STREAM_WINDOW_FACTOR times the context, at least STREAM_WINDOW_FLOOR, at most STREAM_MAX_WINDOW (where the windows are
+    2^20 - context outputs each).  Raises when no window of at most 2^20 positions holds the context and one output."""
+    if context + 1 > STREAM_MAX_WINDOW:
+        raise _lib.HyenaB200Error(f"a streaming window needs {context} positions of context and one output, more than "
+                                  f"the {STREAM_MAX_WINDOW} positions of the longest transform")
+    L_b = STREAM_WINDOW_FLOOR
+    while L_b < STREAM_WINDOW_FACTOR * context and L_b < STREAM_MAX_WINDOW:
+        L_b *= 2
+    return L_b
+
+
+def stream_windows(n, L_b, context):
+    """Overlapping windows over one row of n positions -> [(start, row_start, out_start)]: window w covers the row's
+    positions [start, start + L_b) (start < 0 for a row shorter than L_b), reads nothing before row_start (the row has
+    not begun there) and stores the outputs of [start + out_start, start + L_b).  The first window starts the row without
+    context; every later one ends W = L_b - context outputs after the previous one (the last ends at n), so it carries at
+    least ``context`` positions of context, and every position is stored by exactly one window."""
+    W = L_b - context
+    if W < 1:
+        raise _lib.HyenaB200Error(f"stream_windows: a window of {L_b} positions holds no output after {context} of context")
+    e = min(n, L_b)
+    wins = [(e - L_b, L_b - e, L_b - e)]
+    while e < n:
+        m = min(W, n - e)
+        wins.append((e + m - L_b, 0, L_b - m))
+        e += m
+    return wins
+
+
+class StreamPlan:
+    """How forward(u, stream=True) cuts a (B, L) input (stream_plan).  ``chunks``: [(in_start, out_start, out_end)], the
+    positions of every row that one chunk computes from and the outputs it keeps; its first out_start - in_start positions
+    are the context (``chunk_context``, or all earlier positions).  Inside a chunk row of n positions the core runs on
+    ``windows(n)`` of ``L_b`` positions with ``context`` each: the gated core (order 2), or each recurrence's plain
+    convolution as its own windowed pass over the chunk (order >= 3)."""
+
+    def __init__(self, L, l_max, order, B, L_b, context, chunk_context, chunks):
+        self.L, self.l_max, self.order, self.B = L, l_max, order, B
+        self.L_b, self.context, self.chunk_context, self.chunks = L_b, context, chunk_context, chunks
+
+    def windows(self, n):
+        return stream_windows(n, self.L_b, self.context)
+
+    def __repr__(self):
+        return (f"StreamPlan(L={self.L}, l_max={self.l_max}, order={self.order}, L_b={self.L_b}, "
+                f"context={self.context}, chunks={len(self.chunks)})")
+
+
+def stream_plan(L, l_max, order, B=1, L_b=None, chunk_positions=None):
+    """Window and chunk plan of a streaming forward over B rows of L positions (DESIGN.md section 4.21), on the host.
+    Windows have ``stream_context(l_max, 2)`` positions of context for order 2 and ``stream_context(l_max, 1)`` for the
+    plain passes of order >= 3; a chunk carries ``stream_context(l_max, order)``.  L_b: the window row length (a power of
+    two in [1024, 2^20]).  By default a row of L <= 2^20 positions runs as one window of the smallest power of two that
+    holds it (and its context, at least 1024): one chunk of one window, which measured as fast as or faster than any
+    window route; a longer row takes stream_window_length.  chunk_positions: positions of all B rows one chunk should
+    hold (default STREAM_CHUNK_POSITIONS); a chunk keeps at least max(L_b, its context) outputs."""
+    if L < 1 or B < 1:
+        raise _lib.HyenaB200Error(f"stream_plan: bad shape B={B} L={L}")
+    if l_max > STREAM_MAX_WINDOW - 2:
+        raise _lib.HyenaB200Error(f"streaming forward: l_max = {l_max} leaves no room for an output in a window of at "
+                                  f"most {STREAM_MAX_WINDOW} positions (l_max <= {STREAM_MAX_WINDOW - 2})")
+    c = stream_context(l_max, 2 if order == 2 else 1)
+    cc = stream_context(l_max, order)
+    if L_b is None:
+        L_b = STREAM_MIN_WINDOW
+        while L_b < max(L, c + 1):
+            L_b *= 2
+        if L_b > STREAM_MAX_WINDOW:
+            L_b = stream_window_length(c)
+    if L_b < STREAM_MIN_WINDOW or L_b > STREAM_MAX_WINDOW or L_b & (L_b - 1) or L_b <= c:
+        raise _lib.HyenaB200Error(f"stream_plan: window length {L_b} must be a power of two in [{STREAM_MIN_WINDOW}, "
+                                  f"{STREAM_MAX_WINDOW}] longer than the context {c}")
+    per_row = (chunk_positions or STREAM_CHUNK_POSITIONS) // B
+    n_out = max(per_row - cc, cc, L_b, 1)
+    chunks, a = [], 0
+    while a < L:
+        b = min(L, a + n_out)
+        chunks.append((max(0, a - cc), a, b))
+        a = b
+    return StreamPlan(L, l_max, order, B, L_b, c, cc, chunks)
+
+
+def stream_tables(wins, B, row_stride, device):
+    """The seg_base (int64), row_start and out_start (int32) tables of ``wins`` (stream_windows of one row) repeated over
+    B rows, row b's position 0 at b * row_stride, row-major: one host-to-device copy each."""
+    sb = torch.tensor([b * row_stride + w[0] for b in range(B) for w in wins], dtype=torch.int64)
+    rs = torch.tensor([w[1] for _ in range(B) for w in wins], dtype=torch.int32)
+    os_ = torch.tensor([w[2] for _ in range(B) for w in wins], dtype=torch.int32)
+    if device.type == "cuda":
+        sb, rs, os_ = (t.pin_memory().to(device, non_blocking=True) for t in (sb, rs, os_))
+    return sb, rs, os_
+
+
+def _window_launches(rows):
+    for r0 in range(0, rows, MAX_BUCKET_ROWS):
+        yield r0, min(MAX_BUCKET_ROWS, rows - r0)
+
+
+def core_forward_windows(p, in_bias, sw, sb, kspec, fbias, L_b, tables, total=None):
+    """y_pre (1, D, T) of the fused order-2 core on overlapping windows of packed rows: p (1, 3D, T) (channel stride T),
+    kspec the spectrum of the filter cut or zero-padded to L_b, tables from stream_tables (row stride n for rows of n
+    positions).  Every position is written by the window whose outputs it belongs to; positions [total, T) belong to no
+    row and are 0.  One hyena_b200_core_fwd_windows per 65,535 windows."""
+    _need_cuda(p, in_bias, sw, sb, fbias)
+    _, C3, T = p.shape
+    D = C3 // 3
+    if C3 != 3 * D or p.shape[0] != 1 or not p.is_contiguous():
+        raise _lib.HyenaB200Error("core_forward_windows: p must be contiguous (1, 3D, T)")
+    seg_base, row_start, out_start = tables
+    y = torch.empty(1, D, T, dtype=torch.float32, device=p.device)
+    y[..., T if total is None else total:] = 0.0
+    with torch.cuda.device(p.device):
+        for r0, n in _window_launches(seg_base.numel()):
+            ws = workspace(n, D, L_b, False, p.device)
+            _lib.check(_lib.lib().hyena_b200_core_fwd_windows(
+                _ptr(p), _ptr(in_bias), _ptr(sw), _ptr(sb), _ptr(kspec), _ptr(fbias), _ptr(y), _ptr(seg_base[r0:]),
+                _ptr(row_start[r0:]), _ptr(out_start[r0:]), T, n, D, L_b, _ptr(ws), ws.numel(), _stream()))
+    return y
+
+
+def fftconv_forward_windows(u, kspec, Dvec, L_b, tables):
+    """out (B, H, n) = the plain convolution of fftconv_forward on overlapping windows of the rows of u (B, H, n): kspec
+    the spectrum of the filter cut or zero-padded to L_b, tables from stream_tables with row stride H n (channel stride
+    n; hyena_b200_fftconv_fwd_windows)."""
+    _need_cuda(u, Dvec)
+    if u.dim() != 3 or not u.is_contiguous():
+        raise _lib.HyenaB200Error("fftconv_forward_windows: u must be contiguous (B, H, n)")
+    _, H, T = u.shape
+    if Dvec.numel() != H or not Dvec.is_contiguous():
+        raise _lib.HyenaB200Error(f"fftconv_forward_windows: D must have {H} contiguous elements")
+    seg_base, row_start, out_start = tables
+    out = torch.empty_like(u)
+    with torch.cuda.device(u.device):
+        for r0, n in _window_launches(seg_base.numel()):
+            ws = workspace(n, H, L_b, False, u.device)
+            _lib.check(_lib.lib().hyena_b200_fftconv_fwd_windows(
+                _ptr(u), _ptr(kspec), _ptr(Dvec), _ptr(out), _ptr(seg_base[r0:]), _ptr(row_start[r0:]),
+                _ptr(out_start[r0:]), T, n, H, L_b, _ptr(ws), ws.numel(), _stream()))
+    return out
+
+
 # ------------------------------------------------------------------------------------------ plain fftconv
 def fftconv_forward(u, kspec, Dvec):
     _need_cuda(u, Dvec)

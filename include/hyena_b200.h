@@ -184,6 +184,23 @@ HY_API int hyena_b200_short_bwd_packed(const float* ds, const float* sw, float* 
                                        const long long* seg_base, const int* row_start, long long total, int B, int C3,
                                        int L, void* stream);
 
+/* ---- overlapping windows of long sequences (streaming forward, DESIGN.md section 4.21) ---------
+ * core_fwd_windows: the forward of core_fwd_packed (inference, no c_save / gspec_save) on B window rows of length
+ * L <= 2^20: channel c of row b at position t is element seg_base[b] + c * total + t of p (3D channels) and y_pre (D
+ * channels), positions t < row_start[b] read as zeros (the sequence has not begun), and y_pre is written at the positions
+ * t >= max(out_start[b], row_start[b]) of the row only.  Windows may overlap: the positions of a window before its
+ * out_start are context that another window stores.  fftconv_fwd_windows: the same for the plain convolution of
+ * fftconv_fwd on u and out (H channels, channel stride total).  B <= 65535 rows per call (callers split larger sets); the launches of
+ * core_fwd / fftconv_fwd, counted under their kinds; no allocation, no synchronisation. */
+HY_API int hyena_b200_core_fwd_windows(const float* p, const float* in_bias, const float* sw, const float* sb,
+                                       const float* kspec, const float* fbias, float* y_pre, const long long* seg_base,
+                                       const int* row_start, const int* out_start, long long total, int B, int D, int L,
+                                       void* workspace, size_t workspace_bytes, void* stream);
+HY_API int hyena_b200_fftconv_fwd_windows(const float* u, const float* kspec, const float* Dvec, float* out,
+                                          const long long* seg_base, const int* row_start, const int* out_start,
+                                          long long total, int B, int H, int L, void* workspace, size_t workspace_bytes,
+                                          void* stream);
+
 /* ---- plain long convolution (the reference extension's own surface) ---------------------------
  * fftconv_fwd replaces csrc/fftconv/fftconv.cpp:53-132 for fp32, gelu=false, no dropout mask, no q/v,
  * head_dim=1:  out[b,h,:] = causal_conv(u[b,h,:], k[h,:]) + u[b,h,:] * Dvec[h]     (fftconv_ref,
