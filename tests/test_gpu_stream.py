@@ -50,6 +50,8 @@ def _ops():
 CASES = [(o, lm, L, D) for o in (2, 3) for lm in (61, 1026, 4099, 1 << 16)
          for L, D in ((lm + 1, 100), (3 * lm + 5, 100), ((1 << 20) + 1, 3), ((1 << 21) + 3, 1))]
 CASES += [(2, 1026, 1 << 20, 100), (3, 61, (1 << 20) + 1, 100), (2, 4099, (1 << 21) + 3, 3)]
+# one window of L_b = 2^15 (LOGM1 = 5, the first two-level transform) for both orders, and of 2^19 for the plain passes
+CASES += [(2, 4099, 20001, 100), (3, 4099, 20001, 100), (3, 1026, 300001, 3)]
 
 
 @pytest.mark.parametrize("order,l_max,L,D", CASES)
@@ -103,10 +105,10 @@ def test_stream_agrees_with_an_unbounded_decode_cache(order, l_max):
     PU.check(y, yd, f"stream vs decode o{order} l_max {l_max}", ref64=stream_truth(op, u, torch.float64))
 
 
-@pytest.mark.parametrize("order,L_b", [(2, 2048), (2, 8192), (2, 1 << 16), (3, 2048), (3, 8192), (3, 1 << 16)])
+@pytest.mark.parametrize("order,L_b", [(o, L_b) for o in (2, 3) for L_b in (2048, 8192, 1 << 15, 1 << 16, 1 << 19)])
 def test_window_route_matches_one_window_of_the_whole_row(order, L_b):
     """Windows of L_b positions against the default plan of a row that fits, one window of 2^20: the same outputs up to
-    rounding."""
+    rounding, and that window against the truth."""
     ops = _ops()
     op = _op(32, 1026, order, seed=17)
     L = (1 << 20) - 3
@@ -116,7 +118,58 @@ def test_window_route_matches_one_window_of_the_whole_row(order, L_b):
     with torch.no_grad():
         y = op._forward_stream(u, ops.stream_plan(L, 1026, order, 2, L_b=L_b))
         y1 = op._forward_stream(u, pl)
-    PU.check(y, y1, f"o{order} windows of {L_b} vs one window", ref64=stream_truth(op, u, torch.float64))
+    ref64 = stream_truth(op, u, torch.float64)
+    PU.check(y, y1, f"o{order} windows of {L_b} vs one window", ref64=ref64)
+    PU.check(y1, stream_truth(op, u, torch.float32), f"o{order} one window of 2^20", ref64=ref64)
+
+
+def _chunked_plan(L, l_max, order, B, L_b, chunk_positions, short=0):
+    """ops.stream_plan with small windows and chunks, so that several chunk edges fall inside the sequence; ``short``
+    positions less chunk context than the plan's rule (the same chunk outputs, each chunk starting later)."""
+    ops = _ops()
+    pl = ops.stream_plan(L, l_max, order, B, L_b=L_b, chunk_positions=chunk_positions)
+    assert len(pl.chunks) >= 3
+    if not short:
+        return pl
+    cc = pl.chunk_context - short
+    return ops.StreamPlan(pl.L, pl.l_max, pl.order, pl.B, pl.L_b, pl.context, cc,
+                          [(max(0, a - cc), a, e) for _, a, e in pl.chunks])
+
+
+@pytest.mark.parametrize("l_max,L,L_b,chunk_positions", [(61, 5000, 1024, 3000), (1026, 20001, 4096, 3 * 8192)])
+def test_stream_order_4_across_chunk_edges(l_max, L, L_b, chunk_positions):
+    """Order 4 (three windowed recurrences per chunk, chunk context 3 (l_max - 1) + 2) with chunks small enough that
+    several chunk edges fall inside the sequence, against the truth."""
+    op = _op(16, l_max, 4, seed=l_max)
+    u = _input(3, L, 16, seed=L)
+    with torch.no_grad():
+        y = op._forward_stream(u, _chunked_plan(L, l_max, 4, 3, L_b, chunk_positions))
+    PU.check(y, stream_truth(op, u, torch.float32), f"stream o4 l_max {l_max} L {L} chunked",
+             ref64=stream_truth(op, u, torch.float64))
+
+
+@pytest.mark.parametrize("order", [3, 4])
+def test_truth_rejects_a_chunk_one_position_short_of_context(order):
+    """The order >= 3 counterpart of test_stream_cpu.test_truth_rejects_a_plan_with_one_position_too_little_context: a
+    StreamPlan whose chunks carry one position less than (order - 1)(l_max - 1) + 2 of context fails the bar the plan's
+    own chunks pass.  The filter is random and does not decay, so its last tap, which the missing position reaches
+    through, is not negligible."""
+    l_max, L = 61, 5000
+    op = _op(8, l_max, order, seed=order)
+    k = torch.randn(8 * (order - 1), l_max, generator=torch.Generator(device=_dev()).manual_seed(5), device=_dev())
+    op.filter_fn.filter_channel_major = lambda n: k[:, :n] / 4
+    u = _input(2, L, 8, seed=order)
+    ref64, ref32 = stream_truth(op, u, torch.float64), stream_truth(op, u, torch.float32)
+    with torch.no_grad():
+        good = op._forward_stream(u, _chunked_plan(L, l_max, order, 2, 1024, 2000))
+        bad = op._forward_stream(u, _chunked_plan(L, l_max, order, 2, 1024, 2000, short=1))
+    n0 = len(PU._records)
+    try:
+        PU.check(good, ref32, f"o{order} chunk context exact", ref64=ref64)
+        with pytest.raises(AssertionError):
+            PU.check(bad, ref32, f"o{order} chunk context one short", ref64=ref64)
+    finally:
+        del PU._records[n0:]            # a self-check of the bar, not a parity record
 
 
 # ---------------------------------------------------------------------------------------------- Block and Backbone
